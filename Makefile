@@ -1,6 +1,6 @@
-# ehb200 — builds the CUDA library (sm_100a only) and the CPU oracle.
+# ehb200 — builds the CUDA library (sm_90a only) and the CPU oracle.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function --expt-relaxed-constexpr
 CSRC      := embeddinghub_b200/csrc
 OBJDIR    := build/obj

@@ -2,9 +2,10 @@
 """ehb200 benchmark — batched k-NN over the HNSW graph at the north-star configurations.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ehb200|reference] [--workload auto|c2|c3|...]
+                  [--dump-outputs DIR]
 
 Default workload ("auto"): ONE GPU -> BASELINE.json configs[2] (C3: N=10M d=768 Q=10k k=10 ef=128 InnerProduct,
-the north-star target, 30.7 GB of vectors on one B200); N > 1 GPUs -> configs[4] (C5: d=128 Q=10k k=100 ef=256
+the north-star target, 30.7 GB of vectors on one H100); N > 1 GPUs -> configs[4] (C5: d=128 Q=10k k=100 ef=256
 cosine, range-sharded, 12.5M points per GPU = 100M at 8 GPUs).  A step = one pass of the hot path over one
 batch of Q synthetic queries.
   value        queries/s over the WHOLE index (Q / step time), index and queries resident in HBM, device-timed
@@ -27,8 +28,14 @@ one push + flag + merge kernel per rank over NVLink, no collective; --exchange n
 kernel).  Weak scaling: the shard size per GPU is fixed, so the index grows with N; `value` stays Q / step
 time (queries answered over N_total points) and `shard_searches_per_s` = N x that is the aggregate of
 shard-level searches.
+
+--dump-outputs DIR writes what the last timed step returned to its caller (rank 0): labels.npy (float64; -1 for
+an empty slot), distances.npy (float32) and counts.npy (float32), one row per query; above 64 MB in all, a fixed,
+seeded sample of query rows, whose indices go to rows.npy.  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
+import atexit
 import ctypes as C
 import json
 import os
@@ -57,7 +64,7 @@ WORKLOADS = {
     "c5": dict(N=12_500_000, d=128, Q=10000, k=100, ef=256, metric="cosine",
                desc="HNSW N=100M d=128 Q=10k k=100 ef=256 cosine range-sharded over 8 GPUs = 12.5M per GPU "
                     "(BASELINE.json configs[4]; with fewer ranks the total shrinks accordingly)"),
-    # brute force on the bf16 tensor-core path (tcgen05 GEMM + fp32 re-rank); recall is measured against the
+    # brute force on the bf16 tensor-core path (wgmma GEMM + fp32 re-rank); recall is measured against the
     # exact fp32 path
     "c4s": dict(N=1_000_000, d=768, Q=4096, k=100, ef=0, metric="ip", brute="bf16",
                 desc="brute force N=1M d=768 Q=4096 k=100 bf16 tensor-core path (C4 shape at N=1M)"),
@@ -67,6 +74,7 @@ WORKLOADS = {
 BASE_SEED, QUERY_SEED = 1234, 4321  # SURVEY.md §8d
 CHUNK = 1 << 20                     # rows per generated chunk (SURVEY.md §8d: chunks of 1M rows)
 
+DUMP_BYTES, DUMP_SEED = 64 << 20, 7  # --dump-outputs: size cap, seed of the row sample above it
 DIST = "gaussian"   # --dist gmm: report-only secondary distribution (SURVEY.md §8d): 1024-centre GMM, sigma 0.3
 
 
@@ -118,6 +126,22 @@ def shared_config(wl, world):
             "k": wl["k"], "ef": wl["ef"], "metric_space": wl["metric"], "M": 16, "ef_construction": 200}
 
 
+def dump_outputs(out_dir, res):
+    """Writes one step's result arrays as float .npy files (see the module docstring)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"labels": res["l"].cpu().numpy().astype(np.float64),       # int64 labels; empty slots are -1
+              "distances": res["d"].cpu().numpy().astype(np.float32),
+              "counts": res["c"].cpu().numpy().astype(np.float32)}
+    nq = arrays["counts"].shape[0]
+    row_bytes = sum(a.nbytes for a in arrays.values()) // max(nq, 1)
+    if row_bytes * nq > DUMP_BYTES:    # a fixed, seeded sample of query rows, listed in rows.npy
+        rows = np.sort(np.random.default_rng(DUMP_SEED).choice(nq, (DUMP_BYTES - 4096) // (row_bytes + 8), replace=False))  # 4 KB: .npy headers
+        arrays = {name: a[rows] for name, a in arrays.items()}
+        arrays["rows"] = rows.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def recall_at_k(found, truth):
     k = truth.shape[1]
     return float(np.mean([len(set(a.tolist()) & set(b.tolist())) / k for a, b in zip(found, truth)]))
@@ -143,6 +167,7 @@ class ClockSampler:
                 self.p = subprocess.Popen(["nvidia-smi", f"--id={self.gpu}", f"--query-gpu={q}",
                                            "--format=csv,noheader,nounits", "-lms", "20"],
                                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+                atexit.register(self.p.kill)  # never outlive the benchmark, even when it fails mid-run
                 threading.Thread(target=self._read, daemon=True).start()
                 time.sleep(0.3)
                 return
@@ -277,8 +302,8 @@ def oracle_build_prefix(orc, wl, budget_s, cores, cap, tune=None):
 
 # ---------------------------------------------------------------------------------------------
 def run_reference(args, wl):
-    """The reference arm: the CPU oracle (hnswlib restatement; oracle/_ref cannot exist because the hnswlib
-    headers are not in /root/reference) with every host thread pinned, its own CPU-built graph."""
+    """The reference arm: the CPU oracle (hnswlib restatement; the reference cannot be built without the hnswlib
+    headers, which its tree does not contain) with every host thread pinned, its own CPU-built graph."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -424,7 +449,7 @@ def run_ehb(args, wl):
     torch.cuda.set_stream(stream)
     sptr = stream.cuda_stream
     dq = [torch.from_numpy(x).cuda() for x in qsets]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     from embeddinghub_b200.sharded import ShardedSearcher
 
     searcher = ShardedSearcher(ix, world, local, exchange=args.exchange)
@@ -467,6 +492,8 @@ def run_ehb(args, wl):
     st = counters[-1]
     kernel_name = ix.last_kernel_name()
     labels_dev = last["l"].cpu().numpy().view(np.uint64).copy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # the local shard alone (no exchange), same steps: lets a reader separate the walk from the exchange
     shard_ms = None
@@ -556,24 +583,16 @@ def run_ehb(args, wl):
     if peaks:
         peak, peak_src = peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "fallback (H100 SXM data sheet, HBM3)"
     k_ms = float(np.mean(kernel_ms))
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "walk_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        ent = tj.get(args.workload)
-        if isinstance(ent, dict):
-            traffic, traffic_src = ent.get("dram_bytes_per_launch"), ent.get("source")
-        elif ent is not None:
-            traffic = ent
+    traffic, traffic_src = None, None   # DRAM bytes of the kernel: not measured (no counter profiler)
     if brute:
-        tpeak = peaks.get("bf16_tflops_sustained", 1400.0)
+        tpeak = peaks.get("bf16_tflops_sustained", 989.0)
         flops = 2.0 * Q * N * d
         ach = flops / (k_ms * 1e-3) / 1e12
         roofline = {"bound": "tensor", "achieved": ach, "peak": tpeak, "unit": "TFLOP/s", "frac": ach / tpeak,
                     "traffic": traffic, "peak_source": "measured sustained cuBLAS bf16 (MEASURED_PEAKS.json)"
-                    if peaks else "fallback (B200_PROFILING.md)", "kernel": "bf16_topk_gemm_kernel (persistent tcgen05 "
+                    if peaks else "fallback (H100 SXM data sheet, dense bf16)", "kernel": "bf16_topk_gemm_kernel (persistent wgmma "
                     "GEMM, selection fused into the epilogue) + compaction + fp32 re-rank: the whole brute-force "
                     "pipeline is timed", "kernel_ms": k_ms, "flops_per_launch": flops}
     else:
@@ -670,7 +689,7 @@ def run_ehb(args, wl):
         "steps": steps, "warmup": warmup, "ms_per_step": dev_ms, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic" if DIST == "gaussian" else "synthetic (gmm)",
         "config": shared_config(wl, world),
-        "details": {"path": "bruteforce bf16 tcgen05 + fp32 re-rank" if brute else "graph walk",
+        "details": {"path": "bruteforce bf16 wgmma + fp32 re-rank" if brute else "graph walk",
                     "l2": "flushed between timed steps (256 MB write) and the index (vectors+links) is larger than L2",
                     "parallelism": f"range-sharded x{world}, one {searcher.exchange} exchange of per-shard top-k + merge"
                     if world > 1 else "single GPU", "exchange": searcher.exchange, "build_s": round(t_build, 2),
@@ -710,6 +729,8 @@ def main():
     ap.add_argument("--ref-max-points", type=int, default=1_000_000)
     ap.add_argument("--recall-queries", type=int, default=2000)
     ap.add_argument("--dist", default="gaussian", choices=["gaussian", "gmm"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's labels / distances / counts to DIR/*.npy")
     args = ap.parse_args()
     global DIST
     DIST = args.dist

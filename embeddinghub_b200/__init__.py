@@ -1,7 +1,7 @@
-"""embeddinghub_b200 — B200-native ANN search backend for embeddinghub.
+"""embeddinghub_b200 — H100-native ANN search backend for embeddinghub.
 
 Only the k-NN hot path of featureform/embeddinghub is implemented here (see
-DESIGN.md): a hand-written sm_100a CUDA library behind a C ABI
+DESIGN.md): a hand-written sm_90a CUDA library behind a C ABI
 (include/ehb200.h) plus the host-side mirrors of the reference's interfaces for
 that path.
 """

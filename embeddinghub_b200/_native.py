@@ -2,7 +2,7 @@
 
 There is no CPU fallback: importing works anywhere (so the ABI can be checked on
 a CPU-only box), but every compute call raises EhbError when the CUDA library is
-missing or no B200-class device is present.
+missing or no H100-class (sm_90) device is present.
 """
 import ctypes as C
 import os
@@ -125,7 +125,7 @@ def lib():
     global _LIB
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
-            raise EhbError(-1, f"{LIB_PATH} is missing: run `make` (nvcc, sm_100a). There is no CPU fallback.")
+            raise EhbError(-1, f"{LIB_PATH} is missing: run `make` (nvcc, sm_90a). There is no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(L, name)

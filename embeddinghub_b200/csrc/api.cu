@@ -65,8 +65,8 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
   // Visited table.  A hop admits at most 2M new ids and the walk makes about ef hops.  "roomy" keeps
   // the final load near 0.5 even on iid Gaussian data (~29 new ids per hop); but every KB of table
   // costs occupancy, and a crowded table only costs re-evaluations (probes are bounded; duplicates
-  // are filtered against the result set): measured at d=768/ef=128, a table HALF the visited count
-  // gave +1.3 % evaluations and 1.5x the throughput of the roomy one.  So: as roomy as the
+  // are filtered against the result set), so a table smaller than the visited count adds only a few
+  // re-evaluations while the occupancy it buys speeds up the memory-bound walk.  So: as roomy as the
   // occupancy target allows, never below a quarter of the worst case.
   const uint32_t roomy = 2u * M0 * ef_eff + 64u, tight = std::max(256u, M0 * ef_eff / 4u);
   uint32_t hs = roomy;
@@ -372,7 +372,7 @@ int ehb_index::build() {
       continue;
     }
     // a wave never exceeds 1/64 of the linked graph: points of one wave cannot see each other
-    // (measured: recall within sampling noise of the sequential build from 1/32 on)
+    // (recall stays within the seed-to-seed noise of the sequential build; tests/test_gpu_parity.py checks it)
     const uint64_t frac = o_build_frac ? o_build_frac : 64;
     uint64_t b = std::min<uint64_t>(maxb, std::max<uint64_t>(1, n_linked / frac));
     b = std::min<uint64_t>(b, n - n_linked);
@@ -485,8 +485,9 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   uint32_t ef_eff = std::max(ef_in ? ef_in : ef, k);
   if (ef_eff > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
   // Warps per query (rows <= 1 KB, ef <= 256): four while 3 CTAs of 128 threads per SM hold every query (small
-  // online batches; Q=1: 135 us vs 252 us with one warp), two while 7 CTAs of 64 threads do (C2, Q=1000:
-  // 0.288 ms vs 0.409 ms), else one warp per query (C5 shape, Q=10k: 9.2 ms vs 10.7 ms with two).
+  // online batches, where one warp's serial chain of memory round trips is the bound), two while 7 CTAs of 64
+  // threads do (C2, Q=1000), else one warp per query: once the batch alone fills the SMs, the team walk's
+  // speculative expansions only add work (C5 shape, Q=10k).
   uint32_t team = t_team;
   if (team == 0) team = nq <= (uint64_t)sms * 3 ? 4 : (nq <= (uint64_t)sms * 7 ? 2 : 1);
   if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
@@ -584,7 +585,6 @@ int ehb_index::bruteforce_dev(uint64_t nq, const float* dq, uint32_t k, int prec
     // fused selection state (option "bf16_unfused" keeps the distance tiles in HBM: A/B switch); tombstones
     // are filtered where keys are formed, which only the unfused selection does
     bctx.fused = !o_bf16_unfused && !n_deleted;
-    bctx.variant = o_gemm_2cta ? 1 : 0;
     bctx.ccap = 2 * kc + 64;
     CU(bf_thr.grow(nq, 0, -1, s));
     CU(bf_cbuf.grow(nq * bctx.ccap, 0, -1, s));
@@ -778,7 +778,8 @@ int ehb_index_create(const ehb_params* p, ehb_index** out) {
   CU(cudaSetDevice(p->device));
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, p->device));
-  if (prop.major < 10) return fail(EHB_ERR_CUDA, "ehb200 kernels are built for sm_100a only");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(EHB_ERR_CUDA, "ehb200 kernels are built for sm_90a (compute capability 9.0) only");
   ehb_index* ix = new (std::nothrow) ehb_index();
   if (!ix) return fail(EHB_ERR_OOM, "host allocation failed");
   ix->prm = *p;
@@ -1009,8 +1010,6 @@ int ehb_index_set_option(ehb_index* ix, const char* name, int64_t value) {
     ix->o_build_frac = (uint32_t)value;
   } else if (o == "bf16_unfused") {
     ix->o_bf16_unfused = value != 0;
-  } else if (o == "gemm_2cta") {
-    ix->o_gemm_2cta = value != 0;
   } else if (o == "walk_prefetch") {
     ix->o_walk_prefetch = value != 0;
   } else if (o == "combine") {

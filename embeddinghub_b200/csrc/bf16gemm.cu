@@ -1,17 +1,16 @@
-// K3 — brute-force distances as a bf16 tensor-core GEMM (tcgen05 + TMEM + TMA).
+// K3 — brute-force distances as a bf16 tensor-core GEMM (Hopper wgmma + TMA).
 //
 // The batched exact scan is a genuine dense contraction: D[q][n] = <Q[q], X[n]> over
-// d, Q x N x d multiply-adds (C4: 4096 x 10M x 768 = 3.1e13 MACs).  This kernel
-// computes 128 x 256 tiles of it on the 5th-generation tensor cores:
-//   warp 0  : TMA producer — cp.async.bulk.tensor.2d (SASS UTMALDG) of a 128 x 64 bf16
-//             query box and a 256 x 64 bf16 base box per k-block, 128B-swizzled, into a
-//             4-stage shared-memory ring, completion on mbarriers;
-//   warp 1  : MMA issuer — one elected thread issues tcgen05.mma.cta_group::1.kind::f16
-//             (SASS UTCHMMA), M=128 N=256 K=16, fp32 accumulators in TMEM (256 columns);
-//             tcgen05.commit releases the smem stage / signals the epilogue;
-//   warps 2-5: epilogue — tcgen05.ld (SASS LDTM) 32 lanes x 32 columns at a time, turn the
-//             dot products into distances (1 - dot, or |q|^2 + |x|^2 - 2 dot) and store
-//             the fp32 tile.
+// d, Q x N x d multiply-adds (C4: 4096 x 10M x 768 = 3.1e13 MACs).  These kernels
+// compute 128 x 256 tiles of it on the sm_90a warpgroup tensor cores:
+//   warpgroup 0   : TMA producer — one thread issues cp.async.bulk.tensor.2d of a 128 x 64 bf16
+//                   query box and a 256 x 64 bf16 base box per k-block, 128B-swizzled, into a
+//                   4-stage shared-memory ring (48 KB a stage), completion on mbarriers;
+//   warpgroups 1-2: consumers — each issues wgmma.mma_async m64n256k16 (bf16 in, fp32 out) for its
+//                   64 query rows of the tile straight from the swizzled stages, with the 64 x 256
+//                   fp32 accumulator in registers (128 a thread; setmaxnreg moves registers from the
+//                   producer), releases each stage once the wgmma that read it has retired, then turns
+//                   the dot products into distances (1 - dot, or |q|^2 + |x|^2 - 2 dot).
 // The candidate selection (top-k' per query over the tile rows), and the fp32
 // re-rank that restores exact ids, reuse the K1 select / merge kernels
 // (bruteforce.cu) and rerank_kernel below.
@@ -28,6 +27,7 @@
 namespace ehb {
 
 constexpr int GM = 128, GN = 256, GK = 64, GSTAGES = 4;
+constexpr int kGemmThreads = 384;  // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kStageBytesA = GM * GK * 2, kStageBytesB = GN * GK * 2;
 constexpr uint32_t kGemmSmem = GSTAGES * (kStageBytesA + kStageBytesB) + 1024 /*align*/ + 256 /*barriers*/;
 
@@ -38,446 +38,230 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_c), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+__device__ __forceinline__ void fence_acc(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, both operands K-major bf16 in shared memory, fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(1u));
+}
 
 // K-major, 128B-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row swizzle atoms of 1024 B):
-// start address >> 4, SBO = 1024 B >> 4, descriptor version 1 (sm_100), layout type SWIZZLE_128B (2).
+// start address >> 4, SBO = 1024 B >> 4, layout type SWIZZLE_128B (1 in the sm_90 encoding).
 __device__ __forceinline__ uint64_t make_smem_desc(const void* smem_tile) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_u32(smem_tile) & 0x3FFFFu) >> 4);  // bits [0,14)
-  d |= (uint64_t)0 << 16;                                   // leading byte offset: unused for swizzled K-major
+  d |= (uint64_t)1 << 16;                                   // leading byte offset: unused for swizzled K-major
   d |= (uint64_t)(1024u >> 4) << 32;                        // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                                   // version
-  d |= (uint64_t)2 << 61;                                   // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                                   // SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: D = F32, A = B = BF16, both K-major, N >> 3, M >> 4.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+
+// The operand ring shared by both GEMM kernels: full[s] completes on the TMA bytes, empty[s] on one arrival
+// from each consumer warpgroup.
+struct GemmRing {
+  unsigned char* sA;  // [stage][128 x 64] query rows
+  unsigned char* sB;  // [stage][256 x 64] base rows
+  uint64_t* full;
+  uint64_t* empty;
+};
+
+__device__ __forceinline__ GemmRing gemm_ring_setup(unsigned char* smem_raw, const CUtensorMap* mq,
+                                                    const CUtensorMap* mx) {
+  unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // 128B swizzle: 1 KB align
+  GemmRing r;
+  r.sA = smem;
+  r.sB = smem + GSTAGES * kStageBytesA;
+  r.full = (uint64_t*)(smem + GSTAGES * (kStageBytesA + kStageBytesB));
+  r.empty = r.full + GSTAGES;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < GSTAGES; ++s) mbar_init(&r.full[s], 1), mbar_init(&r.empty[s], 2);
+    fence_mbar_init();
+    asm volatile("prefetch.tensormap [%0];" ::"l"(mq) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(mx) : "memory");
+  }
+  __syncthreads();
+  return r;
 }
+
+// producer: the k-blocks of one (query rows qr, base rows nr) tile; `it` counts ring slots across tiles
+__device__ __forceinline__ void gemm_produce(const GemmRing& r, const CUtensorMap* mq, const CUtensorMap* mx,
+                                             uint32_t kblocks, int qr, int nr, uint32_t& it) {
+  for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
+    uint32_t s = it % GSTAGES, ph = (it / GSTAGES) & 1u;
+    mbar_wait(&r.empty[s], ph ^ 1u);  // first pass through the ring passes immediately
+    mbar_arrive_expect_tx(&r.full[s], kStageBytesA + kStageBytesB);
+    tma_load_2d(r.sA + s * kStageBytesA, mq, (int)(kb * GK), qr, &r.full[s]);
+    tma_load_2d(r.sB + s * kStageBytesB, mx, (int)(kb * GK), nr, &r.full[s]);
+  }
+}
+
+// consumer warpgroup wg (0, 1): acc = rows [64 wg, 64 wg + 64) of the 128 x 256 tile.  One wgmma group stays in
+// flight: the stage a k-block read is released once the next k-block's group has been issued and the older one
+// has retired.
+__device__ __forceinline__ void gemm_consume(const GemmRing& r, uint32_t kblocks, uint32_t wg, float (&acc)[128],
+                                             uint32_t& it) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  const bool signal = (threadIdx.x & 127u) == 0;
+  for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
+    uint32_t s = it % GSTAGES, ph = (it / GSTAGES) & 1u;
+    mbar_wait(&r.full[s], ph);
+    uint64_t da = make_smem_desc(r.sA + s * kStageBytesA + wg * (64u * GK * 2)), db = make_smem_desc(r.sB + s * kStageBytesB);
+    fence_acc(acc);
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t k4 = 0; k4 < GK / 16; ++k4)  // K = 16 bf16 = 32 B = +2 in the (>>4) start address
+      wgmma_m64n256k16(acc, da + 2 * k4, db + 2 * k4);
+    wgmma_commit();
+    wgmma_wait<1>();
+    fence_acc(acc);
+    if (kb > 0 && signal) mbar_arrive(&r.empty[(it - 1) % GSTAGES]);
+  }
+  wgmma_wait<0>();
+  fence_acc(acc);
+  if (kblocks > 0 && signal) mbar_arrive(&r.empty[(it - 1) % GSTAGES]);
+}
+
+// Accumulator fragment of thread (warp w, lane l) of a consumer warpgroup: acc[4 j + 2 h + e] holds row
+// 16 w + l / 4 + 8 h of the warpgroup's 64 rows, column 8 j + 2 (l % 4) + e of the tile's 256.
 
 // dist[(q - q0) * ldd + (n - n0)], q in [q0, q0 + qn), n in [n0, n0 + nn).
 // metric 0: qnorm[q] + xnorm[n] - 2 dot;  metric 1: 1 - dot.
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
     bf16_dist_gemm_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x,
                           uint32_t kblocks, int metric, const float* __restrict__ qnorm,
                           const float* __restrict__ xnorm, uint64_t q0, uint64_t qn, uint64_t n0, uint64_t nn,
                           float* __restrict__ dist, uint64_t ldd) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // 128B swizzle: 1 KB align
-  unsigned char* sA = smem;
-  unsigned char* sB = smem + GSTAGES * kStageBytesA;
-  uint64_t* full = (uint64_t*)(smem + GSTAGES * (kStageBytesA + kStageBytesB));
-  uint64_t* empty = full + GSTAGES;
-  uint64_t* tmem_full = empty + GSTAGES;
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_full + 1);
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const GemmRing r = gemm_ring_setup(smem_raw, &map_q, &map_x);
   // query tiles vary fastest: the CTAs that share one 256-row base tile run together, so the base set is
-  // read from HBM once per chunk (ncu, base-tile-fastest order: 3.2 GB read per launch for a 0.2 GB chunk)
+  // read from HBM about once per chunk
   const uint32_t tile_q = blockIdx.x, tile_n = blockIdx.y;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < GSTAGES; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], 1);
-    mbar_init(tmem_full, 1);
-    fence_mbar_init();
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+  const uint32_t wg = threadIdx.x >> 7;
+  uint32_t it = 0;
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0)
+      gemm_produce(r, &map_q, &map_x, kblocks, (int)(q0 + (uint64_t)tile_q * GM), (int)(n0 + (uint64_t)tile_n * GN), it);
+    return;
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, GN);  // 256 fp32 columns x 128 lanes
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (uint32_t kb = 0; kb < kblocks; ++kb) {
-        uint32_t s = kb % GSTAGES, ph = (kb / GSTAGES) & 1u;
-        mbar_wait(&empty[s], ph ^ 1u);  // first pass through the ring passes immediately
-        mbar_arrive_expect_tx(&full[s], kStageBytesA + kStageBytesB);
-        tma_load_2d(sA + s * kStageBytesA, &map_q, (int)(kb * GK), (int)(q0 + (uint64_t)tile_q * GM), &full[s]);
-        tma_load_2d(sB + s * kStageBytesB, &map_x, (int)(kb * GK), (int)(n0 + (uint64_t)tile_n * GN), &full[s]);
+  setmaxnreg_inc<232>();
+  float acc[128];
+  gemm_consume(r, kblocks, wg - 1, acc, it);
+  const uint32_t t = threadIdx.x & 127u, w = t >> 5, l = t & 31u;
+  const uint64_t row0 = (uint64_t)tile_q * GM + (wg - 1) * 64u + w * 16u + (l >> 2);  // relative to q0
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const uint64_t qrow = row0 + 8u * h;
+    if (qrow >= qn) continue;
+    const float qn2 = metric == 0 ? qnorm[q0 + qrow] : 0.f;
+    float* out = dist + qrow * ldd;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const uint64_t ncol = (uint64_t)tile_n * GN + 8u * j + 2u * (l & 3u);  // relative to n0
+      float v[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float dot = acc[4 * j + 2 * h + e];
+        float xn = (metric == 0 && ncol + e < nn) ? xnorm[n0 + ncol + e] : 0.f;
+        v[e] = metric == 0 ? fmaxf(qn2 + xn - 2.0f * dot, 0.f) : 1.0f - dot;
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(GM, GN);
-      for (uint32_t kb = 0; kb < kblocks; ++kb) {
-        uint32_t s = kb % GSTAGES, ph = (kb / GSTAGES) & 1u;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        uint64_t da = make_smem_desc(sA + s * kStageBytesA), db = make_smem_desc(sB + s * kStageBytesB);
-#pragma unroll
-        for (uint32_t k4 = 0; k4 < GK / 16; ++k4)  // UMMA_K = 16 bf16 = 32 B = +2 in the (>>4) start address
-          umma_bf16(tmem_base, da + 2 * k4, db + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-        umma_commit(&empty[s]);  // frees the smem stage once these MMAs have read it
-      }
-      umma_commit(tmem_full);    // accumulators complete
-    }
-  } else {
-    // epilogue warp w covers TMEM lanes [32 * (warp % 4), +32) = query rows of the tile
-    const uint32_t quarter = warp & 3u;
-    const uint64_t qrow = (uint64_t)tile_q * GM + quarter * 32u + lane;  // relative to q0
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const float qn2 = (metric == 0 && qrow < qn) ? qnorm[q0 + qrow] : 0.f;
-    for (uint32_t c0 = 0; c0 < GN; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((quarter * 32u) << 16) + c0, r);
-      uint64_t ncol = (uint64_t)tile_n * GN + c0;  // relative to n0
-      if (qrow < qn) {
-        float* out = dist + qrow * ldd + ncol;
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float dot = __uint_as_float(r[j]);
-          float xn = (metric == 0 && ncol + j < nn) ? xnorm[n0 + ncol + j] : 0.f;
-          v[j] = metric == 0 ? fmaxf(qn2 + xn - 2.0f * dot, 0.f) : 1.0f - dot;
-        }
-        if (ncol + 32 <= nn && (ldd & 3u) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) *(float4*)(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (ncol + j < nn) out[j] = v[j];
-        }
+      if (ncol + 2 <= nn && (ldd & 1u) == 0) {
+        *(float2*)(out + ncol) = make_float2(v[0], v[1]);
+      } else {
+        if (ncol < nn) out[ncol] = v[0];
+        if (ncol + 1 < nn) out[ncol + 1] = v[1];
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, GN);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // Persistent variant with the selection fused into the epilogue: the Q x N distance tile never goes to HBM.
 // One CTA per SM walks the (query tile, base tile) list (query tile fastest, so the CTAs that share a base
-// tile run together); accumulators are double-buffered in TMEM (2 x 256 columns), so the epilogue of tile i
-// overlaps the MMAs of tile i+1.  The epilogue compares every distance with the query's current threshold
-// thr[q] (its kc-th best bf16 distance so far) and appends the survivors (ordered distance | row index) to
-// the query's candidate buffer with one global atomic each; compact_candidates_kernel folds the buffer into
-// the running top-kc and tightens thr between chunks.  With chunk sizes that double, a chunk admits about kc
-// candidates per query, so the buffer (capacity 2 kc + 64) practically never overflows; if it does the
-// driver re-runs that chunk through the unfused path.
+// tile run together); the producer runs up to four k-blocks ahead, so the loads of tile i+1 overlap the
+// epilogue of tile i.  The epilogue compares every distance with the query's current threshold thr[q] (its
+// kc-th best bf16 distance so far) and appends the survivors (ordered distance | row index) to the query's
+// candidate buffer with one global atomic each; compact_candidates_kernel folds the buffer into the running
+// top-kc and tightens thr between chunks.  With chunk sizes that double, a chunk admits about kc candidates
+// per query, so the buffer (capacity 2 kc + 64) practically never overflows; if it does the driver re-runs
+// that chunk through the unfused path.
 // ---------------------------------------------------------------------------------------------------
-constexpr uint32_t kFusedSmem = GSTAGES * (kStageBytesA + kStageBytesB) + 1024 + 256;
 static cudaError_t make_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t dpad, uint32_t box_rows);
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
     bf16_topk_gemm_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x,
                           uint32_t kblocks, int metric, const float* __restrict__ qnorm,
                           const float* __restrict__ xnorm, uint64_t nq, uint64_t n_lo, uint64_t n_hi,
                           const float* __restrict__ thr, uint64_t* __restrict__ cbuf, uint32_t* __restrict__ ccount,
                           uint32_t ccap) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* sA = smem;
-  unsigned char* sB = smem + GSTAGES * kStageBytesA;
-  uint64_t* full = (uint64_t*)(smem + GSTAGES * (kStageBytesA + kStageBytesB));
-  uint64_t* empty = full + GSTAGES;
-  uint64_t* tmem_full = empty + GSTAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;    // [2]
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 2);
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const GemmRing r = gemm_ring_setup(smem_raw, &map_q, &map_x);
   const uint64_t q_tiles = (nq + GM - 1) / GM, n_tiles = (n_hi - n_lo + GN - 1) / GN;
   const uint64_t tiles = q_tiles * n_tiles;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < GSTAGES; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], 1);
-    for (int a = 0; a < 2; ++a) mbar_init(&tmem_full[a], 1), mbar_init(&tmem_empty[a], 4);
-    fence_mbar_init();
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+  const uint32_t wg = threadIdx.x >> 7;
+  uint32_t it = 0;
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0)
+      for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x)
+        gemm_produce(r, &map_q, &map_x, kblocks, (int)((t % q_tiles) * GM), (int)(n_lo + (t / q_tiles) * GN), it);
+    return;
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, 2 * GN);  // 512 columns: two accumulator stages
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
-        const uint64_t tq = t % q_tiles, tn = t / q_tiles;
-        for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
-          uint32_t s = it % GSTAGES, ph = (it / GSTAGES) & 1u;
-          mbar_wait(&empty[s], ph ^ 1u);
-          mbar_arrive_expect_tx(&full[s], kStageBytesA + kStageBytesB);
-          tma_load_2d(sA + s * kStageBytesA, &map_q, (int)(kb * GK), (int)(tq * GM), &full[s]);
-          tma_load_2d(sB + s * kStageBytesB, &map_x, (int)(kb * GK), (int)(n_lo + tn * GN), &full[s]);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(GM, GN);
-      uint32_t it = 0, ti = 0;
-      for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x, ++ti) {
-        const uint32_t acc = ti & 1u, aph = (ti >> 1) & 1u;
-        mbar_wait(&tmem_empty[acc], aph ^ 1u);  // epilogue has drained this accumulator stage
-        tc_fence_after();
-        for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
-          uint32_t s = it % GSTAGES, ph = (it / GSTAGES) & 1u;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          uint64_t da = make_smem_desc(sA + s * kStageBytesA), db = make_smem_desc(sB + s * kStageBytesB);
+  setmaxnreg_inc<232>();
+  const uint32_t t_ = threadIdx.x & 127u, w = t_ >> 5, l = t_ & 31u;
+  float acc[128];
+  for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const uint64_t tq = t % q_tiles, tn = t / q_tiles;
+    gemm_consume(r, kblocks, wg - 1, acc, it);
+    uint64_t q[2];
+    float tau[2], qn2[2];
 #pragma unroll
-          for (uint32_t k4 = 0; k4 < GK / 16; ++k4)
-            umma_bf16(tmem_base + acc * GN, da + 2 * k4, db + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        umma_commit(&tmem_full[acc]);
-      }
+    for (int h = 0; h < 2; ++h) {
+      q[h] = tq * GM + (wg - 1) * 64u + w * 16u + (l >> 2) + 8u * h;
+      const bool qok = q[h] < nq;
+      tau[h] = qok ? thr[q[h]] : -INFINITY;
+      qn2[h] = (metric == 0 && qok) ? qnorm[q[h]] : 0.f;
     }
-  } else {
-    const uint32_t quarter = warp & 3u;
-    uint32_t ti = 0;
-    for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x, ++ti) {
-      const uint64_t tq = t % q_tiles, tn = t / q_tiles;
-      const uint32_t acc = ti & 1u, aph = (ti >> 1) & 1u;
-      const uint64_t q = tq * GM + quarter * 32u + lane;
-      const bool qok = q < nq;
-      const float tau = qok ? thr[q] : -INFINITY;
-      const float qn2 = (metric == 0 && qok) ? qnorm[q] : 0.f;
-      mbar_wait(&tmem_full[acc], aph);
-      tc_fence_after();
-      for (uint32_t c0 = 0; c0 < GN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + acc * GN + ((quarter * 32u) << 16) + c0, r);
-        const uint64_t nbase = n_lo + tn * GN + c0;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float dot = __uint_as_float(r[j]);
-          float d;
-          if (metric == 0) {
-            float xn = nbase + j < n_hi ? xnorm[nbase + j] : 0.f;
-            d = fmaxf(qn2 + xn - 2.0f * dot, 0.f);
-          } else {
-            d = 1.0f - dot;
-          }
-          if (d < tau && nbase + j < n_hi) {
-            uint32_t pos = atomicAdd(&ccount[q], 1u);
-            if (pos < ccap) cbuf[q * ccap + pos] = make_key(d, (uint32_t)(nbase + j));
+    for (int j = 0; j < 32; ++j) {
+      const uint64_t nb = n_lo + tn * GN + 8u * j + 2u * (l & 3u);
+      float xn[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) xn[e] = (metric == 0 && nb + e < n_hi) ? xnorm[nb + e] : 0.f;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float dot = acc[4 * j + 2 * h + e];
+          float d = metric == 0 ? fmaxf(qn2[h] + xn[e] - 2.0f * dot, 0.f) : 1.0f - dot;
+          if (d < tau[h] && nb + e < n_hi) {
+            uint32_t pos = atomicAdd(&ccount[q[h]], 1u);
+            if (pos < ccap) cbuf[q[h] * ccap + pos] = make_key(d, (uint32_t)(nb + e));
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 2 * GN);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// 2-CTA form of the fused kernel (cta_group::2): a cluster of two SMs owns a 256 x 256 tile.  Each CTA
-// stages its own 128 query rows and HALF of the base tile (128 rows) per k-block — 32 KB instead of 48 KB for
-// the same tensor-pipe time — so the six-stage ring covers the L2 -> SM latency that bounds the 1-CTA kernel.
-// The leader CTA's MMA thread issues tcgen05.mma.cta_group::2 (M = 256); both CTAs' TMA loads complete on the
-// leader's `full` barrier; tcgen05.commit multicasts the `empty` / `tmem_full` arrivals to both CTAs; the
-// non-leader's epilogue warps release the accumulator stage on the leader's `tmem_empty` barrier remotely.
-// Opt-in (ehb_index_set_option "gemm_2cta"): measured on C4-shaped chunks it reaches 765 TFLOP/s in-kernel vs 826 TFLOP/s
-// for the 1-CTA kernel — both sit on the L2 -> SM operand traffic (92 resp. 61 B/clk/SM requested against
-// a chip-wide LTS cap of ~6.3 KB/clk), so the next step is TMA multicast across a larger cluster, not this.
-// ---------------------------------------------------------------------------------------------------
-constexpr int G2STAGES = 6;
-constexpr uint32_t kStage2 = (GM * GK * 2) + (128 * GK * 2);  // A 128x64 + B-half 128x64 bf16 = 32 KB
-constexpr uint32_t kFused2Smem = G2STAGES * kStage2 + 1024 + 256;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  // both CTAs execute this; clearing the peer bit makes the transaction bytes land on CTA 0's barrier
-  uint32_t mbar = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(mbar), "r"(c0), "r"(c1), "l"(0x1000000000000000ull)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_c), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cta(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-
-__global__ void __launch_bounds__(192, 1)
-    bf16_topk_gemm2_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x,
-                           uint32_t kblocks, int metric, const float* __restrict__ qnorm,
-                           const float* __restrict__ xnorm, uint64_t nq, uint64_t n_lo, uint64_t n_hi,
-                           const float* __restrict__ thr, uint64_t* __restrict__ cbuf, uint32_t* __restrict__ ccount,
-                           uint32_t ccap) {
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* sA = smem;                                   // [stage][128 x 64]
-  unsigned char* sB = smem + G2STAGES * (GM * GK * 2);        // [stage][128 x 64] (this CTA's half of the base tile)
-  uint64_t* full = (uint64_t*)(smem + G2STAGES * kStage2);
-  uint64_t* empty = full + G2STAGES;
-  uint64_t* tmem_full = empty + G2STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;     // [2] (used in the leader)
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 2);
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const uint32_t cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-  const uint64_t q_tiles = (nq + 2 * GM - 1) / (2 * GM), n_tiles = (n_hi - n_lo + GN - 1) / GN;
-  const uint64_t tiles = q_tiles * n_tiles;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < G2STAGES; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], 1);
-    for (int a = 0; a < 2; ++a) mbar_init(&tmem_full[a], 1), mbar_init(&tmem_empty[a], 8);
-    fence_mbar_init();
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)),
-                 "r"(2u * GN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (uint64_t t = cluster_id; t < tiles; t += n_clusters) {
-        const uint64_t tq = t % q_tiles, tn = t / q_tiles;
-        for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
-          uint32_t s = it % G2STAGES, ph = (it / G2STAGES) & 1u;
-          mbar_wait(&empty[s], ph ^ 1u);
-          if (rank == 0) mbar_arrive_expect_tx(&full[s], 2u * kStage2);  // both CTAs' bytes land here
-          tma_load_2d_2sm(sA + s * (GM * GK * 2), &map_q, (int)(kb * GK), (int)(tq * 2 * GM + rank * GM), &full[s]);
-          tma_load_2d_2sm(sB + s * (128 * GK * 2), &map_x, (int)(kb * GK), (int)(n_lo + tn * GN + rank * 128),
-                          &full[s]);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (rank == 0 && lane == 0) {
-      constexpr uint32_t idesc = make_idesc(2 * GM, GN);
-      uint32_t it = 0, ti = 0;
-      for (uint64_t t = cluster_id; t < tiles; t += n_clusters, ++ti) {
-        const uint32_t acc = ti & 1u, aph = (ti >> 1) & 1u;
-        mbar_wait(&tmem_empty[acc], aph ^ 1u);
-        tc_fence_after();
-        for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
-          uint32_t s = it % G2STAGES, ph = (it / G2STAGES) & 1u;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          uint64_t da = make_smem_desc(sA + s * (GM * GK * 2)), db = make_smem_desc(sB + s * (128 * GK * 2));
-#pragma unroll
-          for (uint32_t k4 = 0; k4 < GK / 16; ++k4)
-            umma_bf16_2sm(tmem_base + acc * GN, da + 2 * k4, db + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-          umma_commit_2sm(&empty[s]);
-        }
-        umma_commit_2sm(&tmem_full[acc]);
-      }
-    }
-  } else {
-    const uint32_t quarter = warp & 3u;
-    uint32_t ti = 0;
-    for (uint64_t t = cluster_id; t < tiles; t += n_clusters, ++ti) {
-      const uint64_t tq = t % q_tiles, tn = t / q_tiles;
-      const uint32_t acc = ti & 1u, aph = (ti >> 1) & 1u;
-      const uint64_t q = tq * 2 * GM + rank * GM + quarter * 32u + lane;
-      const bool qok = q < nq;
-      const float tau = qok ? thr[q] : -INFINITY;
-      const float qn2 = (metric == 0 && qok) ? qnorm[q] : 0.f;
-      mbar_wait(&tmem_full[acc], aph);
-      tc_fence_after();
-      for (uint32_t c0 = 0; c0 < GN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + acc * GN + ((quarter * 32u) << 16) + c0, r);
-        const uint64_t nbase = n_lo + tn * GN + c0;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float dot = __uint_as_float(r[j]);
-          float d;
-          if (metric == 0) {
-            float xn = nbase + j < n_hi ? xnorm[nbase + j] : 0.f;
-            d = fmaxf(qn2 + xn - 2.0f * dot, 0.f);
-          } else {
-            d = 1.0f - dot;
-          }
-          if (d < tau && nbase + j < n_hi) {
-            uint32_t pos = atomicAdd(&ccount[q], 1u);
-            if (pos < ccap) cbuf[q * ccap + pos] = make_key(d, (uint32_t)(nbase + j));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cta(&tmem_empty[acc], 0);  // the leader's MMA thread owns the accumulator hand-off
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2u * GN) : "memory");
 }
 
 // One warp per query: fold the candidate buffer into the running top-kc, publish the new threshold, reset
@@ -527,43 +311,19 @@ __global__ void compact_candidates_kernel(uint64_t* __restrict__ run_keys, uint6
 cudaError_t launch_bf16_topk_chunk(const void* q_bf16, uint64_t nq, const void* x_bf16, uint64_t x_rows, uint32_t dpad,
                                    int metric, const float* qnorm, const float* xnorm, uint64_t n_lo, uint64_t n_hi,
                                    float* thr, uint64_t* cbuf, uint32_t* ccount, uint32_t ccap, uint64_t* run_keys,
-                                   uint32_t kc, uint32_t* overflow, int sms, int variant, cudaStream_t s) {
+                                   uint32_t kc, uint32_t* overflow, int sms, cudaStream_t s) {
   if (dpad % GK != 0) return cudaErrorInvalidValue;
   CUtensorMap mq, mx;
   cudaError_t e;
   if ((e = make_map(&mq, q_bf16, nq, dpad, GM)) != cudaSuccess) return e;
   if ((e = make_map(&mx, x_bf16, x_rows, dpad, GN)) != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(bf16_topk_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmem);
+  e = cudaFuncSetAttribute(bf16_topk_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmem);
   if (e != cudaSuccess) return e;
   if (n_hi > n_lo) {
-    const bool two_cta = variant == 1;
-    if (two_cta) {
-      if ((e = make_map(&mx, x_bf16, x_rows, dpad, 128)) != cudaSuccess) return e;  // each CTA stages half a base tile
-      e = cudaFuncSetAttribute(bf16_topk_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFused2Smem);
-      if (e != cudaSuccess) return e;
-      uint64_t tiles = ((nq + 2 * GM - 1) / (2 * GM)) * ((n_hi - n_lo + GN - 1) / GN);
-      unsigned clusters = (unsigned)(tiles < (uint64_t)(sms / 2) ? tiles : (uint64_t)(sms / 2));
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(clusters * 2);
-      cfg.blockDim = dim3(192);
-      cfg.dynamicSmemBytes = kFused2Smem;
-      cfg.stream = s;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = 2;
-      at[0].val.clusterDim.y = 1;
-      at[0].val.clusterDim.z = 1;
-      cfg.attrs = at;
-      cfg.numAttrs = 1;
-      e = cudaLaunchKernelEx(&cfg, bf16_topk_gemm2_kernel, mq, mx, dpad / GK, metric == 0 ? 0 : 1, qnorm, xnorm,
-                             (uint64_t)nq, n_lo, n_hi, (const float*)thr, cbuf, ccount, ccap);
-      if (e != cudaSuccess) return e;
-    } else {
-      uint64_t tiles = ((nq + GM - 1) / GM) * ((n_hi - n_lo + GN - 1) / GN);
-      unsigned grid = (unsigned)(tiles < (uint64_t)sms ? tiles : (uint64_t)sms);
-      bf16_topk_gemm_kernel<<<grid, 192, kFusedSmem, s>>>(mq, mx, dpad / GK, metric == 0 ? 0 : 1, qnorm, xnorm, nq,
-                                                        n_lo, n_hi, thr, cbuf, ccount, ccap);
-    }
+    uint64_t tiles = ((nq + GM - 1) / GM) * ((n_hi - n_lo + GN - 1) / GN);
+    unsigned grid = (unsigned)(tiles < (uint64_t)sms ? tiles : (uint64_t)sms);
+    bf16_topk_gemm_kernel<<<grid, kGemmThreads, kGemmSmem, s>>>(mq, mx, dpad / GK, metric == 0 ? 0 : 1, qnorm, xnorm,
+                                                                nq, n_lo, n_hi, thr, cbuf, ccount, ccap);
   }
   // fold the survivors into the running top-kc
   uint32_t P = 64;
@@ -640,7 +400,7 @@ cudaError_t launch_bf16_dist_tile(const void* q_bf16, uint64_t q_rows, const voi
   e = cudaFuncSetAttribute(bf16_dist_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmem);
   if (e != cudaSuccess) return e;
   dim3 grid((unsigned)((qn + GM - 1) / GM), (unsigned)((nn + GN - 1) / GN));
-  bf16_dist_gemm_kernel<<<grid, 192, kGemmSmem, s>>>(mq, mx, dpad / GK, metric == 0 ? 0 : 1, qnorm, xnorm, q0, qn, n0,
+  bf16_dist_gemm_kernel<<<grid, kGemmThreads, kGemmSmem, s>>>(mq, mx, dpad / GK, metric == 0 ? 0 : 1, qnorm, xnorm, q0, qn, n0,
                                                     nn, dist, ldd);
   return cudaGetLastError();
 }

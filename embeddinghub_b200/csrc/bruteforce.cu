@@ -243,14 +243,14 @@ cudaError_t launch_bruteforce(const float* vecs, uint32_t dpad, uint32_t dim, ui
     if ((e = unfused_range(0, s0)) != cudaSuccess) return e;
     // compaction with empty buffers publishes thr[q] from the bootstrap lists
     e = launch_bf16_topk_chunk(bf->q_bf16, nq, bf->x_bf16, n, dpad, metric, bf->qnorm, bf->xnorm, 0, 0, bf->thr,
-                               bf->cbuf, bf->ccount, bf->ccap, sc.run_keys, ksel, bf->overflow, bf->sms, bf->variant, s);
+                               bf->cbuf, bf->ccount, bf->ccap, sc.run_keys, ksel, bf->overflow, bf->sms, s);
     if (e != cudaSuccess) return e;
     uint64_t seen = s0;
     while (seen < n) {
       uint64_t chunk = n - seen < seen ? n - seen : seen;
       e = launch_bf16_topk_chunk(bf->q_bf16, nq, bf->x_bf16, n, dpad, metric, bf->qnorm, bf->xnorm, seen,
                                  seen + chunk, bf->thr, bf->cbuf, bf->ccount, bf->ccap, sc.run_keys, ksel,
-                                 bf->overflow, bf->sms, bf->variant, s);
+                                 bf->overflow, bf->sms, s);
       if (e != cudaSuccess) return e;
       uint32_t ovf = 0;
       if ((e = cudaMemcpyAsync(&ovf, bf->overflow, 4, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
@@ -259,7 +259,7 @@ cudaError_t launch_bruteforce(const float* vecs, uint32_t dpad, uint32_t dim, ui
         if ((e = cudaMemsetAsync(bf->overflow, 0, 4, s)) != cudaSuccess) return e;
         if ((e = unfused_range(seen, seen + chunk)) != cudaSuccess) return e;
         e = launch_bf16_topk_chunk(bf->q_bf16, nq, bf->x_bf16, n, dpad, metric, bf->qnorm, bf->xnorm, 0, 0, bf->thr,
-                                   bf->cbuf, bf->ccount, bf->ccap, sc.run_keys, ksel, bf->overflow, bf->sms, bf->variant, s);
+                                   bf->cbuf, bf->ccount, bf->ccap, sc.run_keys, ksel, bf->overflow, bf->sms, s);
         if (e != cudaSuccess) return e;
       }
       seen += chunk;

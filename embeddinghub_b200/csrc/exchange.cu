@@ -113,7 +113,7 @@ struct ehb_exchange {
   uint32_t epoch = 0;
   uint64_t slot_nq = 0;
   uint32_t slot_k = 0;
-  int sms = 148;
+  int sms = 132;
   std::mutex mu;
 };
 

@@ -197,7 +197,7 @@ struct ehb_index {
   uint32_t dim, dpad, M, M0;
   int metric;
   int device;
-  int sms = 148;
+  int sms = 132;
   cudaStream_t stream = nullptr;  // mutation / construction / brute-force stream
   cudaEvent_t bf_ev0 = nullptr, bf_ev1 = nullptr;
   ehb::RwLock rw;
@@ -262,11 +262,9 @@ struct ehb_index {
   // options (ehb_index_set_option)
   uint32_t o_build_frac = 0;     // a wave links at most n_linked / build_frac points (0 = 64)
   bool o_bf16_unfused = false;   // bf16 brute force: keep the distance tiles in HBM (A/B)
-  bool o_gemm_2cta = false;      // bf16 brute force: cta_group::2 cluster form of the fused GEMM
   bool o_combine = true;         // coalesce concurrent small host searches
-  // L2 prefetch of the speculated next hop's vectors (rows <= 1 KB).  Off: on the full C5 shard ncu showed 52.7 GB
-  // of DRAM traffic for 41.4 GB algorithmic (already-visited neighbours and wrong guesses are fetched too) and
-  // the walk is 5.9 % faster without it (10.43 -> 9.82 ms); r1 had measured no gain at C2 either.
+  // L2 prefetch of the speculated next hop's vectors (rows <= 1 KB).  Off: already-visited neighbours and wrong
+  // guesses are fetched too, which adds DRAM traffic to a walk that is bound by DRAM traffic.
   bool o_walk_prefetch = false;
 
   std::default_random_engine level_rng;

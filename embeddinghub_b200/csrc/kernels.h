@@ -43,7 +43,7 @@ cudaError_t launch_bruteforce_exact(const float* vecs, uint32_t dpad, uint32_t d
                                     BruteScratch& sc, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
                                     cudaStream_t s);
 
-// K3 — bf16 tensor-core (tcgen05) distance tiles + fp32 re-rank.
+// K3 — bf16 tensor-core (wgmma) distance tiles + fp32 re-rank.
 struct Bf16Ctx {
   const void* q_bf16;   // [nq][dpad] bf16
   const void* x_bf16;   // [n][dpad] bf16
@@ -58,12 +58,11 @@ struct Bf16Ctx {
   uint32_t* overflow;   // device flag
   int sms;
   bool fused;
-  int variant;          // 0 = 1-CTA persistent kernel, 1 = cta_group::2 cluster form
 };
 cudaError_t launch_bf16_topk_chunk(const void* q_bf16, uint64_t nq, const void* x_bf16, uint64_t x_rows, uint32_t dpad,
                                    int metric, const float* qnorm, const float* xnorm, uint64_t n_lo, uint64_t n_hi,
                                    float* thr, uint64_t* cbuf, uint32_t* ccount, uint32_t ccap, uint64_t* run_keys,
-                                   uint32_t kc, uint32_t* overflow, int sms, int variant, cudaStream_t s);
+                                   uint32_t kc, uint32_t* overflow, int sms, cudaStream_t s);
 cudaError_t launch_to_bf16(const float* in, uint32_t in_stride, void* out_bf16, float* norms, uint64_t n, uint32_t dpad,
                            cudaStream_t s);
 cudaError_t launch_bf16_dist_tile(const void* q_bf16, uint64_t q_rows, const void* x_bf16, uint64_t x_rows,

@@ -79,9 +79,9 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   }
 }
 
-// Register budget of the default form: ptxas chooses (128 registers for d = 128 / ef = 256, 16 vectors in
-// flight per warp).  An explicit minBlocksPerSM changes its heuristics — even "1" gives 143 registers, and
-// capping this body at 128 serialised the load batches: 9.1 -> 22.7 ms on the C5 shape — so none is given.
+// Register budget of the default form: ptxas chooses (16 vectors in flight per warp).  An explicit
+// minBlocksPerSM changes its heuristics, and a register cap below what the 16 loads in flight need serialises
+// the load batches — so none is given.
 template <int LPV, int NQ, int KPL, bool HASDEL>
 __global__ void __launch_bounds__(128) hnsw_search_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries,
                                                           uint32_t nq, uint32_t k, uint32_t ef,
@@ -93,8 +93,7 @@ __global__ void __launch_bounds__(128) hnsw_search_kernel(GraphView g, WalkCfg c
 
 // "Dense" form for big batches of short rows (LPV = 8, d <= 128): 8 vectors in flight per warp instead of 16
 // and a 96-register budget -> 20 resident warps per SM instead of 16 (the visited table shrinks to match,
-// api.cu walk_cfg).  Measured on the C5 shape (N = 1M, Q = 10k, ef = 256): 8.66 ms vs 9.08 ms; with the
-// same 8-vector batches but 16 warps: 9.48 ms (profiles/r02_ab_walk_occupancy.txt).
+// api.cu walk_cfg): with many queries in flight, more warps hide more of each hop's memory latency.
 template <int LPV, int NQ, int KPL>
 __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, WalkCfg cfg,
                                                                    const float* __restrict__ queries, uint32_t nq,
@@ -127,8 +126,8 @@ template <int LPV, int NQ>
 cudaError_t launch_search_kpl(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t wpb,
                               cudaStream_t s) {
-  // (Keeping a whole 2M-neighbour hop in flight per batch (~168 registers) was measured on C2:
-  //  0.446 ms vs 0.423 ms — no gain, so batches stay at 16 vectors.)
+  // (Keeping a whole 2M-neighbour hop in flight per batch needs about 168 registers, which costs occupancy;
+  //  batches stay at 16 vectors.)
 #define EHB_KPL(K)                                                                                          \
   return g.deleted ? launch_search_t<LPV, NQ, K, true>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s) \
                    : launch_search_t<LPV, NQ, K, false>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s)

@@ -1,7 +1,7 @@
 // K2t — team variant of the graph walk: T warps (one CTA) per query.
 //
 // When a batch has fewer queries than the machine has warp slots (C2: 1000
-// queries on 148 SMs = 6.8 warps per SM) the warp-per-query walk is bound by one
+// queries on 132 SMs = 7.6 warps per SM) the warp-per-query walk is bound by one
 // warp's serial chain of memory round trips.  Here the T warps of a CTA expand
 // the T closest unexpanded entries of the result set concurrently:
 //   * every warp keeps an identical replica of the unordered result set (ulist)

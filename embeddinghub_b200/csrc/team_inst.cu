@@ -20,8 +20,8 @@ static cudaError_t team_t(uint32_t T, const GraphView& g, uint32_t hash_size, co
   constexpr int U2 = NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2);   // T = 2: 64
   constexpr int U4 = NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1);   // T = 3, 4: 32
   // T = 4 with the full 16-vector batches when the batch is so small that registers are no constraint
-  // (<= 3 CTAs of 128 threads per SM at ~125 registers)
-  if (T >= 4 && nq <= 148u * 3u)
+  // (<= 3 CTAs of 128 threads per SM of the H100's 132 at ~125 registers)
+  if (T >= 4 && nq <= 132u * 3u)
     return team_kpl<NQ, 4, U2>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
   if (T >= 4) return team_kpl<NQ, 4, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
   if (T == 3) return team_kpl<NQ, 3, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);

@@ -2,7 +2,7 @@
 //
 // Replaces hnswlib's searchKnn / searchBaseLayerST / searchBaseLayer hot loops
 // (called from embeddinghub/embeddingstore/index.cc:36,41) with a design that
-// fits the B200 memory system:
+// fits the H100 memory system:
 //   * one warp owns one query (or one point being inserted);
 //   * an adjacency row is one 128 B line (2M = 32 u32, padded with kInvalid);
 //   * hnswlib's ef-bounded result heap and its candidate heap are ONE unordered
@@ -17,9 +17,8 @@
 //         memory (cp.async.bulk, one bulk copy per vector, completion counted
 //         on an mbarrier) in a ring of groups, and the math on group r overlaps
 //         the copies of the following groups.
-//     (v1 staged every row through TMA; ncu showed the walk issue-bound with
-//      17 % of all issued instructions in the per-lane UBLKCP serialisation
-//      loops at d=128, see profiles/r01_walk_v1_summary.md.)
+//     (Staging every row through TMA makes the walk issue-bound on the
+//      per-lane bulk-copy issue loops at d=128.)
 //   * rows are padded to an exact multiple of the per-lane tile, so the inner
 //     loops carry no bounds checks.
 #pragma once
@@ -350,9 +349,8 @@ __device__ __forceinline__ uint32_t ul_worst(const UList<KPL>& u) {
 // Insert (hi, id) [warp-uniform]; cnt/worst_hi are maintained by the caller's copies.
 // Precondition when cnt == ef: hi < worst_hi.
 // (Round 2 tried a per-lane form — every lane reduces over its own KPL slots, then ONE ballot elects the
-//  lane, predicated writes select the slot — to cut the ~KPL dependent ballots per insert.  Measured on a
-//  B200 it lost everywhere: C5 shape 22.8 ms vs 9.0 ms (KPL = 8, 136 vs 128 registers), C3 shape 20.9 vs
-//  19.6 ms, C2 0.299 vs 0.293 ms; profiles/r02_ab_ulist.txt.  The slot-walking form below stays.)
+//  lane, predicated writes select the slot — to cut the ~KPL dependent ballots per insert.  It needs more
+//  registers than the slot-walking form below (136 vs 128 at KPL = 8), which costs the walk its occupancy.)
 template <int KPL>
 __device__ __forceinline__ void ul_insert(UList<KPL>& u, uint32_t hi, uint32_t id, uint32_t ef, uint32_t& cnt,
                                           uint32_t& worst_hi, uint32_t lane) {
@@ -588,7 +586,7 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 }
 
 // HASDEL = false compiles every trace of the tombstone machinery out (an index without tombstones runs
-// exactly the round-1 loop: the extra live registers cost the 16-vector load batches their overlap).
+// exactly the plain loop: the extra live registers would cost the 16-vector load batches their overlap).
 template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,

@@ -1,4 +1,4 @@
-/* ehb200 — C ABI of the B200-native ANN backend for embeddinghub.
+/* ehb200 — C ABI of the H100-native ANN backend for embeddinghub.
  *
  * This is the drop-in boundary (SURVEY.md §8b, B4): everything the reference's
  * hnswlib-backed ANNIndex does for the k-NN hot path, as plain C entry points a
@@ -23,7 +23,7 @@
  *     exclusive.  The reference serialises everything under one service mutex
  *     (embeddinghub/embeddingstore/server.cc:175).
  *   - there is no CPU fallback: every call fails with EHB_ERR_CUDA when no
- *     sm_100-class device is usable.
+ *     sm_90 (H100-class) device is usable.
  */
 #ifndef EHB200_H
 #define EHB200_H
@@ -254,9 +254,11 @@ int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a pe
  * the reference's surface).  Unknown names fail with EHB_ERR_INVALID.
  *   "build_frac"    a construction wave links at most size/build_frac points (0 = default 64)
  *   "bf16_unfused"  bf16 brute force keeps the distance tiles in HBM (A/B of the fused epilogue)
- *   "gemm_2cta"     bf16 brute force uses the cta_group::2 cluster form of the GEMM
  *   "combine"       1 (default): concurrent host searches of <= 256 queries share batched launches
- *   "walk_prefetch" 1: L2-prefetch the speculated next hop's vectors (default 0: it cost 27 % extra DRAM traffic) */
+ *   "walk_prefetch" 1: L2-prefetch the speculated next hop's vectors (default 0: it also fetches rows the walk
+ *                   never evaluates, extra DRAM traffic for a DRAM-bound walk)
+ * ABI change with the sm_90a build: "gemm_2cta" (a two-SM cta_group::2 form of the bf16 GEMM that only
+ * Blackwell has) is no longer accepted and fails with EHB_ERR_INVALID like any unknown name. */
 int ehb_index_set_option(ehb_index* ix, const char* name, int64_t value);
 
 #ifdef __cplusplus

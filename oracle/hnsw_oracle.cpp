@@ -6,7 +6,7 @@
 //   github.com/nmslib/hnswlib @ 21b54fe9544cfbb757b2ea8f3def5542ba2435c7
 //   (embeddinghub/WORKSPACE:80-85; Python side hnswlib==0.5.2,
 //    embeddinghub/sdk/python/requirements.txt:1)
-// which is NOT vendored in /root/reference and cannot be fetched here, so this
+// which is NOT vendored in the reference tree, so this
 // file restates its published algorithm (Malkov & Yashunin, "Efficient and
 // robust approximate nearest neighbor search using HNSW graphs", and the
 // upstream hnswalg.h / space_l2.h / space_ip.h / bruteforce.h behaviour as

@@ -1,7 +1,7 @@
 // Known-answer cases of the reference's ANNIndex unit test
 // (embeddinghub/embeddingstore/test/index_test.cc:17-60: TestSimpleANN, TestMultiANN,
 // TestUpdateANN, TestANN0Items), table-driven and without gtest, run against the drop-in
-// twin in include/ehb200_ann_index.hpp on a B200 (tests/test_gpu_host.py).
+// twin in include/ehb200_ann_index.hpp on the GPU (tests/test_gpu_host.py).
 #include <cstdio>
 #include <string>
 #include <utility>

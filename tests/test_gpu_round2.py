@@ -1,4 +1,4 @@
-"""GPU parity tests (B200) of the round-2 surface: north-star shapes at scale, tombstones, faithful
+"""GPU parity tests of the round-2 surface: north-star shapes at scale, tombstones, faithful
 updatePoint, re-entrant / combined host searches, streaming persistence, the sharded index and the
 peer-memory shard exchange.  Everything calls through the C ABI; the oracle is the checker."""
 import ctypes as C
