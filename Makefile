@@ -8,7 +8,13 @@ SRCS      := $(wildcard $(CSRC)/*.cu)
 OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(SRCS))
 LIB       := embeddinghub_b200/libehb200.so
 
-all: $(LIB) oracle tests/cpp/ann_index_cases tests/cpp/concurrent_search tests/cpp/sharded_two_dev tests/cpp/rwlock_stress
+all: $(LIB) oracle tests/cpp/ann_index_cases tests/cpp/concurrent_search tests/cpp/sharded_two_dev tests/cpp/rwlock_stress \
+     tests/cpp/libbf16_probe.so
+
+# test-only extern "C" wrappers around the K3 launchers of the shipped library (run by tests/test_gpu_bf16_gemm.py)
+tests/cpp/libbf16_probe.so: tests/cpp/bf16_probe.cu $(CSRC)/kernels.h $(LIB)
+	$(NVCC) $(ARCH) -O2 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC,-Wall -shared -I$(CSRC) $< \
+	  -Lembeddinghub_b200 -lehb200 -Xlinker -rpath,'$$ORIGIN/../../embeddinghub_b200' -o $@
 
 # the reference's ANNIndex unit-test cases against the C++ drop-in twin (run by tests/test_gpu_host.py)
 tests/cpp/ann_index_cases: tests/cpp/ann_index_cases.cc include/ehb200_ann_index.hpp $(LIB)
