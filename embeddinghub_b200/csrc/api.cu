@@ -524,11 +524,12 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     const uint32_t kpl = ef_eff <= 64 ? 2 : (ef_eff <= 128 ? 4 : (ef_eff <= 256 ? 8 : 16));
     const uint32_t lpv = dpad > 256 ? 32 : 8;
     if (team >= 2)
-      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "hnsw_search_team_kernel<NQ=%u,KPL=%u,T=%u>",
-                    dpad / (4 * lpv), kpl, team);
-    else
-      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "%s<LPV=%u,NQ=%u,KPL=%u>",
-                    cfg.dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", lpv, dpad / (4 * lpv), kpl);
+      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "hnsw_search_team_kernel<NQ=%u,KPL=%u,T=%u,U=%u>",
+                    dpad / (4 * lpv), kpl, team, ehb::team_eval_steps(team, dpad, (uint32_t)nq));
+    else  // (HASDEL is named only when set, so the common instantiations keep their short names)
+      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "%s<LPV=%u,NQ=%u,KPL=%u%s>",
+                    cfg.dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", lpv, dpad / (4 * lpv), kpl,
+                    n_deleted ? ",HASDEL=1" : "");
   }
   {
     std::lock_guard<std::mutex> g(last_mu);

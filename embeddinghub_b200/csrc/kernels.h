@@ -17,10 +17,12 @@ cudaError_t launch_search(const GraphView& g, const WalkCfg& cfg, const float* q
                           uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                           uint32_t warps_per_block, cudaStream_t s);
 
-// K2t — team walk (T warps per query, T in {2,4}); rows <= 1 KB and ef <= 256 only.
+// K2t — team walk (T warps per query, T in {2,3,4}); rows <= 1 KB and ef <= 256 only.
 cudaError_t launch_search_team(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,
                                uint32_t k, uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
                                uint32_t* stats, cudaStream_t s);
+// the U (4-vector load steps in flight) that launch_search_team instantiates for this shape
+uint32_t team_eval_steps(uint32_t T, uint32_t dpad, uint32_t nq);
 
 // row-wise L2 normalisation (hnswlib cosine convention), canonical arithmetic.
 cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, uint32_t out_stride, uint64_t n,

@@ -3,6 +3,20 @@
 
 namespace ehb {
 
+// Vector-load steps (4 vectors each) a team warp keeps in flight: the U template argument of K2t.  Registers of
+// loads in flight per lane are sized so that 7 CTAs fit an SM (T = 2: 64, T = 3 and 4: 32), except that T = 4
+// keeps the full 16-vector batches when the batch is so small that registers are no constraint (<= 3 CTAs of 128
+// threads per SM of the H100's 132 at ~125 registers).
+constexpr uint32_t kTeamWideMaxQueries = 132u * 3u;
+__host__ __device__ constexpr int team_u_wide(int NQ) { return NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2); }
+__host__ __device__ constexpr int team_u_narrow(int NQ) { return NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1); }
+static bool team_wide(uint32_t T, uint32_t nq) { return T == 2 || (T >= 4 && nq <= kTeamWideMaxQueries); }
+
+uint32_t team_eval_steps(uint32_t T, uint32_t dpad, uint32_t nq) {
+  const int NQ = (int)(dpad / 32u);
+  return (uint32_t)(team_wide(T, nq) ? team_u_wide(NQ) : team_u_narrow(NQ));
+}
+
 template <int NQ, int T, int U>
 static cudaError_t team_kpl(const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq, uint32_t k,
                             uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
@@ -16,12 +30,8 @@ template <int NQ>
 static cudaError_t team_t(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,
                           uint32_t k, uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
                           uint32_t* stats, cudaStream_t s) {
-  // registers of vector loads in flight per lane are sized so that 7 CTAs fit an SM:
-  constexpr int U2 = NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2);   // T = 2: 64
-  constexpr int U4 = NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1);   // T = 3, 4: 32
-  // T = 4 with the full 16-vector batches when the batch is so small that registers are no constraint
-  // (<= 3 CTAs of 128 threads per SM of the H100's 132 at ~125 registers)
-  if (T >= 4 && nq <= 132u * 3u)
+  constexpr int U2 = team_u_wide(NQ), U4 = team_u_narrow(NQ);
+  if (T >= 4 && team_wide(T, nq))
     return team_kpl<NQ, 4, U2>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
   if (T >= 4) return team_kpl<NQ, 4, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
   if (T == 3) return team_kpl<NQ, 3, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);

@@ -558,7 +558,10 @@ __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, c
 // searchBaseLayerST<has_deletions=true> puts a tombstoned node into candidate_set (it is traversed) but never
 // into top_candidates (it is not a result and does not move lowerBound).  Such nodes cannot live in the
 // result set, so they wait here, unordered, until they are the closest unexpanded candidate.
-__device__ __forceinline__ void dq_push(WarpCtx& c, uint32_t& dn, uint32_t hi, uint32_t id, uint32_t& overflow) {
+// bound: the worst result once the result set is full, else 0xFFFFFFFF.  An entry beyond it can never be expanded
+// (the set stays full and its worst only shrinks: the walk stops before reaching it), so dropping one is exact.
+__device__ __forceinline__ void dq_push(WarpCtx& c, uint32_t& dn, uint32_t hi, uint32_t id, uint32_t bound,
+                                        uint32_t& overflow) {
   if (dn < c.dcap) {
     if (c.lane == 0) c.dq_hi[dn] = hi, c.dq_id[dn] = id;
     dn++;
@@ -570,7 +573,7 @@ __device__ __forceinline__ void dq_push(WarpCtx& c, uint32_t& dn, uint32_t hi, u
     uint32_t b = __ballot_sync(0xffffffffu, w == wm);
     uint32_t pos = __shfl_sync(0xffffffffu, wp, __ffs(b) - 1);
     if (hi < wm && c.lane == 0) c.dq_hi[pos] = hi, c.dq_id[pos] = id;
-    overflow = 1;
+    if (max(hi, wm) <= bound) overflow = 1;  // the dropped entry could still have been expanded
   }
   __syncwarp();
 }
@@ -657,7 +660,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
         if (HASDEL && ((delmask >> j) & 1u)) {  // admitted like any candidate, but queued instead of becoming a result
           // (a tombstone whose visited status is only a guess is dropped: nothing else would keep it from
           //  being queued and expanded again and again once the visited table is full)
-          if (!((unsure >> j) & 1u)) dq_push(c, dn, hj, ij, ovf);
+          if (!((unsure >> j) & 1u)) dq_push(c, dn, hj, ij, cnt >= ef ? worst_hi : 0xFFFFFFFFu, ovf);
           continue;
         }
         if (ovf_any && ul_contains<KPL>(u, ij)) continue;
@@ -684,7 +687,9 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
     if (node == kInvalid) break;
     nb = (node == spec) ? spec_row : load_row(g, node, level, c.lane);
   }
-  wc.overflow |= ovf_any ? 1u : 0u;
+  // ovf_any is folded before a hop's candidates are admitted; a side-queue overflow raised while admitting them
+  // (dq_push) in the walk's last hop is only in ovf
+  wc.overflow |= (ovf_any || __any_sync(0xffffffffu, ovf)) ? 1u : 0u;
 }
 
 }  // namespace ehb
