@@ -75,6 +75,7 @@ SYMBOLS = {
     "ehb_index_add_dev": (C.c_int, [_VP, _U64, _VP, _VP]),
     "ehb_index_build": (C.c_int, [_VP]),
     "ehb_index_remove": (C.c_int, [_VP, _U64, _VP]),
+    "ehb_index_compact": (C.c_int, [_VP]),
     "ehb_index_set_ef": (C.c_int, [_VP, _U32]),
     "ehb_index_size": (C.c_int, [_VP, C.POINTER(_U64)]),
     "ehb_index_get": (C.c_int, [_VP, _U64, _VP]),
@@ -103,6 +104,7 @@ SYMBOLS = {
     "ehb_sharded_get": (C.c_int, [_VP, _U64, _VP]),
     "ehb_sharded_size": (C.c_int, [_VP, C.POINTER(_U64)]),
     "ehb_sharded_build": (C.c_int, [_VP]),
+    "ehb_sharded_compact": (C.c_int, [_VP]),
     "ehb_sharded_set_ef": (C.c_int, [_VP, _U32]),
     "ehb_sharded_search": (C.c_int, [_VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP]),
     "ehb_sharded_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
@@ -204,6 +206,11 @@ class NativeIndex:
         if rc == 5:
             raise KeyError(labels)
         check(rc)
+
+    def compact(self):
+        """Drops every tombstone and repairs the graph on the GPU: size() counts the survivors, labels and vectors
+        are kept, internal ids change, capacity is kept (ehb_index_compact)."""
+        check(lib().ehb_index_compact(self._h))
 
     def set_ef(self, ef):
         check(lib().ehb_index_set_ef(self._h, int(ef)))
@@ -367,6 +374,9 @@ class ShardedIndex:
 
     def build(self):
         check(lib().ehb_sharded_build(self._h))
+
+    def compact(self):
+        check(lib().ehb_sharded_compact(self._h))
 
     def get(self, label):
         out = np.empty(self.dim, np.float32)

@@ -69,6 +69,15 @@ class ANNIndex:
             self._nn.remove(np.array([self._key_to_label[k] for k in keys], np.uint64))
             self._deleted.update(keys)
 
+    def compact(self):
+        """Removes the deleted keys for good (ehb_index_compact): the graph is repaired on the GPU and the index
+        searches at full speed again.  len, keys, `in`, get and approx_nearest answer as before; a deleted key
+        that is set again later gets a fresh label."""
+        self._nn.compact()
+        for k in self._deleted:
+            del self._label_to_key[self._key_to_label.pop(k)]
+        self._deleted.clear()
+
     def delete_all(self):
         self.multidelete([k for k in self._key_to_label if k not in self._deleted])
 
@@ -104,7 +113,7 @@ class ANNIndex:
         return [k for k in self._key_to_label if k not in self._deleted]
 
     def __len__(self):
-        return self._next_label - len(self._deleted)
+        return len(self._key_to_label) - len(self._deleted)
 
     def __contains__(self, key):
         return key in self._key_to_label and key not in self._deleted

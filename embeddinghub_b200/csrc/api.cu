@@ -143,7 +143,7 @@ bool ehb_index::find_id(uint64_t label, uint32_t* id) const {
 }
 
 void ehb_index::reset_content() {
-  n = n_linked = up_rows = n_deleted = 0;
+  n = n_linked = up_rows = n_deleted = n_removed = 0;
   entry = 0;
   max_level = -1;
   lookup.clear();
@@ -171,7 +171,7 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
     bool contiguous_new = true;
     uint64_t nn = n;
     for (uint64_t i = 0; i < m; ++i) {
-      const uint64_t l = lab ? lab[off + i] : nn;
+      const uint64_t l = lab ? lab[off + i] : nn + n_removed;  // labels removed by compact() are not reused
       bool exists = false;
       uint32_t id = 0;
       if (identity_labels) {
@@ -338,6 +338,7 @@ ehb::BuildBuffers ehb_index::build_buffers(uint64_t edges) {
   bb.seg_dist = b_seg_dist.p;
   bb.error_flag = b_counters.p + 3;
   bb.upd_cand = b_upd_cand.p;
+  bb.repair_out = nullptr;
   return bb;
 }
 
@@ -380,7 +381,8 @@ int ehb_index::build() {
     RET(ensure_build_scratch(edges, 1, false));
     ehb::BuildGraph bg = build_graph();
     ehb::BuildBuffers bb = build_buffers(edges);
-    CU(ehb::launch_build_batch(bg, cfg, nullptr, (uint32_t)n_linked, (uint32_t)b, false, bb, wpb, stream));
+    CU(ehb::launch_build_batch(bg, cfg, nullptr, (uint32_t)n_linked, (uint32_t)b, ehb::kBuildInsert, bb, wpb,
+                               stream));
     for (uint64_t i = n_linked; i < n_linked + b; ++i)
       if ((int)h_levels[i] > max_level) max_level = h_levels[i], entry = (uint32_t)i;
     n_linked += b;
@@ -413,7 +415,7 @@ int ehb_index::build() {
         CU(cudaMemcpyAsync(b_ids.p, ups.data() + off, (size_t)b * 4, cudaMemcpyHostToDevice, stream));
         ehb::BuildGraph bg = build_graph();
         ehb::BuildBuffers bb = build_buffers(edges);
-        CU(ehb::launch_build_batch(bg, cfg, b_ids.p, 0, b, true, bb, wpb, stream));
+        CU(ehb::launch_build_batch(bg, cfg, b_ids.p, 0, b, ehb::kBuildUpdate, bb, wpb, stream));
       }
       CU(cudaStreamSynchronize(stream));
     }
@@ -424,6 +426,146 @@ int ehb_index::build() {
   CU(cudaStreamSynchronize(stream));
   if (err) return fail(EHB_ERR_STATE, "build: edge buffer overflow");
   return EHB_OK;
+}
+
+// ---- compaction -------------------------------------------------------------------------------------------
+// Removes every tombstone.  All passes read the pre-compaction graph, so the result does not depend on
+// scheduling:
+//   1. rows of live nodes that name deleted ids are found (and level-0 in-degrees counted);
+//   2. each such row is re-selected over its live ids and the live ids of its deleted members' rows
+//      (repair_rows_kernel), into a side buffer that is copied back once every repair has read the old graph;
+//   3. the entry point stays if it is live, else the live node of highest level (smallest id) takes over;
+//   4. survivors are renumbered densely in insertion order (new id = live ids below the old id): adjacency is
+//      gathered into new arrays, vectors are moved down in place through a bounded staging buffer;
+//   5. survivors left with an empty level-0 row, or with level-0 in-links before and none after, are
+//      re-linked by the updatePoint path (ascending new id);
+//   6. host tables follow.  Capacity is kept; later adds reuse the freed rows.
+int ehb_index::compact() {
+  RET(build());
+  if (n_deleted == 0) return EHB_OK;
+  cudaStream_t s = stream;
+  const uint64_t n_old = n;
+  std::vector<uint32_t> remap(n_old, ehb::kInvalid), inv;
+  inv.reserve(n_old - n_deleted);
+  for (uint64_t i = 0; i < n_old; ++i)
+    if (!h_deleted[i]) remap[i] = (uint32_t)inv.size(), inv.push_back((uint32_t)i);
+  const uint64_t nn = inv.size();
+  if (nn == 0) {  // everything deleted: an empty index, later adds start a fresh graph
+    const uint64_t removed = n_removed + n_old;
+    CU(cudaMemsetAsync(links0.p, 0xFF, links0.bytes(), s));
+    CU(cudaMemsetAsync(up_off.p, 0xFF, up_off.bytes(), s));
+    CU(cudaMemsetAsync(deleted.p, 0, deleted.bytes(), s));
+    CU(cudaMemsetAsync(links_up.p, 0xFF, links_up.bytes(), s));
+    CU(cudaStreamSynchronize(s));
+    reset_content();
+    n_removed = removed;
+    return EHB_OK;
+  }
+  // host side of the renumbering: old upper rows are laid out consecutively in id order
+  std::vector<uint64_t> labels_new(nn);
+  std::vector<uint8_t> levels_new(nn);
+  std::vector<uint32_t> up_off_new(nn), owner_new, src_up;
+  {
+    std::vector<uint32_t> up_off_old(n_old);
+    uint32_t r = 0;
+    for (uint64_t i = 0; i < n_old; ++i) up_off_old[i] = r, r += h_levels[i];
+    for (uint64_t i = 0; i < nn; ++i) {
+      const uint32_t o = inv[i];
+      labels_new[i] = h_labels[o];
+      levels_new[i] = h_levels[o];
+      up_off_new[i] = h_levels[o] ? (uint32_t)owner_new.size() : ehb::kInvalid;
+      for (uint32_t l = 0; l < h_levels[o]; ++l) owner_new.push_back((uint32_t)i), src_up.push_back(up_off_old[o] + l);
+    }
+  }
+  const uint64_t rows_new = owner_new.size();
+  uint32_t entry_new;
+  int32_t max_level_new = max_level;
+  if (!h_deleted[entry]) {
+    entry_new = remap[entry];
+  } else {
+    entry_new = 0;
+    for (uint64_t i = 1; i < nn; ++i)
+      if (levels_new[i] > levels_new[entry_new]) entry_new = (uint32_t)i;
+    max_level_new = levels_new[entry_new];
+  }
+  // 1. affected rows + level-0 in-degrees of the old graph
+  ehb::DevBuf<uint32_t> rows, indeg_old, indeg_new, d_remap, d_inv, d_src_up, repaired, nl0, nlu;
+  ehb::DevBuf<uint8_t> orphan;
+  ehb::DevBuf<float> stage;
+  CU(rows.grow(n_old + up_rows, 0, -1, s));
+  CU(indeg_old.grow(n_old, 0, 0, s));
+  CU(b_counters.grow(8, 0, 0, s));
+  CU(cudaMemsetAsync(b_counters.p + 5, 0, 4, s));
+  CU(ehb::launch_compact_mark(links0.p, links_up.p, up_owner.p, deleted.p, n_old, up_rows, M0, M, (uint32_t)cap,
+                              rows.p, b_counters.p + 5, indeg_old.p, s));
+  uint32_t nrows = 0;
+  CU(cudaMemcpyAsync(&nrows, b_counters.p + 5, 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  // every allocation before the graph changes, so running out of memory leaves the index as it was
+  const uint64_t stage_rows = std::max<uint64_t>(1, std::min<uint64_t>(nn, (256ull << 20) / (dpad * 4ull)));
+  const uint32_t warps = std::min<uint32_t>(std::max<uint32_t>(nrows, 1), ehb::kRepairWarps);
+  RET(ensure_build_scratch(0, warps, true));
+  CU(repaired.grow(std::max<uint64_t>(nrows, 1) * M0, 0, -1, s));
+  CU(d_remap.grow(n_old, 0, -1, s));
+  CU(d_inv.grow(nn, 0, -1, s));
+  CU(d_src_up.grow(std::max<uint64_t>(rows_new, 1), 0, -1, s));
+  CU(indeg_new.grow(nn, 0, -1, s));
+  CU(orphan.grow(nn, 0, -1, s));
+  CU(nl0.grow(cap * M0, 0, 0xFF, s));
+  CU(nlu.grow(links_up.n, 0, 0xFF, s));
+  CU(stage.grow(stage_rows * dpad, 0, -1, s));
+  // 2. repair, then copy the rows back
+  if (nrows) {
+    ehb::BuildGraph bg = build_graph();
+    ehb::BuildBuffers bb = build_buffers(0);
+    bb.repair_out = repaired.p;
+    const ehb::WalkCfg cfg = walk_cfg(bg.efc, 256, warps, 1);
+    CU(ehb::launch_build_batch(bg, cfg, rows.p, 0, nrows, ehb::kBuildRepair, bb, wpb_for(cfg, 256), s));
+    CU(ehb::launch_compact_apply(rows.p, nrows, repaired.p, links0.p, links_up.p, M0, M, (uint32_t)cap, s));
+  }
+  // 4. renumber the adjacency into the new arrays, find the orphans, move the vectors
+  CU(cudaMemcpyAsync(d_remap.p, remap.data(), n_old * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(d_inv.p, inv.data(), nn * 4, cudaMemcpyHostToDevice, s));
+  if (rows_new) CU(cudaMemcpyAsync(d_src_up.p, src_up.data(), rows_new * 4, cudaMemcpyHostToDevice, s));
+  CU(ehb::launch_compact_remap_rows(links0.p, d_inv.p, nn, M0, d_remap.p, nl0.p, s));
+  CU(ehb::launch_compact_remap_rows(links_up.p, d_src_up.p, rows_new, M, d_remap.p, nlu.p, s));
+  CU(ehb::launch_compact_orphans(nl0.p, nn, M0, d_inv.p, indeg_old.p, indeg_new.p, orphan.p, s));
+  uint64_t lo = 0;
+  while (lo < nn && inv[lo] == lo) ++lo;  // rows below the first tombstone stay where they are
+  CU(ehb::launch_compact_move_rows(vecs.p, dpad, d_inv.p, lo, nn, stage.p, stage_rows, s));
+  CU(cudaMemcpyAsync(labels.p, labels_new.data(), nn * 8, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(levels.p, levels_new.data(), nn, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(up_off.p, up_off_new.data(), nn * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemsetAsync(up_off.p + nn, 0xFF, (cap - nn) * 4, s));
+  if (rows_new) CU(cudaMemcpyAsync(up_owner.p, owner_new.data(), rows_new * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemsetAsync(deleted.p, 0, deleted.bytes(), s));
+  std::vector<uint8_t> is_orphan(nn);
+  CU(cudaMemcpyAsync(is_orphan.data(), orphan.p, nn, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  std::swap(links0.p, nl0.p);
+  std::swap(links_up.p, nlu.p);
+  // 6. host tables
+  identity_labels = true;
+  for (uint64_t i = 0; i < nn && identity_labels; ++i) identity_labels = labels_new[i] == i;
+  lookup.clear();
+  if (!identity_labels) {
+    lookup.reserve(nn * 2);
+    for (uint64_t i = 0; i < nn; ++i) lookup[labels_new[i]] = (uint32_t)i;
+  }
+  h_labels = std::move(labels_new);
+  h_levels = std::move(levels_new);
+  h_deleted.assign(nn, 0);
+  n_removed += n_old - nn;
+  n = n_linked = nn;
+  up_rows = rows_new;
+  n_deleted = 0;
+  entry = entry_new;
+  max_level = max_level_new;
+  bf16_rows = 0;
+  // 5. re-link the orphans (updatePoint: a beam search from the entry point, then mutual links)
+  for (uint64_t i = 0; i < nn; ++i)
+    if (is_orphan[i]) pending_updates.push_back((uint32_t)i);
+  return build();
 }
 
 // Searches link pending points lazily; that needs the writer side of the lock.
@@ -836,6 +978,12 @@ int ehb_index_remove(ehb_index* ix, uint64_t n, const uint64_t* labels) {
 int ehb_index_build(ehb_index* ix) {
   ENTER_X(ix);
   RET(ix->build());
+  CU(cudaStreamSynchronize(ix->stream));
+  return EHB_OK;
+}
+int ehb_index_compact(ehb_index* ix) {
+  ENTER_X(ix);
+  RET(ix->compact());
   CU(cudaStreamSynchronize(ix->stream));
   return EHB_OK;
 }

@@ -142,14 +142,75 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
   }
 }
 
+// Adds one id per lane (kInvalid = none; the ids of one call are distinct) to the candidate set cand[0..ncand),
+// deduplicated through the visited table.  A probe-budget overflow falls back to a linear scan of what is
+// stored, so the set is exact.
+__device__ __forceinline__ void cand_add(WarpCtx& c, uint32_t* cand, uint32_t& ncand, uint32_t id) {
+  uint32_t o = 0;
+  bool is_new = id != kInvalid && hash_insert(c, id, o);
+  __syncwarp();
+  if (__any_sync(0xffffffffu, o != 0)) {
+    if (o)
+      for (uint32_t i = 0; i < ncand && is_new; ++i) is_new = cand[i] != id;
+    __syncwarp();
+  }
+  const uint32_t mask = __ballot_sync(0xffffffffu, is_new);
+  if (is_new) cand[ncand + __popc(mask & lanemask_lt())] = id;
+  ncand += __popc(mask);
+  __syncwarp();
+}
+
+// The keep-then-select step of hnswlib updatePoint for one row: the `keep` members of cand[0..ncand) closest
+// to `owner` (owner itself skipped), ordered by (distance, id), then the heuristic with Mmax.  The selected
+// ids are left in a.sel_id; returns their number.
+template <int LPV, int NQ, int KPL>
+__device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g, const Aux& a, const uint32_t* cand,
+                                                 uint32_t ncand, uint32_t owner, uint32_t keep, uint32_t Mmax) {
+  float4 qr[NQ];
+  load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)owner * g.dpad, c.lane);
+  UList<KPL> u;
+  ul_clear<KPL>(u, keep, c.lane);
+  uint32_t cnt = 0, worst_hi = 0xFFFFFFFFu;
+  for (uint32_t b0 = 0; b0 < ncand; b0 += 32) {
+    uint32_t id = b0 + c.lane < ncand ? cand[b0 + c.lane] : kInvalid;
+    if (id == owner) id = kInvalid;
+    uint32_t mask = __ballot_sync(0xffffffffu, id != kInvalid);
+    uint32_t m = __popc(mask);
+    if (!m) continue;
+    if (id != kInvalid) c.cand_id[__popc(mask & lanemask_lt())] = id;
+    __syncwarp();
+    eval_candidates<LPV, NQ>(c, g.vecs, qr, m, g.metric);
+    uint32_t myhi = 0xFFFFFFFFu, myid = kInvalid;
+    if (c.lane < m) myhi = f2ord(c.cand_dist[c.lane]), myid = c.cand_id[c.lane];
+    __syncwarp();
+    uint32_t qual = __ballot_sync(0xffffffffu, c.lane < m && (cnt < keep || myhi < worst_hi));
+    while (qual) {
+      int l = __ffs(qual) - 1;
+      qual &= qual - 1;
+      uint32_t hj = __shfl_sync(0xffffffffu, myhi, l);
+      uint32_t ij = __shfl_sync(0xffffffffu, myid, l);
+      if (cnt >= keep && hj >= worst_hi) continue;
+      ul_insert<KPL>(u, hj, ij, keep, cnt, worst_hi, c.lane);
+    }
+  }
+  c.cnt = 0;
+  for (;;) {
+    uint64_t key = ul_extract_min<KPL>(u, c.lane);
+    if (key == kMaxKey) break;
+    if (c.lane == 0) c.keys[c.cnt] = key;
+    c.cnt++;
+  }
+  __syncwarp();
+  return heuristic_select<LPV, NQ>(c, g, Mmax, a);
+}
+
 // hnswlib updatePoint, first half (the part before repairConnectionsForUpdate): when the vector of an
 // already linked point p changes, every one-hop neighbour nb of p (per layer) gets its adjacency row
 // re-selected by the heuristic over the closest ef_construction members of
 //   sCand = {p} U one-hop(p) U two-hop(p)   (minus nb itself),
 // distances measured from nb.  One warp per updated point; sCand (<= 1 + 2M + 2M*2M ids) is gathered
-// into `upd_cand` with the visited table deduplicating (a probe-budget overflow falls back to a linear
-// scan, so the set is exact).  Rows are written under a per-row spin lock (bb.row_fill, idle in this
-// phase) because two updated points of one wave may share a neighbour.
+// into `upd_cand`.  Rows are written under a per-row spin lock (bb.row_fill, idle in this phase) because
+// two updated points of one wave may share a neighbour.
 template <int LPV, int NQ, int KPL>
 __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, WalkCfg cfg,
                                                                const uint32_t* __restrict__ ids, uint32_t b,
@@ -174,67 +235,18 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
     // ---- sCand ----------------------------------------------------------------------------------
     hash_clear(c);
     uint32_t ncand = 0;
-    auto add_ids = [&](uint32_t id) {  // one id per lane (kInvalid = none; ids of one call are distinct)
-      uint32_t o = 0;
-      bool is_new = id != kInvalid && hash_insert(c, id, o);
-      __syncwarp();
-      if (__any_sync(0xffffffffu, o != 0)) {  // probe budget exhausted: decide by scanning what is stored
-        if (o)
-          for (uint32_t i = 0; i < ncand && is_new; ++i) is_new = cand[i] != id;
-        __syncwarp();
-      }
-      const uint32_t mask = __ballot_sync(0xffffffffu, is_new);
-      if (is_new) cand[ncand + __popc(mask & lanemask_lt())] = id;
-      ncand += __popc(mask);
-      __syncwarp();
-    };
-    add_ids(c.lane == 0 ? p : kInvalid);
-    add_ids(one);
+    cand_add(c, cand, ncand, c.lane == 0 ? p : kInvalid);
+    cand_add(c, cand, ncand, one);
     for (uint32_t j = 0; j < n1; ++j) {
       const uint32_t e1 = __shfl_sync(0xffffffffu, one, j);
-      add_ids(load_row(g, e1, layer, c.lane));
+      cand_add(c, cand, ncand, load_row(g, e1, layer, c.lane));
     }
     // ---- re-select the row of every one-hop neighbour ----------------------------------------------
     const uint32_t Mmax = layer == 0 ? g.M0 : g.M;
     for (uint32_t j = 0; j < n1; ++j) {
       const uint32_t nbid = __shfl_sync(0xffffffffu, one, j);
-      float4 qr[NQ];
-      load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)nbid * g.dpad, c.lane);
-      const uint32_t keep = min(bg.efc, ncand - 1u);  // nb is always a member of sCand
-      UList<KPL> u;
-      ul_clear<KPL>(u, keep, c.lane);
-      uint32_t cnt = 0, worst_hi = 0xFFFFFFFFu;
-      for (uint32_t b0 = 0; b0 < ncand; b0 += 32) {
-        uint32_t id = b0 + c.lane < ncand ? cand[b0 + c.lane] : kInvalid;
-        if (id == nbid) id = kInvalid;
-        uint32_t mask = __ballot_sync(0xffffffffu, id != kInvalid);
-        uint32_t m = __popc(mask);
-        if (!m) continue;
-        if (id != kInvalid) c.cand_id[__popc(mask & lanemask_lt())] = id;
-        __syncwarp();
-        eval_candidates<LPV, NQ>(c, g.vecs, qr, m, g.metric);
-        uint32_t myhi = 0xFFFFFFFFu, myid = kInvalid;
-        if (c.lane < m) myhi = f2ord(c.cand_dist[c.lane]), myid = c.cand_id[c.lane];
-        __syncwarp();
-        uint32_t qual = __ballot_sync(0xffffffffu, c.lane < m && (cnt < keep || myhi < worst_hi));
-        while (qual) {
-          int l = __ffs(qual) - 1;
-          qual &= qual - 1;
-          uint32_t hj = __shfl_sync(0xffffffffu, myhi, l);
-          uint32_t ij = __shfl_sync(0xffffffffu, myid, l);
-          if (cnt >= keep && hj >= worst_hi) continue;
-          ul_insert<KPL>(u, hj, ij, keep, cnt, worst_hi, c.lane);
-        }
-      }
-      c.cnt = 0;
-      for (;;) {
-        uint64_t key = ul_extract_min<KPL>(u, c.lane);
-        if (key == kMaxKey) break;
-        if (c.lane == 0) c.keys[c.cnt] = key;
-        c.cnt++;
-      }
-      __syncwarp();
-      const uint32_t nsel = heuristic_select<LPV, NQ>(c, g, Mmax, a);
+      // nb is always a member of sCand
+      const uint32_t nsel = reselect_row<LPV, NQ, KPL>(c, g, a, cand, ncand, nbid, min(bg.efc, ncand - 1u), Mmax);
       const uint32_t rid = layer == 0 ? nbid : bg.cap + g.up_off[nbid] + (uint32_t)(layer - 1);
       uint32_t* row = layer == 0 ? links0 + (size_t)nbid * g.M0
                                  : links_up + (size_t)(g.up_off[nbid] + (uint32_t)(layer - 1)) * g.M;
@@ -248,6 +260,47 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
       if (c.lane == 0) atomicExch(&bb.row_fill[rid], 0u);
     }
   }
+}
+
+// Compaction repair (ehb_index_compact): the row of a live node p at layer l that names deleted points is
+// re-selected over
+//   C = {live ids of row_l(p)} U {live ids of row_l(v) : v in row_l(p), v deleted}   (minus p),
+// keeping the efc closest to p and then the heuristic with Mmax -- the step updatePoint applies to a
+// neighbour's row.  Every warp reads the pre-compaction graph and writes its result to bb.repair_out
+// ([b][M0], kInvalid padded), so the outcome does not depend on scheduling.  rows[] holds row ids in the
+// edge_row convention (< cap: level-0 row of that node; >= cap: upper row - cap).  One warp per row.
+template <int LPV, int NQ, int KPL>
+__global__ void __launch_bounds__(128) repair_rows_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ rows,
+                                                          uint32_t b, BuildBuffers bb, uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const GraphView& g = bg.g;
+  const uint32_t w = threadIdx.x >> 5;
+  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
+  if (pi >= b) return;
+  WarpCtx c;
+  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
+  Aux a = aux_of(c);
+  uint32_t* cand = bb.upd_cand + (size_t)pi * kUpdCandCap;
+  const uint32_t r = rows[pi];
+  uint32_t p = r, layer = 0;
+  if (r >= bg.cap) {
+    p = bg.up_owner[r - bg.cap];
+    layer = r - bg.cap - g.up_off[p] + 1u;
+  }
+  const uint32_t one = load_row(g, p, (int)layer, c.lane);
+  const bool dead = one != kInvalid && g.deleted[one];
+  hash_clear(c);
+  uint32_t ncand = 0;
+  cand_add(c, cand, ncand, dead ? kInvalid : one);
+  for (uint32_t dm = __ballot_sync(0xffffffffu, dead); dm; dm &= dm - 1) {
+    const uint32_t v = __shfl_sync(0xffffffffu, one, __ffs(dm) - 1);
+    const uint32_t two = load_row(g, v, (int)layer, c.lane);
+    cand_add(c, cand, ncand, two == kInvalid || two == p || g.deleted[two] ? kInvalid : two);
+  }
+  const uint32_t nsel =
+      ncand ? reselect_row<LPV, NQ, KPL>(c, g, a, cand, ncand, p, min(bg.efc, ncand), layer ? g.M : g.M0) : 0u;
+  uint32_t* out = bb.repair_out + (size_t)pi * g.M0;
+  if (c.lane < g.M0) out[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
 }
 
 static __global__ void edge_count_kernel(BuildBuffers bb) {
@@ -383,9 +436,32 @@ __global__ void __launch_bounds__(128) merge_rows_kernel(BuildGraph bg, WalkCfg 
 
 template <int LPV, int NQ>
 cudaError_t launch_build_t(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first, uint32_t b,
-                           bool is_update, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
+                           int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
   constexpr int KPL = 8;  // ef_construction <= 256
   cudaError_t e;
+  const bool is_update = mode == kBuildUpdate;
+  if (mode == kBuildUpdate || mode == kBuildRepair) {
+    if (!ids || !bb.upd_cand || (mode == kBuildRepair && (!bb.repair_out || !bg.g.deleted))) return cudaErrorInvalidValue;
+    // the two-hop candidate sets are deduplicated through a visited table of >= 4096 entries
+    WalkCfg ucfg = cfg;
+    if (ucfg.hash_size < 4096) ucfg.hash_size = 4096;
+    uint32_t uwsm = build_warp_smem(ucfg, bg.g.dpad), uwpb = wpb;
+    while (uwpb > 1 && (size_t)uwsm * uwpb > 200 * 1024) uwpb >>= 1;
+    auto ku = mode == kBuildUpdate ? update_neighbors_kernel<LPV, NQ, KPL> : repair_rows_kernel<LPV, NQ, KPL>;
+    if ((e = cudaFuncSetAttribute(ku, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)uwsm * uwpb))) !=
+        cudaSuccess)
+      return e;
+    // one warp per moved point / repaired row; repairs go in launches of <= kRepairWarps rows (upd_cand slots)
+    const uint32_t chunk = mode == kBuildUpdate ? b : kRepairWarps;
+    for (uint32_t off = 0; off < b; off += chunk) {
+      const uint32_t m = min(chunk, b - off);
+      BuildBuffers cb = bb;
+      if (mode == kBuildRepair) cb.repair_out += (size_t)off * bg.g.M0;
+      ku<<<(m + uwpb - 1) / uwpb, 32 * uwpb, (size_t)uwsm * uwpb, s>>>(bg, ucfg, ids + off, m, cb, uwsm);
+    }
+    // updatePoint's neighbour re-selection runs before the moved points are re-linked
+    if (mode == kBuildRepair) return cudaGetLastError();
+  }
   if ((e = cudaMemsetAsync(bb.edge_count, 0, 4, s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(bb.touched_count, 0, 4, s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(bb.seg_cursor, 0, 4, s)) != cudaSuccess) return e;
@@ -403,19 +479,6 @@ cudaError_t launch_build_t(const BuildGraph& bg, const WalkCfg& cfg, const uint3
   uint32_t ethreads = bb.edge_cap;
   auto ks = bg.g.deleted ? build_search_kernel<LPV, NQ, KPL, true> : build_search_kernel<LPV, NQ, KPL, false>;
   auto km = merge_rows_kernel<LPV, NQ>;
-  if (is_update) {
-    // updatePoint's neighbour re-selection runs before the moved points are re-linked
-    if (!ids || !bb.upd_cand) return cudaErrorInvalidValue;
-    WalkCfg ucfg = cfg;
-    if (ucfg.hash_size < 4096) ucfg.hash_size = 4096;
-    uint32_t uwsm = build_warp_smem(ucfg, bg.g.dpad), uwpb = wpb;
-    while (uwpb > 1 && (size_t)uwsm * uwpb > 200 * 1024) uwpb >>= 1;
-    auto ku = update_neighbors_kernel<LPV, NQ, KPL>;
-    if ((e = cudaFuncSetAttribute(ku, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)uwsm * uwpb))) !=
-        cudaSuccess)
-      return e;
-    ku<<<(b + uwpb - 1) / uwpb, 32 * uwpb, (size_t)uwsm * uwpb, s>>>(bg, ucfg, ids, b, bb, uwsm);
-  }
   if ((e = cudaFuncSetAttribute(ks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(km, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem)) != cudaSuccess) return e;
   ks<<<grid, block, smem, s>>>(bg, cfg, ids, first, b, is_update ? 1 : 0, bb, wsm);
@@ -427,9 +490,9 @@ cudaError_t launch_build_t(const BuildGraph& bg, const WalkCfg& cfg, const uint3
 }
 
 #define EHB_BUILD_ARGS                                                                                     \
-  const BuildGraph &bg, const WalkCfg &cfg, const uint32_t *ids, uint32_t first, uint32_t b, bool is_update, \
+  const BuildGraph &bg, const WalkCfg &cfg, const uint32_t *ids, uint32_t first, uint32_t b, int mode, \
       BuildBuffers &bb, uint32_t wpb, cudaStream_t s
-#define EHB_BUILD_PASS bg, cfg, ids, first, b, is_update, bb, wpb, s
+#define EHB_BUILD_PASS bg, cfg, ids, first, b, mode, bb, wpb, s
 cudaError_t launch_build_d32(EHB_BUILD_ARGS);
 cudaError_t launch_build_d64(EHB_BUILD_ARGS);
 cudaError_t launch_build_d128(EHB_BUILD_ARGS);

@@ -514,6 +514,25 @@ int ehb_sharded_build(ehb_sharded* sh) {
   return EHB_OK;
 }
 
+// Compacts every shard; the shards compact concurrently (one host thread per device).
+int ehb_sharded_compact(ehb_sharded* sh) {
+  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
+  std::lock_guard<std::mutex> g(sh->mu);
+  const size_t G = sh->shard.size();
+  std::vector<int> rc(G, EHB_OK);
+  std::vector<std::string> msg(G);
+  std::vector<std::thread> th;
+  for (size_t i = 0; i < G; ++i)
+    th.emplace_back([&, i]() {
+      rc[i] = ehb_index_compact(sh->shard[i]);
+      if (rc[i] != EHB_OK) msg[i] = ehb::last_error_text();
+    });
+  for (auto& t : th) t.join();
+  for (size_t i = 0; i < G; ++i)
+    if (rc[i] != EHB_OK) return fail(rc[i], msg[i]);
+  return EHB_OK;
+}
+
 int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   for (ehb_index* ix : sh->shard) RET(ehb_index_set_ef(ix, ef));

@@ -4,7 +4,8 @@
 //
 // Concurrency (SURVEY.md §8b B4: "searches re-entrant ... mutations exclusive").  The reference
 // serialises every RPC under one service mutex (embeddinghub/embeddingstore/server.cc:175); here
-//   * `rw` is a reader/writer lock: searches share it, mutations (add / remove / build / import) own it;
+//   * `rw` is a reader/writer lock: searches share it, mutations (add / remove / build / compact / import) own
+//     it, so a compaction waits for the searches in flight and later searches see the compacted graph;
 //   * every in-flight graph search works on a SearchSlot (own stream, own device scratch, own pinned
 //     staging) taken from a small pool, so host threads never share scratch;
 //   * concurrent small host searches are coalesced into one batched launch by the combining queue
@@ -207,6 +208,9 @@ struct ehb_index {
   uint64_t n_linked = 0;   // vectors linked into the graph
   uint64_t up_rows = 0;    // used upper rows
   uint64_t n_deleted = 0;  // tombstones
+  // points removed by compact() so far: automatic labels continue at n + n_removed, and the level generator has
+  // made n + n_removed draws (saved in the file header so a loaded index continues both sequences)
+  uint64_t n_removed = 0;
   uint32_t entry = 0;
   int32_t max_level = -1;
   uint32_t ef;
@@ -284,6 +288,7 @@ struct ehb_index {
   ehb::BuildBuffers build_buffers(uint64_t edges);
   ehb::BuildGraph build_graph() const;
   int build();
+  int compact();
   bool needs_build() const { return n_linked != n || !pending_updates.empty(); }
   int ensure_built(std::shared_lock<ehb::RwLock>& lk);
   int acquire_slot(ehb::SearchSlot** out);

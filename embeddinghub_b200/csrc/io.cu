@@ -245,7 +245,7 @@ int ehb_index_import_graph(ehb_index* ix, uint64_t n, const float* vectors, cons
 }
 
 // File format (little endian): "EHB200\0\2", ehb_params, u64 hdr[6] = {n, upper_rows, entry, max_level,
-// tombstones, 0}, then the sections in device-array order: vectors [n][dim] f32 (unpadded), labels [n] u64,
+// tombstones, points removed by ehb_index_compact (0 in files written before it existed)}, then the sections in device-array order: vectors [n][dim] f32 (unpadded), labels [n] u64,
 // levels [n] u8, deleted [n] u8, links0 [n][2M] u32, up_off [n] u32, links_up [upper_rows][M] u32.
 static uint64_t file_bytes(const ehb_params& p, uint64_t n, uint64_t rows) {
   return 8 + sizeof(ehb_params) + 48 + n * p.dim * 4ull + n * 8 + n + n + n * 2ull * p.M * 4 + n * 4 + rows * p.M * 4ull;
@@ -264,7 +264,7 @@ int ehb_index_save(ehb_index* ix, const char* path) {
     RET(pipe.init());
     const char magic[8] = {'E', 'H', 'B', '2', '0', '0', 0, 2};
     const uint64_t n = ix->n, rows = ix->up_rows;
-    uint64_t hdr[6] = {n, rows, ix->entry, (uint64_t)(int64_t)ix->max_level, ix->n_deleted, 0};
+    uint64_t hdr[6] = {n, rows, ix->entry, (uint64_t)(int64_t)ix->max_level, ix->n_deleted, ix->n_removed};
     if (std::fwrite(magic, 1, 8, f) != 8 || std::fwrite(&ix->prm, sizeof(ehb_params), 1, f) != 1 ||
         std::fwrite(hdr, 8, 6, f) != 6)
       return fail(EHB_ERR_IO, "short write");
@@ -298,7 +298,7 @@ int ehb_index_load(const char* path, int32_t device, ehb_index** out) {
     if (std::fread(&p, sizeof(p), 1, f) != 1 || std::fread(hdr, 8, 6, f) != 6) return fail(EHB_ERR_IO, "bad header");
     const uint64_t n = hdr[0], rows = hdr[1];
     if (p.dim == 0 || p.dim > ehb::kMaxDim || p.M < 2 || p.M > 16 || p.metric < 0 || p.metric > 2 ||
-        p.ef_construction > 256 || n >= 0x7FFFFFFFull || rows > n * 31ull)
+        p.ef_construction > 256 || n >= 0x7FFFFFFFull || rows > n * 31ull || hdr[5] >= (1ull << 40))
       return fail(EHB_ERR_IO, "corrupt header");
     struct stat st;
     if (fstat(fileno(f), &st) != 0 || (uint64_t)st.st_size != file_bytes(p, n, rows))
@@ -335,10 +335,12 @@ int ehb_index_load(const char* path, int32_t device, ehb_index** out) {
     CU(cudaStreamSynchronize(s));
     RET(check_links(ix, ix->links0.p, n * ix->M0, n));
     RET(check_links(ix, ix->links_up.p, rows * ix->M, n));
-    // the level generator continues after the loaded points: replay its draws
-    for (uint64_t i = 0; i < n; ++i) (void)ix->draw_level();
-    return adopt_host_tables(ix, n, rows, std::move(labels), std::move(levels), std::move(deleted), up_off.data(),
-                             (uint32_t)hdr[2], (int32_t)(int64_t)hdr[3]);
+    // the level generator continues after the loaded points and the compacted-away ones: replay its draws
+    for (uint64_t i = 0; i < n + hdr[5]; ++i) (void)ix->draw_level();
+    RET(adopt_host_tables(ix, n, rows, std::move(labels), std::move(levels), std::move(deleted), up_off.data(),
+                          (uint32_t)hdr[2], (int32_t)(int64_t)hdr[3]));
+    ix->n_removed = hdr[5];
+    return EHB_OK;
   };
   int rc = body();
   std::fclose(f);

@@ -10,6 +10,7 @@ namespace ehb {
 constexpr uint32_t kMaxDim = 2048;  // pad_dim() supports rows up to 2048 floats
 constexpr uint32_t kMaxEf = 512;    // register-resident list: 16 keys per lane
 constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved point, >= 1 + 32 + 32*32
+constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
 
 // K2 — batched k-NN graph walk (hnswlib searchKnn).  ef >= k, cfg.lcap >= ef.
 // stats: [nq][4] u32 = hops_upper, hops_base, evals, overflow.
@@ -102,6 +103,7 @@ struct BuildBuffers {
   float* seg_dist;      // [edge_cap]
   uint32_t* error_flag; // [1]
   uint32_t* upd_cand;   // [batch][kUpdCandCap] sCand scratch of the update path (nullptr for plain inserts)
+  uint32_t* repair_out; // [rows][M0] re-selected rows of the compaction repair (nullptr otherwise)
 };
 struct BuildGraph {
   GraphView g;          // links are written through these pointers (const-cast inside)
@@ -110,9 +112,34 @@ struct BuildGraph {
   uint32_t cap;         // row id space split: rows >= cap are upper rows
   uint32_t efc;
 };
-// Links points ids[0..b) (or first..first+b when ids == nullptr) into the graph.
+enum BuildMode : int {
+  kBuildInsert = 0,  // link points ids[0..b) (or first..first+b when ids == nullptr) into the graph
+  kBuildUpdate = 1,  // hnswlib updatePoint of the already linked points ids[0..b)
+  kBuildRepair = 2,  // compaction: re-select the rows ids[0..b) (row ids as edge_row) into bb.repair_out
+};
 cudaError_t launch_build_batch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
-                               uint32_t b, bool is_update, BuildBuffers& bb, uint32_t warps_per_block,
-                               cudaStream_t s);
+                               uint32_t b, int mode, BuildBuffers& bb, uint32_t warps_per_block, cudaStream_t s);
+
+// K6 — compaction (ehb_index_compact).  Row ids follow the edge_row convention: < cap a level-0 row, >= cap an
+// upper row.
+// Appends to rows[] (count in *nrows) every row of a live node that names a deleted id, and counts the level-0
+// in-links of every node (indeg, zeroed by the caller).
+cudaError_t launch_compact_mark(const uint32_t* links0, const uint32_t* links_up, const uint32_t* up_owner,
+                                const uint8_t* deleted, uint64_t n, uint64_t up_rows, uint32_t M0, uint32_t M,
+                                uint32_t cap, uint32_t* rows, uint32_t* nrows, uint32_t* indeg, cudaStream_t s);
+// Copies the re-selected rows repair_out[i] back over rows[i] (after every repair has read the old graph).
+cudaError_t launch_compact_apply(const uint32_t* rows, uint32_t nrows, const uint32_t* repair_out, uint32_t* links0,
+                                 uint32_t* links_up, uint32_t M0, uint32_t M, uint32_t cap, cudaStream_t s);
+// dst[i][j] = remap[src[src_row[i]][j]] (kInvalid stays kInvalid) for i < rows, j < width.
+cudaError_t launch_compact_remap_rows(const uint32_t* src, const uint32_t* src_row, uint64_t rows, uint32_t width,
+                                      const uint32_t* remap, uint32_t* dst, cudaStream_t s);
+// flag[i] = 1 for a node of the renumbered level-0 graph that must be re-linked: an empty row, or level-0
+// in-links before compaction (indeg_old[inv[i]] > 0) and none after.
+cudaError_t launch_compact_orphans(const uint32_t* links0, uint64_t n, uint32_t M0, const uint32_t* inv,
+                                   const uint32_t* indeg_old, uint32_t* indeg_new, uint8_t* flag, cudaStream_t s);
+// Moves vector rows inv[i] -> i for i in [lo, n) in place, through `stage` (stage_rows rows).  Safe because
+// inv[i] >= i and the chunks go in increasing i.
+cudaError_t launch_compact_move_rows(float* vecs, uint32_t dpad, const uint32_t* inv, uint64_t lo, uint64_t n,
+                                     float* stage, uint64_t stage_rows, cudaStream_t s);
 
 }  // namespace ehb

@@ -109,7 +109,8 @@ int ehb_index_destroy(ehb_index* ix);
 
 /* ANNIndex::set -> hnswlib addPoint / resizeIndex — index.cc:20-37.  Insert or
  * update-in-place (existing label).  labels == NULL assigns labels
- * size()..size()+n-1.  Points are linked into the graph lazily by the next
+ * s..s+n-1 with s = size() + the number of points removed by ehb_index_compact
+ * so far (= size() on an index that was never compacted).  Points are linked into the graph lazily by the next
  * ehb_index_build / search (batched GPU construction replaces the reference's
  * one-addPoint-per-row loop, version.cc:64-74). */
 int ehb_index_add(ehb_index* ix, uint64_t n, const float* vecs_host, const uint64_t* labels_host);
@@ -122,6 +123,19 @@ int ehb_index_build(ehb_index* ix);
  * already deleted: EHB_ERR_STATE.  Adding a deleted label again un-deletes it and updates it in place
  * (hnswlib addPoint). */
 int ehb_index_remove(ehb_index* ix, uint64_t n, const uint64_t* labels_host);
+
+/* Compaction: removes every tombstone for good.  Pending points are linked first (like ehb_index_save).  Rows
+ * of live points that named deleted points are re-selected on the GPU over their live neighbours and the live
+ * neighbours of those deleted points (hnswlib's updatePoint selection); the survivors are renumbered densely
+ * in insertion order, and survivors left without level-0 in-links (or with an empty row) are re-linked by
+ * updatePoint.  If the entry point was deleted, the live point of highest level (smallest internal id on a
+ * tie) becomes the entry point.  Afterwards size() counts the survivors only, labels and vectors are kept,
+ * internal ids (ehb_index_export_graph) change, capacity is kept (later adds reuse the freed rows) and the
+ * tombstone-free search paths apply again.  Deleting everything and compacting gives an empty index.
+ * Searches in flight finish first; later ones see the compacted graph.  No deletes: no change.
+ * The number of points removed so far is kept (automatic labels, level draws) and saved by ehb_index_save;
+ * ehb_index_export_graph / ehb_index_import_graph do not carry it, so an imported index counts from 0. */
+int ehb_index_compact(ehb_index* ix);
 
 /* hnswlib setEf (never called by the reference; named by BASELINE configs). */
 int ehb_index_set_ef(ehb_index* ix, uint32_t ef);
@@ -217,6 +231,7 @@ int ehb_sharded_remove(ehb_sharded* sh, uint64_t n, const uint64_t* labels_host)
 int ehb_sharded_get(ehb_sharded* sh, uint64_t label, float* out_vec_host);
 int ehb_sharded_size(ehb_sharded* sh, uint64_t* out);
 int ehb_sharded_build(ehb_sharded* sh); /* shards build concurrently */
+int ehb_sharded_compact(ehb_sharded* sh); /* ehb_index_compact on every shard, concurrently */
 int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef);
 int ehb_sharded_search(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef,
                        uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);

@@ -16,6 +16,7 @@
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "ehb200.h"
@@ -50,6 +51,7 @@ class ANNIndex {
       label = it->second;
     }
     check(ehb_index_add(ix_, 1, value.data(), &label));
+    deleted_.erase(key);  // hnswlib addPoint un-deletes a re-added label
   }
 
   // index.cc:39-52 — keys nearest-first.
@@ -84,6 +86,19 @@ class ANNIndex {
     if (it == key_to_label_.end()) throw std::runtime_error("ANNIndex::remove: unknown key");
     uint64_t label = it->second;
     check(ehb_index_remove(ix_, 1, &label));
+    deleted_.insert(key);
+  }
+
+  // Removes the deleted keys for good (ehb_index_compact): the graph is repaired on the GPU and the tombstone-free
+  // search paths apply again.  A removed key that is set later gets a fresh label.
+  void compact() {
+    check(ehb_index_compact(ix_));
+    for (const std::string& key : deleted_) {
+      auto it = key_to_label_.find(key);
+      label_to_key_.erase(it->second);
+      key_to_label_.erase(it);
+    }
+    deleted_.clear();
   }
 
  private:
@@ -95,6 +110,7 @@ class ANNIndex {
   std::unordered_map<std::string, uint64_t> key_to_label_;
   std::unordered_map<uint64_t, std::string> label_to_key_;
   uint64_t next_label_;
+  std::unordered_set<std::string> deleted_;  // removed (and not set again) since the last compact()
 };
 
 }  // namespace embedding
