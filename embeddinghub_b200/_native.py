@@ -81,6 +81,8 @@ SYMBOLS = {
     "ehb_index_get": (C.c_int, [_VP, _U64, _VP]),
     "ehb_index_search": (C.c_int, [_VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP]),
     "ehb_index_search_dev": (C.c_int, [_VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP, _VP]),
+    "ehb_index_search_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_index_search_ex_dev": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce_dev": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP, _VP]),
     "ehb_index_stats": (C.c_int, [_VP, C.POINTER(Stats)]),
@@ -107,6 +109,7 @@ SYMBOLS = {
     "ehb_sharded_compact": (C.c_int, [_VP]),
     "ehb_sharded_set_ef": (C.c_int, [_VP, _U32]),
     "ehb_sharded_search": (C.c_int, [_VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP]),
+    "ehb_sharded_search_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_sharded_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_exchange_create": (C.c_int, [_I32, _U32, _U32, _U64, _U32, C.POINTER(_VP)]),
     "ehb_exchange_destroy": (C.c_int, [_VP]),
@@ -242,10 +245,13 @@ class NativeIndex:
     def _alloc(self, nq, k):
         return (np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.empty(nq, np.uint32))
 
-    def search(self, q, k, ef=0):
+    def search(self, q, k, ef=0, precision=FP32):
+        """Graph search.  precision=BF16 walks the bf16 copy of the rows and re-ranks the walk's whole result set
+        in fp32: every distance is the exact fp32 one (ehb_index_search_ex)."""
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
         labels, dists, counts = self._alloc(q.shape[0], k)
-        check(lib().ehb_index_search(self._h, q.shape[0], _p(q), k, ef, _p(labels), _p(dists), _p(counts)))
+        check(lib().ehb_index_search_ex(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
+                                        _p(counts)))
         if k == 0:
             counts[:] = 0
         return labels, dists, counts
@@ -259,11 +265,12 @@ class NativeIndex:
             counts[:] = 0
         return labels, dists, counts
 
-    def search_dev(self, q_ptr, nq, k, ef, labels_ptr, dists_ptr, counts_ptr, stream=0):
-        check(lib().ehb_index_search_dev(self._h, nq, C.c_void_p(q_ptr), k, ef, C.c_void_p(labels_ptr),
-                                         C.c_void_p(dists_ptr) if dists_ptr else None,
-                                         C.c_void_p(counts_ptr) if counts_ptr else None,
-                                         C.c_void_p(stream) if stream else None))
+    def search_dev(self, q_ptr, nq, k, ef, labels_ptr, dists_ptr, counts_ptr, stream=0, precision=FP32):
+        check(lib().ehb_index_search_ex_dev(self._h, nq, C.c_void_p(q_ptr), k, ef, int(precision),
+                                            C.c_void_p(labels_ptr),
+                                            C.c_void_p(dists_ptr) if dists_ptr else None,
+                                            C.c_void_p(counts_ptr) if counts_ptr else None,
+                                            C.c_void_p(stream) if stream else None))
 
     def search_bruteforce_dev(self, q_ptr, nq, k, precision, labels_ptr, dists_ptr, counts_ptr, stream=0):
         check(lib().ehb_index_search_bruteforce_dev(self._h, nq, C.c_void_p(q_ptr), k, precision,
@@ -400,11 +407,12 @@ class ShardedIndex:
         ix._owned = False   # borrowed: the sharded index destroys it
         return ix
 
-    def search(self, q, k, ef=0):
+    def search(self, q, k, ef=0, precision=FP32):
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
         nq = q.shape[0]
         labels, dists, counts = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
-        check(lib().ehb_sharded_search(self._h, nq, _p(q), k, ef, _p(labels), _p(dists), _p(counts)))
+        check(lib().ehb_sharded_search_ex(self._h, nq, _p(q), k, ef, int(precision), _p(labels), _p(dists),
+                                          _p(counts)))
         return labels, dists, counts
 
     def search_bruteforce(self, q, k, precision=FP32):

@@ -10,7 +10,7 @@ exactly as the reference (which never calls setEf).
 """
 import numpy as np
 
-from ._native import NativeIndex
+from ._native import FP32, NativeIndex
 
 
 class ANNIndex:
@@ -85,19 +85,21 @@ class ANNIndex:
     def approx_nearest(self, value, num):
         return self.approx_nearest_batch(np.asarray(value, np.float32)[None, :], num)[0]
 
-    def approx_nearest_batch(self, values, num, ef=0):
+    def approx_nearest_batch(self, values, num, ef=0, precision=FP32):
         """Batched k-NN (docs/inference.md:14-22 promises multi_nearest_neighbor;
-        the reference never implemented it)."""
+        the reference never implemented it).  precision=BF16 walks the graph over bf16 rows and re-ranks in fp32
+        (ehb_index_search_ex); the exact-scan fallback below runs at the same precision."""
         if num == 0:
             return [[] for _ in range(len(values))]
         values = np.asarray(values, np.float32)
         if values.ndim != 2 or values.shape[1] != self._dims:
             raise ValueError(f"query has {values.shape[-1] if values.ndim else 0} values, the index has {self._dims} dimensions")
+        extra = () if precision == FP32 else (precision,)   # the default keeps the plain fp32 call
         if max(num, ef) > 512:
             # beyond the register-resident beam (ef <= 512) the exact scan answers (any num the reference accepts)
-            labels, _, counts = self._nn.search_bruteforce(values, num)
+            labels, _, counts = self._nn.search_bruteforce(values, num, *extra)
         else:
-            labels, _, counts = self._nn.search(values, num, ef)
+            labels, _, counts = self._nn.search(values, num, ef, *extra)
         return [[self._label_to_key[int(l)] for l in row[:c]] for row, c in zip(labels, counts)]
 
     def get(self, key):

@@ -40,21 +40,23 @@ ehb::GraphView ehb_index::view() const {
   g.entry = entry;
   g.max_level = max_level;
   g.metric = metric == EHB_L2 ? 0 : 1;
+  g.vecs16 = nullptr;
   return g;
 }
 
 // ef_eff: beam width; smem_list: capacity of the shared-memory key list (0 for plain searches);
 // jobs: warps (queries or points) of the launch; team: warps sharing one visited table.
-ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team) const {
+ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16) const {
   ehb::WalkCfg c;
+  const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);  // bytes of a row as the walk reads it
   c.lcap = smem_list;
-  c.staged = dpad > 256 ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
+  c.staged = vbytes > 1024 ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
   c.dcap = n_deleted ? ehb::kDeletedQueue : 0;
   c.prefetch = o_walk_prefetch ? 1 : 0;
   // dense walk (search_impl.cuh): batches big enough to fill 20 warps per SM, rows <= 512 B, no tombstones
   c.dense = (!smem_list && team == 1 && !c.staged && dpad <= 128 && !n_deleted && jobs >= 20ull * (uint64_t)sms) ? 1 : 0;
+  if (bf16 && dpad == 128 && ef_eff > 128) c.dense = 0;  // no dense bf16 form there (search_impl.cuh dense_form)
   const uint32_t warp_target = c.dense ? 20u : 16u;  // resident warps per SM the visited-table sizing aims at
-  uint32_t vbytes = dpad * 4;
   uint32_t nslots = std::max(4u, std::min(32u, 24576u / vbytes));
   uint32_t ng = 2;                      // two groups: math on one overlaps the copies of the other
   uint32_t g = std::max(4u, nslots / ng / 4 * 4);  // vectors per group, multiple of the 4-vector math step
@@ -77,7 +79,7 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
     uint32_t want = (uint32_t)std::min<uint64_t>((ctas + sms - 1) / sms, c.staged ? 5u : warp_target / team);
     want = std::max(want, 4u);
     c.hash_size = 0;
-    uint32_t fixed = ehb::warp_smem_bytes(c, dpad) * team + 1024u + (smem_list ? 256u : 0u);
+    uint32_t fixed = ehb::warp_smem_bytes(c, vbytes) * team + 1024u + (smem_list ? 256u : 0u);
     uint32_t per_cta = (227u * 1024u) / want;
     uint32_t avail = per_cta > fixed + 1024u ? (per_cta - fixed) / 4u : 256u;
     hs = std::min(roomy, std::max(tight, avail));
@@ -85,14 +87,15 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
   }
   c.hash_size = ehb::align_up(std::max(hs, 256u), 32);
   // stay inside the 227 KB per-block limit
-  while (ehb::warp_smem_bytes(c, dpad) + 256 > 200 * 1024 && c.hash_size > 512)
+  while (ehb::warp_smem_bytes(c, vbytes) + 256 > 200 * 1024 && c.hash_size > 512)
     c.hash_size = ehb::align_up(c.hash_size / 2, 32);
   return c;
 }
 
-uint32_t ehb_index::wpb_for(const ehb::WalkCfg& c, uint32_t extra) const {
+uint32_t ehb_index::wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16) const {
   uint32_t w = t_wpb ? t_wpb : 1;
-  while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, dpad) + extra) * w > 220 * 1024) w >>= 1;
+  const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);
+  while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, vbytes) + extra) * w > 220 * 1024) w >>= 1;
   return w;
 }
 
@@ -107,7 +110,35 @@ int ehb_index::ensure_capacity(uint64_t want) {
   CU(deleted.grow(nc, n, 0, stream));
   CU(links0.grow(nc * M0, n * M0, 0xFF, stream));
   CU(up_off.grow(nc, n, 0xFF, stream));
+  if (shadow) {
+    CU(x_bf16.grow(nc * dpad, n * dpad, -1, stream));
+    CU(x_norm.grow(nc, n, -1, stream));
+  }
   cap = nc;
+  return EHB_OK;
+}
+
+// ---- bf16 shadow ----------------------------------------------------------------------------------------
+// Writer side.  Sized like vecs (capacity rows), so adds within the capacity never reallocate it.
+int ehb_index::create_shadow() {
+  if (shadow) return EHB_OK;
+  CU(x_bf16.grow(std::max<uint64_t>(cap, 1) * dpad, 0, -1, stream));
+  CU(x_norm.grow(std::max<uint64_t>(cap, 1), 0, -1, stream));
+  CU(ehb::launch_to_bf16(vecs.p, dpad, x_bf16.p, x_norm.p, n, dpad, stream));
+  CU(cudaStreamSynchronize(stream));
+  shadow = true;
+  return EHB_OK;
+}
+
+void ehb_index::drop_shadow() {
+  x_bf16.release();
+  x_norm.release();
+  shadow = false;
+}
+
+int ehb_index::shadow_rows(uint64_t first, uint64_t cnt) {
+  if (!shadow || cnt == 0) return EHB_OK;
+  CU(ehb::launch_to_bf16(vecs.p + first * dpad, dpad, x_bf16.p + first * dpad, x_norm.p + first, cnt, dpad, stream));
   return EHB_OK;
 }
 
@@ -152,7 +183,7 @@ void ehb_index::reset_content() {
   h_deleted.clear();
   pending_updates.clear();
   identity_labels = true;
-  bf16_rows = 0;
+  drop_shadow();
 }
 
 // ---- ingest ---------------------------------------------------------------------------------------
@@ -242,6 +273,7 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
       }
       if (contiguous_new) {
         CU(ehb::launch_pad_rows(dsrc, vecs.p + first_new * dpad, m, dim, dpad, metric == EHB_COSINE, stream));
+        RET(shadow_rows(first_new, m));
       } else {
         // rows go to arbitrary ids: one launch per run of consecutive destinations
         uint64_t i = 0;
@@ -250,6 +282,7 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
           while (j < m && dst[j] == dst[j - 1] + 1) ++j;
           CU(ehb::launch_pad_rows(dsrc + i * dim, vecs.p + (uint64_t)dst[i] * dpad, j - i, dim, dpad,
                                   metric == EHB_COSINE, stream));
+          RET(shadow_rows(dst[i], j - i));
           i = j;
         }
       }
@@ -272,7 +305,6 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
     pending_updates.insert(pending_updates.end(), relink.begin(), relink.end());
     n = nn;
     up_rows = rows;
-    bf16_rows = 0;
   }
   return EHB_OK;
 }
@@ -294,7 +326,6 @@ int ehb_index::remove_labels(uint64_t cnt, const uint64_t* lab) {
   CU(cudaStreamSynchronize(stream));
   for (uint32_t id : ids) h_deleted[id] = 1;
   n_deleted += cnt;
-  bf16_rows = 0;
   return EHB_OK;
 }
 
@@ -533,6 +564,7 @@ int ehb_index::compact() {
   uint64_t lo = 0;
   while (lo < nn && inv[lo] == lo) ++lo;  // rows below the first tombstone stay where they are
   CU(ehb::launch_compact_move_rows(vecs.p, dpad, d_inv.p, lo, nn, stage.p, stage_rows, s));
+  RET(shadow_rows(lo, nn - lo));  // the survivors' rows moved: re-convert them in their new places
   CU(cudaMemcpyAsync(labels.p, labels_new.data(), nn * 8, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(levels.p, levels_new.data(), nn, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(up_off.p, up_off_new.data(), nn * 4, cudaMemcpyHostToDevice, s));
@@ -561,21 +593,36 @@ int ehb_index::compact() {
   n_deleted = 0;
   entry = entry_new;
   max_level = max_level_new;
-  bf16_rows = 0;
   // 5. re-link the orphans (updatePoint: a beam search from the entry point, then mutual links)
   for (uint64_t i = 0; i < nn; ++i)
     if (is_orphan[i]) pending_updates.push_back((uint32_t)i);
   return build();
 }
 
-// Searches link pending points lazily; that needs the writer side of the lock.
-int ehb_index::ensure_built(std::shared_lock<ehb::RwLock>& lk) {
-  while (needs_build()) {
+// Searches link pending points lazily, and the first bf16 search creates the bf16 shadow; both need the writer
+// side of the lock.  Another writer may run between the unlock and the lock, so the state is checked again.
+int ehb_index::ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16) {
+  while (needs_build() || (bf16 && !shadow)) {
     lk.unlock();
     int rc;
     {
       std::unique_lock<ehb::RwLock> x(rw);
       rc = build();
+      if (rc == EHB_OK && bf16) rc = create_shadow();
+    }
+    lk.lock();
+    if (rc != EHB_OK) return rc;
+  }
+  return EHB_OK;
+}
+
+int ehb_index::ensure_shadow(std::shared_lock<ehb::RwLock>& lk) {
+  while (!shadow) {
+    lk.unlock();
+    int rc;
+    {
+      std::unique_lock<ehb::RwLock> x(rw);
+      rc = create_shadow();
     }
     lk.lock();
     if (rc != EHB_OK) return rc;
@@ -621,11 +668,16 @@ void ehb_index::release_slot(ehb::SearchSlot* sl, cudaStream_t used) {
 // ---- search --------------------------------------------------------------------------------------------
 // Caller holds the shared lock, the graph is built, `sl` is acquired.
 int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uint32_t k, uint32_t ef_in, uint64_t* dl,
-                          float* dd, uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink, bool* pushed) {
+                          float* dd, uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink, bool* pushed,
+                          int precision) {
   if (pushed) *pushed = false;
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (k == 0 || nq == 0) return EHB_OK;
   uint32_t ef_eff = std::max(ef_in ? ef_in : ef, k);
   if (ef_eff > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
+  const bool bf16 = precision == EHB_BF16;
+  if (bf16 && sink) return fail(EHB_ERR_INVALID, "the fused shard exchange walks fp32 rows only");
+  if (bf16 && !shadow) return fail(EHB_ERR_STATE, "bf16 shadow missing");
   // Warps per query (rows <= 1 KB, ef <= 256): four while 3 CTAs of 128 threads per SM hold every query (small
   // online batches, where one warp's serial chain of memory round trips is the bound), two while 7 CTAs of 64
   // threads do (C2, Q=1000), else one warp per query: once the batch alone fills the SMs, the team walk's
@@ -633,7 +685,8 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   uint32_t team = t_team;
   if (team == 0) team = nq <= (uint64_t)sms * 3 ? 4 : (nq <= (uint64_t)sms * 7 ? 2 : 1);
   if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
-  ehb::WalkCfg cfg = walk_cfg(ef_eff, 0, nq * team, team);
+  if (bf16) team = 1;                                       // the team walk reads fp32 rows only
+  ehb::WalkCfg cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16);
   if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
   const float* q = dq;
   if (metric == EHB_COSINE) {
@@ -643,9 +696,25 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   }
   CU(sl->stats.grow(nq * 4, 0, -1, s));
   CU(sl->stat_sum.grow(4, 0, 0, s));
-  uint32_t wpb = wpb_for(cfg, 0);
+  if (bf16) {
+    CU(sl->q_pad.grow(nq * dpad, 0, -1, s));
+    CU(sl->walk_keys.grow(nq * ef_eff, 0, -1, s));
+    CU(sl->walk_counts.grow(nq, 0, -1, s));
+    CU(ehb::launch_pad_rows(dq, sl->q_pad.p, nq, dim, dpad, metric == EHB_COSINE, s));
+  }
+  uint32_t wpb = wpb_for(cfg, 0, bf16);
   CU(cudaEventRecord(sl->ev0, s));
-  if (team >= 2)
+  if (bf16) {
+    // walk the bf16 rows keeping the whole retained set, then re-rank it with the canonical fp32 chain
+    ehb::ResultSink ks;
+    std::memset(&ks, 0, sizeof(ks));
+    ks.keys = sl->walk_keys.p;
+    ehb::GraphView g = view();
+    g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
+    CU(ehb::launch_search_bf16(g, cfg, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, wpb, s));
+    CU(ehb::launch_rerank(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
+                          labels.p, nq, k, dl, dd, dc, s));
+  } else if (team >= 2)
     CU(ehb::launch_search_team(team, view(), cfg.hash_size, q, (uint32_t)nq, k, ef_eff, dl, dd, dc, sl->stats.p, s));
   else {
     ehb::ResultSink one;
@@ -662,16 +731,17 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   }
   CU(cudaEventRecord(sl->ev1, s));
   sl->last_nq = nq;
+  sl->last_bf16 = bf16;
   {
     const uint32_t kpl = ef_eff <= 64 ? 2 : (ef_eff <= 128 ? 4 : (ef_eff <= 256 ? 8 : 16));
-    const uint32_t lpv = dpad > 256 ? 32 : 8;
+    const uint32_t lpv = cfg.staged ? 32 : 8;
     if (team >= 2)
       std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "hnsw_search_team_kernel<NQ=%u,KPL=%u,T=%u,U=%u>",
                     dpad / (4 * lpv), kpl, team, ehb::team_eval_steps(team, dpad, (uint32_t)nq));
     else  // (HASDEL is named only when set, so the common instantiations keep their short names)
-      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "%s<LPV=%u,NQ=%u,KPL=%u%s>",
+      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "%s<LPV=%u,NQ=%u,KPL=%u%s%s>",
                     cfg.dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", lpv, dpad / (4 * lpv), kpl,
-                    n_deleted ? ",HASDEL=1" : "");
+                    n_deleted ? ",HASDEL=1" : "", bf16 ? ",ROW=bf16" : "");
   }
   {
     std::lock_guard<std::mutex> g(last_mu);
@@ -710,13 +780,9 @@ int ehb_index::bruteforce_dev(uint64_t nq, const float* dq, uint32_t k, int prec
   sc.deleted = n_deleted ? deleted.p : nullptr;
   ehb::Bf16Ctx bctx;
   if (bf16) {
-    // bf16 shadow of the base rows (+ squared norms), refreshed lazily after mutations
-    if (bf16_rows != n) {
-      CU(x_bf16.grow(std::max<uint64_t>(n, 1) * dpad, 0, -1, s));
-      CU(x_norm.grow(std::max<uint64_t>(n, 1), 0, -1, s));
-      CU(ehb::launch_to_bf16(vecs.p, dpad, x_bf16.p, x_norm.p, n, dpad, s));
-      bf16_rows = n;
-    }
+    // the bf16 shadow of the base rows (+ squared norms): the caller made sure it exists (ensure_shadow), and
+    // the mutations keep it current
+    if (!shadow) return fail(EHB_ERR_STATE, "bf16 shadow missing");
     CU(q_bf16.grow(nq * dpad, 0, -1, s));
     CU(q_norm2.grow(nq, 0, -1, s));
     CU(ehb::launch_to_bf16(bf_qpad.p, dpad, q_bf16.p, q_norm2.p, nq, dpad, s));
@@ -765,8 +831,8 @@ int ehb_index::bruteforce_dev(uint64_t nq, const float* dq, uint32_t k, int prec
 namespace {
 
 // One host graph search on its own slot: H2D (from `q`, host), walk, D2H, synchronise.
-int search_host_direct(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
-                       uint32_t* oc) {
+int search_host_direct(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                       uint64_t* ol, float* od, uint32_t* oc) {
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = sl->stream;
@@ -777,7 +843,8 @@ int search_host_direct(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, u
     CU(sl->o_dists.grow(nq * k, 0, -1, s));
     CU(sl->o_counts.grow(nq, 0, -1, s));
     CU(cudaMemcpyAsync(sl->q_in.p, q, nq * ix->dim * 4, cudaMemcpyHostToDevice, s));
-    RET(ix->search_dev(sl, nq, sl->q_in.p, k, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s));
+    RET(ix->search_dev(sl, nq, sl->q_in.p, k, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s, nullptr, nullptr,
+                       precision));
     CU(cudaMemcpyAsync(ol, sl->o_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s));
     if (od) CU(cudaMemcpyAsync(od, sl->o_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s));
     if (oc) CU(cudaMemcpyAsync(oc, sl->o_counts.p, nq * 4, cudaMemcpyDeviceToHost, s));
@@ -789,12 +856,13 @@ int search_host_direct(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, u
   return rc;
 }
 
-// The leader's part of the combining queue: all taken requests share (k, ef) and go out as one launch.
+// The leader's part of the combining queue: all taken requests share (k, ef, precision) and go out as one launch.
 // (Every queued caller holds the shared lock and has seen the graph built, so no mutation can intervene.)
 int run_combined(ehb_index* ix, std::vector<ehb::CombineReq*>& batch) {
   uint64_t tot = 0;
   for (auto* r : batch) tot += r->nq;
   const uint32_t k = batch[0]->k, ef = batch[0]->ef, dim = ix->dim;
+  const int precision = batch[0]->precision;
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = sl->stream;
@@ -814,7 +882,8 @@ int run_combined(ehb_index* ix, std::vector<ehb::CombineReq*>& batch) {
       off += r->nq;
     }
     CU(cudaMemcpyAsync(sl->q_in.p, sl->h_q.p, tot * dim * 4, cudaMemcpyHostToDevice, s));
-    RET(ix->search_dev(sl, tot, sl->q_in.p, k, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s));
+    RET(ix->search_dev(sl, tot, sl->q_in.p, k, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s, nullptr, nullptr,
+                       precision));
     CU(cudaMemcpyAsync(sl->h_l.p, sl->o_labels.p, tot * k * 8, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(sl->h_d.p, sl->o_dists.p, tot * k * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(sl->h_c.p, sl->o_counts.p, tot * 4, cudaMemcpyDeviceToHost, s));
@@ -836,12 +905,12 @@ int run_combined(ehb_index* ix, std::vector<ehb::CombineReq*>& batch) {
 }
 
 // Combining queue ("group commit"): a caller queues its request; whoever finds a free leader seat takes
-// every queued request with its own (k, ef) and runs them as ONE batched search.  Nobody ever waits on a
+// every queued request with its own (k, ef, precision) and runs them as ONE batched search.  Nobody ever waits on a
 // timer: requests pile up only while earlier batches occupy the leader seats, which is exactly when
 // batching pays.  A lone caller becomes its own leader at once.
-int search_host_combined(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
-                         uint32_t* oc) {
-  ehb::CombineReq me{q, nq, k, ef, ol, od, oc};
+int search_host_combined(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                         uint64_t* ol, float* od, uint32_t* oc) {
+  ehb::CombineReq me{q, nq, k, ef, precision, ol, od, oc};
   std::unique_lock<std::mutex> g(ix->cq_mu);
   ix->cq.push_back(&me);
   for (;;) {
@@ -851,7 +920,7 @@ int search_host_combined(ehb_index* ix, uint64_t nq, const float* q, uint32_t k,
       uint64_t tot = 0;
       for (auto it = ix->cq.begin(); it != ix->cq.end();) {
         ehb::CombineReq* r = *it;
-        if (r->k == k && r->ef == ef && (r == &me || tot + r->nq <= ehb::kCombineMaxBatch)) {
+        if (r->k == k && r->ef == ef && r->precision == precision && (r == &me || tot + r->nq <= ehb::kCombineMaxBatch)) {
           r->taken = true;
           tot += r->nq;
           batch.push_back(r);
@@ -1010,30 +1079,41 @@ int ehb_index_get(ehb_index* ix, uint64_t label, float* out) {
   return EHB_OK;
 }
 
-int ehb_index_search(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
-                     uint32_t* oc) {
+int ehb_index_search_ex(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                        uint64_t* ol, float* od, uint32_t* oc) {
   ENTER_S(ix);
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
   if (std::max(ef ? ef : ix->ef, k) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
-  RET(ix->ensure_built(_g));  // before queueing: a waiting follower must never block a writer the leader needs
+  // before queueing: a waiting follower must never block a writer the leader needs
+  RET(ix->ensure_built(_g, precision == EHB_BF16));
   if (ix->o_combine && nq <= ehb::kCombineMaxCall)
-    return search_host_combined(ix, nq, q, k, ef ? ef : ix->ef, ol, od, oc);
-  return search_host_direct(ix, nq, q, k, ef, ol, od, oc);
+    return search_host_combined(ix, nq, q, k, ef ? ef : ix->ef, precision, ol, od, oc);
+  return search_host_direct(ix, nq, q, k, ef, precision, ol, od, oc);
+}
+int ehb_index_search(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
+                     uint32_t* oc) {
+  return ehb_index_search_ex(ix, nq, q, k, ef, EHB_FP32, ol, od, oc);
 }
 
-int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, uint64_t* dl, float* dd,
-                         uint32_t* dc, void* stream) {
+int ehb_index_search_ex_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
+                            uint64_t* dl, float* dd, uint32_t* dc, void* stream) {
   ENTER_S(ix);
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (nq && (!dq || !dl)) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
-  RET(ix->ensure_built(_g));
+  RET(ix->ensure_built(_g, precision == EHB_BF16));
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = stream ? (cudaStream_t)stream : sl->stream;
-  int rc = ix->search_dev(sl, nq, dq, k, ef, dl, dd, dc, s);
+  int rc = ix->search_dev(sl, nq, dq, k, ef, dl, dd, dc, s, nullptr, nullptr, precision);
   ix->release_slot(sl, s);
   return rc;
+}
+int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, uint64_t* dl, float* dd,
+                         uint32_t* dc, void* stream) {
+  return ehb_index_search_ex_dev(ix, nq, dq, k, ef, EHB_FP32, dl, dd, dc, stream);
 }
 
 }  // extern "C"
@@ -1059,6 +1139,7 @@ int ehb_index_search_bruteforce(ehb_index* ix, uint64_t nq, const float* q, uint
   ENTER_S(ix);
   if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
+  if (precision == EHB_BF16) RET(ix->ensure_shadow(_g));  // before bf_mu: the upgrade waits for other readers
   std::lock_guard<std::mutex> bg(ix->bf_mu);
   cudaStream_t s = ix->stream;
   CU(ix->bf_q_in.grow(nq * ix->dim, 0, -1, s));
@@ -1078,6 +1159,7 @@ int ehb_index_search_bruteforce_dev(ehb_index* ix, uint64_t nq, const float* dq,
                                     uint64_t* dl, float* dd, uint32_t* dc, void* stream) {
   ENTER_S(ix);
   if (nq && (!dq || !dl)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (precision == EHB_BF16 && k && nq) RET(ix->ensure_shadow(_g));
   std::lock_guard<std::mutex> bg(ix->bf_mu);
   return ix->bruteforce_dev(nq, dq, k, precision, dl, dd, dc, stream ? (cudaStream_t)stream : ix->stream);
 }
@@ -1094,7 +1176,12 @@ int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
         CU(cudaEventSynchronize(sl->ev1));
         CU(ehb::launch_sum_stats(sl->stats.p, (uint32_t)sl->last_nq, sl->stat_sum.p, ix->stream));
         CU(cudaMemcpyAsync(ix->last_sum, sl->stat_sum.p, 32, cudaMemcpyDeviceToHost, ix->stream));
+        ix->last_reranked = 0;
+        std::vector<uint32_t> cnt(sl->last_bf16 ? sl->last_nq : 0);
+        if (sl->last_bf16)
+          CU(cudaMemcpyAsync(cnt.data(), sl->walk_counts.p, sl->last_nq * 4, cudaMemcpyDeviceToHost, ix->stream));
         CU(cudaStreamSynchronize(ix->stream));
+        for (uint32_t c : cnt) ix->last_reranked += c;
         ix->last_sum_valid = true;
       }
       out->queries = sl->last_nq;
@@ -1102,8 +1189,10 @@ int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
       out->hops_base = ix->last_sum[1];
       out->dist_evals = ix->last_sum[2];
       out->visited_overflow = ix->last_sum[3];
+      // a bf16 walk reads 2 bytes per element, and its re-rank reads the fp32 rows of the retained keys
       out->algorithmic_bytes = out->hops_upper * 4ull * ix->M + out->hops_base * 4ull * ix->M0 +
-                               out->dist_evals * 4ull * ix->dim + out->queries * 4ull * ix->dim;
+                               out->dist_evals * (sl->last_bf16 ? 2ull : 4ull) * ix->dim +
+                               out->queries * 4ull * ix->dim + ix->last_reranked * 4ull * ix->dim;
     }
   }
   out->size = ix->n;

@@ -38,7 +38,7 @@ __device__ __forceinline__ Aux aux_of(const WarpCtx& c) {
   return a;
 }
 __host__ __device__ inline uint32_t build_warp_smem(const WalkCfg& cfg, uint32_t dpad) {
-  return 256u + warp_smem_bytes(cfg, dpad);
+  return 256u + warp_smem_bytes(cfg, dpad * 4u);
 }
 
 // hnswlib getNeighborsByHeuristic2 over keys[0..cnt) (ascending distance to

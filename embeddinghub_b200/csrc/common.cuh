@@ -74,6 +74,16 @@ __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {
   asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
 }
+__device__ __forceinline__ uint4 ld_nc_u4(const uint4* p) {
+  uint4 v;
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ uint2 ld_nc_u2(const uint2* p) {
+  uint2 v;
+  asm volatile("ld.global.nc.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
+  return v;
+}
 
 // system-scope release / acquire on a flag word (peer memory over NVLink)
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {

@@ -540,9 +540,11 @@ int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
 }
 
 // Host queries in, merged host results out.  mode: 0 = graph walk, 1 = exact brute force, 2 = bf16 brute force.
-static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol,
-                          float* od, uint32_t* oc) {
+// precision: of the graph walk (a bf16 walk re-ranks straight into device 0's gather block, like the fp32 walk).
+static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
+                          int precision, uint64_t* ol, float* od, uint32_t* oc) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
   if (nq == 0 || k == 0) return EHB_OK;
   std::lock_guard<std::mutex> g(sh->mu);
@@ -573,7 +575,7 @@ static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q
     uint64_t* dl = (uint64_t*)dst;
     float* dd = (float*)(dst + nq * k * 8ull);
     if (mode == 0)
-      RET(ehb_index_search_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, ef, dl, dd, sh->cnt_dev[i]->p, s));
+      RET(ehb_index_search_ex_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, ef, precision, dl, dd, sh->cnt_dev[i]->p, s));
     else
       RET(ehb_index_search_bruteforce_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, mode == 2 ? EHB_BF16 : EHB_FP32, dl, dd,
                                           sh->cnt_dev[i]->p, s));
@@ -595,11 +597,15 @@ static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q
 
 int ehb_sharded_search(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
                        uint32_t* oc) {
-  return sharded_search(sh, 0, nq, q, k, ef, ol, od, oc);
+  return sharded_search(sh, 0, nq, q, k, ef, EHB_FP32, ol, od, oc);
+}
+int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                          uint64_t* ol, float* od, uint32_t* oc) {
+  return sharded_search(sh, 0, nq, q, k, ef, precision, ol, od, oc);
 }
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, int precision, uint64_t* ol,
                                   float* od, uint32_t* oc) {
-  return sharded_search(sh, precision == EHB_BF16 ? 2 : 1, nq, q, k, 0, ol, od, oc);
+  return sharded_search(sh, precision == EHB_BF16 ? 2 : 1, nq, q, k, 0, EHB_FP32, ol, od, oc);
 }
 
 }  // extern "C"

@@ -156,10 +156,14 @@ struct SearchSlot {
   DevBuf<float> q_in, q_norm, o_dists;
   DevBuf<uint64_t> o_labels;
   DevBuf<uint32_t> o_counts, stats;
+  DevBuf<float> q_pad;          // bf16 graph search: padded (cosine: normalised) queries for the fp32 re-rank
+  DevBuf<uint64_t> walk_keys;   // bf16 graph search: [nq][ef] retained keys of the walk
+  DevBuf<uint32_t> walk_counts; // bf16 graph search: [nq] retained count (the keys re-ranked)
+  bool last_bf16 = false;       // the most recent search on this slot walked the bf16 shadow
   DevBuf<unsigned long long> stat_sum;
   PinBuf h_q, h_l, h_d, h_c;
   uint64_t last_nq = 0;
-  char last_kernel[64] = {0};  // name of the graph-walk kernel of the most recent search on this slot
+  char last_kernel[96] = {0};  // name of the graph-walk kernel of the most recent search on this slot
   ~SearchSlot() {
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
@@ -173,6 +177,7 @@ struct CombineReq {
   const float* q;
   uint64_t nq;
   uint32_t k, ef;
+  int precision;
   uint64_t* ol;
   float* od;
   uint32_t* oc;
@@ -236,6 +241,7 @@ struct ehb_index {
   ehb::SearchSlot* last_slot = nullptr;  // graph search (counters + events)
   bool last_was_brute = false, timed = false;
   unsigned long long last_sum[4] = {0, 0, 0, 0};
+  unsigned long long last_reranked = 0;  // keys the bf16 re-rank read (0 for an fp32 search)
   bool last_sum_valid = false;
 
   // combining queue of small host searches
@@ -250,11 +256,18 @@ struct ehb_index {
   ehb::DevBuf<float> bf_q_in, bf_o_dists, bf_dist, bf_qpad;
   ehb::DevBuf<uint64_t> bf_o_labels, bf_part, bf_run;
   ehb::DevBuf<uint32_t> bf_o_counts;
-  ehb::DevBuf<uint16_t> x_bf16, q_bf16;   // bf16 shadows for the tensor-core path
-  ehb::DevBuf<float> x_norm, q_norm2, bf_thr;
+  ehb::DevBuf<uint16_t> q_bf16;
+  ehb::DevBuf<float> q_norm2, bf_thr;
   ehb::DevBuf<uint64_t> bf_cbuf;
   ehb::DevBuf<uint32_t> bf_ccount;
-  uint64_t bf16_rows = 0;            // rows of x_bf16 that are current (0 = stale)
+  // The bf16 shadow of the base rows ([cap][dpad] bf16 + squared norms of the rounded rows), read by the bf16
+  // graph walk and the bf16 brute force.  The first bf16 search creates it (writer side of `rw`); from then on
+  // every mutation keeps rows [0, n) equal to bf16(vecs) under the writer lock: add_rows converts the rows it
+  // wrote, ensure_capacity grows it with vecs, compact re-converts the survivors, load / import / reset drop it.
+  // An index that never runs a bf16 search allocates none of it.
+  ehb::DevBuf<uint16_t> x_bf16;
+  ehb::DevBuf<float> x_norm;
+  bool shadow = false;
 
   // build scratch
   ehb::DevBuf<uint32_t> b_edge_row, b_edge_src, b_row_cnt, b_row_fill, b_row_start, b_touched, b_seg_src, b_counters,
@@ -276,8 +289,9 @@ struct ehb_index {
   ~ehb_index();
 
   ehb::GraphView view() const;
-  ehb::WalkCfg walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team) const;
-  uint32_t wpb_for(const ehb::WalkCfg& c, uint32_t extra) const;
+  // bf16: the walk reads the bf16 shadow (rows of dpad * 2 bytes)
+  ehb::WalkCfg walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16 = false) const;
+  uint32_t wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16 = false) const;
   int ensure_capacity(uint64_t want);
   int ensure_upper(uint64_t want_rows);
   int draw_level();
@@ -290,13 +304,20 @@ struct ehb_index {
   int build();
   int compact();
   bool needs_build() const { return n_linked != n || !pending_updates.empty(); }
-  int ensure_built(std::shared_lock<ehb::RwLock>& lk);
+  // (re-)take the writer side until the graph is built and, with bf16, the shadow exists
+  int ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16 = false);
+  int ensure_shadow(std::shared_lock<ehb::RwLock>& lk);
+  int create_shadow();
+  void drop_shadow();
+  int shadow_rows(uint64_t first, uint64_t cnt);  // re-convert rows [first, first + cnt) when the shadow exists
   int acquire_slot(ehb::SearchSlot** out);
   void release_slot(ehb::SearchSlot* sl, cudaStream_t used);
   // sink (optional): extra destinations + slice flags for the sharded exchange; *pushed tells whether the
   // launched kernel honoured it (the one-warp walk does, the team walk does not)
+  // precision EHB_BF16 walks the bf16 shadow (caller made sure it exists) and re-ranks the retained set in fp32
   int search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uint32_t k, uint32_t ef_in, uint64_t* dl, float* dd,
-                 uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink = nullptr, bool* pushed = nullptr);
+                 uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink = nullptr, bool* pushed = nullptr,
+                 int precision = EHB_FP32);
   int bruteforce_dev(uint64_t nq, const float* dq, uint32_t k, int precision, uint64_t* dl, float* dd, uint32_t* dc,
                      cudaStream_t s);
   void reset_content();

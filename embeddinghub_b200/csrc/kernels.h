@@ -17,6 +17,12 @@ constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persi
 cudaError_t launch_search(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
                           uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                           uint32_t warps_per_block, cudaStream_t s);
+// K2 over the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation).  Writes the retained set, not results:
+// sink.keys[nq][k] gets the (ordered distance, internal id) keys nearest-first (call with k = ef to keep all of
+// them) and out_counts the retained count; launch_rerank then produces the fp32 results.
+cudaError_t launch_search_bf16(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
+                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
+                               uint32_t warps_per_block, cudaStream_t s);
 
 // K2t — team walk (T warps per query, T in {2,3,4}); rows <= 1 KB and ef <= 256 only.
 cudaError_t launch_search_team(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,

@@ -24,6 +24,24 @@ cudaError_t launch_search(EHB_SEARCH_ARGS) {
   }
 }
 
+cudaError_t launch_search_bf16(EHB_SEARCH_ARGS) {
+  if (nq == 0) return cudaSuccess;
+  if (!g.vecs16 || !sink.keys) return cudaErrorInvalidValue;
+  switch (g.dpad) {
+    case 32: return launch_search_bf16_d32(EHB_SEARCH_PASS);
+    case 64: return launch_search_bf16_d64(EHB_SEARCH_PASS);
+    case 128: return launch_search_bf16_d128(EHB_SEARCH_PASS);
+    case 256: return launch_search_bf16_d256(EHB_SEARCH_PASS);
+    case 384: return launch_search_bf16_d384(EHB_SEARCH_PASS);
+    case 512: return launch_search_bf16_d512(EHB_SEARCH_PASS);
+    case 768: return launch_search_bf16_d768(EHB_SEARCH_PASS);
+    case 1024: return launch_search_bf16_d1024(EHB_SEARCH_PASS);
+    case 1536: return launch_search_bf16_d1536(EHB_SEARCH_PASS);
+    case 2048: return launch_search_bf16_d2048(EHB_SEARCH_PASS);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
 // ---------------------------------------------------------------------------
 // Row utilities.  Normalisation follows hnswlib's Python binding
 // (normalize_vector): inv = 1 / (sqrt(sum x^2) + 1e-30), one sequential fp32 FMA

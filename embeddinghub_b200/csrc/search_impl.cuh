@@ -4,8 +4,9 @@
 
 namespace ehb {
 
-// One warp walks one query (device body shared by the two kernels below).
-template <int LPV, int NQ, int KPL, bool HASDEL, int UDIV>
+// One warp walks one query (device body shared by the two kernels below).  RowT = __nv_bfloat16 walks the bf16
+// shadow (g.vecs16) and writes the key sink (sink.keys, k = ef: the whole retained set) for the fp32 re-rank.
+template <int LPV, int NQ, int KPL, bool HASDEL, int UDIV, class RowT>
 __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& cfg, const float* __restrict__ queries,
                                             uint32_t nq, uint32_t k, uint32_t ef, const ResultSink& sink,
                                             uint32_t* __restrict__ out_counts, uint32_t* __restrict__ stats,
@@ -14,10 +15,14 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   const uint32_t w = threadIdx.x >> 5;
   const uint32_t q = blockIdx.x * (blockDim.x >> 5) + w;
   if (q >= nq) return;
+  constexpr bool kKeys = !std::is_same<RowT, float>::value;
   WarpCtx c;
-  ctx_init(c, smem + (size_t)w * warp_smem, cfg, g.dpad);
+  ctx_init(c, smem + (size_t)w * warp_smem, cfg, g.dpad, (uint32_t)sizeof(RowT));
   float4 qr[NQ];
-  load_query_regs<LPV, NQ>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
+  if constexpr (kKeys)
+    load_query_regs_bf16<LPV, NQ>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
+  else
+    load_query_regs<LPV, NQ>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
   WalkCounters wc = {0, 0, 0, 0};
   UList<KPL> ul;
   ul_clear<KPL>(ul, ef, c.lane);
@@ -25,12 +30,12 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
     uint32_t cur = g.entry;
     if (c.lane == 0) c.cand_id[0] = cur;
     __syncwarp();
-    eval_candidates<LPV, NQ, UDIV>(c, g.vecs, qr, 1, g.metric);
+    eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, 1, g.metric);
     float curdist = c.cand_dist[0];
     __syncwarp();
     wc.evals = 1;
-    greedy_descent<LPV, NQ, UDIV>(c, g, qr, cur, curdist, g.max_level, 0, wc);
-    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc);
+    greedy_descent<LPV, NQ, UDIV, RowT>(c, g, qr, cur, curdist, g.max_level, 0, wc);
+    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV, RowT>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc);
   }
   // nearest-first output: extract the k closest in ascending order into registers (element i -> lane i & 31,
   // slot i >> 5), then store them to every destination of the sink with coalesced stores
@@ -46,30 +51,38 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
       if ((i >> 5) == (uint32_t)s && (i & 31u) == c.lane) rk[s] = key;
     found++;
   }
+  if constexpr (kKeys) {  // the key sink: raw keys, no labels, no peers
 #pragma unroll
-  for (int s = 0; s < KPL; ++s) {
-    const uint32_t idx = (uint32_t)s * 32u + c.lane;
-    if ((uint32_t)s * 32u < k && idx < k) {
-      const bool ok = rk[s] != kMaxKey;
-      const uint64_t lab = ok ? g.labels[key_id(rk[s])] : 0xFFFFFFFFFFFFFFFFull;
-      const float dist = ok ? key_dist(rk[s]) : INFINITY;
-      const size_t at = (size_t)q * k + idx;
-      for (uint32_t t = 0; t < sink.n; ++t) {
-        sink.labels[t][at] = lab;
-        if (sink.dists[t]) sink.dists[t][at] = dist;
+    for (int s = 0; s < KPL; ++s) {
+      const uint32_t idx = (uint32_t)s * 32u + c.lane;
+      if ((uint32_t)s * 32u < k && idx < k) sink.keys[(size_t)q * k + idx] = rk[s];
+    }
+  } else {
+#pragma unroll
+    for (int s = 0; s < KPL; ++s) {
+      const uint32_t idx = (uint32_t)s * 32u + c.lane;
+      if ((uint32_t)s * 32u < k && idx < k) {
+        const bool ok = rk[s] != kMaxKey;
+        const uint64_t lab = ok ? g.labels[key_id(rk[s])] : 0xFFFFFFFFFFFFFFFFull;
+        const float dist = ok ? key_dist(rk[s]) : INFINITY;
+        const size_t at = (size_t)q * k + idx;
+        for (uint32_t t = 0; t < sink.n; ++t) {
+          sink.labels[t][at] = lab;
+          if (sink.dists[t]) sink.dists[t][at] = dist;
+        }
       }
     }
-  }
-  if (sink.qs) {  // sharded: the warp that completes a slice raises its flag on every peer
-    __threadfence_system();
-    __syncwarp();
-    if (c.lane == 0) {
-      const uint32_t slice = q / sink.qs;
-      const uint32_t size = min(sink.qs, nq - slice * sink.qs);
-      if (atomicAdd(&sink.slice_count[slice], 1u) + 1u == size) {
-        sink.slice_count[slice] = 0;  // ready for the next step (which starts after this kernel)
-        __threadfence_system();       // the other warps fenced before their atomicAdd: fence-fence ordering
-        for (uint32_t t = 1; t < sink.n; ++t) st_release_sys(sink.flags[t] + slice, sink.epoch);
+    if (sink.qs) {  // sharded: the warp that completes a slice raises its flag on every peer
+      __threadfence_system();
+      __syncwarp();
+      if (c.lane == 0) {
+        const uint32_t slice = q / sink.qs;
+        const uint32_t size = min(sink.qs, nq - slice * sink.qs);
+        if (atomicAdd(&sink.slice_count[slice], 1u) + 1u == size) {
+          sink.slice_count[slice] = 0;  // ready for the next step (which starts after this kernel)
+          __threadfence_system();       // the other warps fenced before their atomicAdd: fence-fence ordering
+          for (uint32_t t = 1; t < sink.n; ++t) st_release_sys(sink.flags[t] + slice, sink.epoch);
+        }
       }
     }
   }
@@ -81,40 +94,49 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
 
 // Register budget of the default form: ptxas chooses (16 vectors in flight per warp).  An explicit
 // minBlocksPerSM changes its heuristics, and a register cap below what the 16 loads in flight need serialises
-// the load batches — so none is given.
-template <int LPV, int NQ, int KPL, bool HASDEL>
-__global__ void __launch_bounds__(128) hnsw_search_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries,
-                                                          uint32_t nq, uint32_t k, uint32_t ef,
-                                                          const __grid_constant__ ResultSink sink,
-                                                          uint32_t* __restrict__ out_counts,
-                                                          uint32_t* __restrict__ stats, uint32_t warp_smem) {
-  search_body<LPV, NQ, KPL, HASDEL, 1>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
+// the load batches — so none is given for fp32 rows.  Over bf16 rows the default heuristics leave a few bytes of
+// spills in some shapes; minBlocksPerSM = 1 lets ptxas take the registers instead.
+template <class RowT>
+constexpr int kWalkMinBlocks = std::is_same<RowT, float>::value ? 0 : 1;
+template <int LPV, int NQ, int KPL, bool HASDEL, class RowT>
+__global__ void __launch_bounds__(128, kWalkMinBlocks<RowT>)
+    hnsw_search_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries, uint32_t nq, uint32_t k, uint32_t ef,
+                       const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts,
+                       uint32_t* __restrict__ stats, uint32_t warp_smem) {
+  search_body<LPV, NQ, KPL, HASDEL, 1, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
+}
+
+// Shapes with a dense form (LPV = 8, NQ <= 4, no tombstones).  Over bf16 rows the 96-register budget spills at
+// dpad = 128 with KPL >= 8, so those shapes keep the default form (ehb_index::walk_cfg agrees).
+template <class RowT>
+__host__ __device__ constexpr bool dense_form(int NQ, int KPL) {
+  return std::is_same<RowT, float>::value || NQ < 4 || KPL < 8;
 }
 
 // "Dense" form for big batches of short rows (LPV = 8, d <= 128): 8 vectors in flight per warp instead of 16
 // and a 96-register budget -> 20 resident warps per SM instead of 16 (the visited table shrinks to match,
 // api.cu walk_cfg): with many queries in flight, more warps hide more of each hop's memory latency.
-template <int LPV, int NQ, int KPL>
+template <int LPV, int NQ, int KPL, class RowT>
 __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, WalkCfg cfg,
                                                                    const float* __restrict__ queries, uint32_t nq,
                                                                    uint32_t k, uint32_t ef,
                                                                    const __grid_constant__ ResultSink sink,
                                                                    uint32_t* __restrict__ out_counts,
                                                                    uint32_t* __restrict__ stats, uint32_t warp_smem) {
-  search_body<LPV, NQ, KPL, false, 2>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
+  search_body<LPV, NQ, KPL, false, 2, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
-template <int LPV, int NQ, int KPL, bool HASDEL>
+template <int LPV, int NQ, int KPL, bool HASDEL, class RowT>
 cudaError_t launch_search_t(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
                             uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t wpb,
                             cudaStream_t s) {
-  uint32_t wsm = warp_smem_bytes(cfg, g.dpad);
+  uint32_t wsm = warp_smem_bytes(cfg, g.dpad * (uint32_t)sizeof(RowT));
   size_t smem = (size_t)wsm * wpb;
   dim3 grid((nq + wpb - 1) / wpb), block(32 * wpb);
   void (*kern)(GraphView, WalkCfg, const float*, uint32_t, uint32_t, uint32_t, const ResultSink, uint32_t*, uint32_t*,
-               uint32_t) = hnsw_search_kernel<LPV, NQ, KPL, HASDEL>;
-  if constexpr (LPV == 8 && NQ <= 4 && !HASDEL) {
-    if (cfg.dense) kern = hnsw_search_dense_kernel<LPV, NQ, KPL>;
+               uint32_t) = hnsw_search_kernel<LPV, NQ, KPL, HASDEL, RowT>;
+  if constexpr (LPV == 8 && NQ <= 4 && !HASDEL && dense_form<RowT>(NQ, KPL)) {
+    if (cfg.dense) kern = hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
   }
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
@@ -122,15 +144,16 @@ cudaError_t launch_search_t(const GraphView& g, const WalkCfg& cfg, const float*
   return cudaGetLastError();
 }
 
-template <int LPV, int NQ>
+template <int LPV, int NQ, class RowT = float>
 cudaError_t launch_search_kpl(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t wpb,
                               cudaStream_t s) {
   // (Keeping a whole 2M-neighbour hop in flight per batch needs about 168 registers, which costs occupancy;
   //  batches stay at 16 vectors.)
 #define EHB_KPL(K)                                                                                          \
-  return g.deleted ? launch_search_t<LPV, NQ, K, true>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s) \
-                   : launch_search_t<LPV, NQ, K, false>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s)
+  return g.deleted                                                                                          \
+             ? launch_search_t<LPV, NQ, K, true, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s) \
+             : launch_search_t<LPV, NQ, K, false, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s)
   if (ef <= 64) EHB_KPL(2);
   if (ef <= 128) EHB_KPL(4);
   if (ef <= 256) EHB_KPL(8);
@@ -153,5 +176,16 @@ cudaError_t launch_search_d768(EHB_SEARCH_ARGS);
 cudaError_t launch_search_d1024(EHB_SEARCH_ARGS);
 cudaError_t launch_search_d1536(EHB_SEARCH_ARGS);
 cudaError_t launch_search_d2048(EHB_SEARCH_ARGS);
+// the bf16 walk (search_inst_bf16_*.cu)
+cudaError_t launch_search_bf16_d32(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d64(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d128(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d256(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d384(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d512(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d768(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d1024(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d1536(EHB_SEARCH_ARGS);
+cudaError_t launch_search_bf16_d2048(EHB_SEARCH_ARGS);
 
 }  // namespace ehb

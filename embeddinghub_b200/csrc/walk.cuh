@@ -20,8 +20,15 @@
 //     (Staging every row through TMA makes the walk issue-bound on the
 //      per-lane bulk-copy issue loops at d=128.)
 //   * rows are padded to an exact multiple of the per-lane tile, so the inner
-//     loops carry no bounds checks.
+//     loops carry no bounds checks;
+//   * the walk reads either the fp32 rows or their bf16 shadow (RowT = __nv_bfloat16: the bf16 graph
+//     search, re-ranked in fp32 afterwards).  The query stays fp32 in registers either way and the same
+//     "rows <= 1 KB direct, larger rows TMA" rule applies to the row's bytes.
 #pragma once
+#include <cuda_bf16.h>
+
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ehb {
@@ -36,6 +43,7 @@ struct GraphView {
   uint32_t n, dim, dpad, M, M0, entry;
   int32_t max_level;
   int32_t metric;            // 0 = squared L2, 1 = 1 - dot (IP and cosine)
+  const __nv_bfloat16* vecs16;  // [n][dpad] bf16 shadow of vecs (bf16 graph search only), else nullptr
 };
 
 struct WalkCfg {
@@ -61,6 +69,9 @@ struct ResultSink {
   uint32_t* flags[kMaxSinks];  // [slices] of (parity, this rank) on destination t; unused for t = 0
   uint32_t* slice_count;       // local [slices], zero between steps
   uint32_t n, qs, epoch;       // destinations; queries per slice (0: no flags); value the flags take
+  // bf16 walk only (the "key" sink): [nq][k] retained (ordered distance, internal id) keys, nearest-first,
+  // kMaxKey past the retained count; launch_rerank turns them into results.  Nothing above is written then.
+  uint64_t* keys;
 };
 
 __host__ __device__ inline uint32_t align_up(uint32_t x, uint32_t a) { return (x + a - 1) / a * a; }
@@ -73,8 +84,9 @@ __host__ __device__ inline uint32_t pad_dim(uint32_t dim) {
   return 0;
 }
 
-// Per-warp shared-memory slice; every region offset is a multiple of 128 B.
-__host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t dpad) {
+// Per-warp shared-memory slice; every region offset is a multiple of 128 B.  vbytes: bytes of one row as the
+// walk reads it (dpad * 4 for fp32 rows, dpad * 2 for the bf16 shadow); it sizes the TMA staging ring.
+__host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t vbytes) {
   uint32_t b = 0;
   b += align_up(c.lcap * 8u, 128);
   b += align_up(c.hash_size * 4u, 128);
@@ -82,7 +94,7 @@ __host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t d
   b += 128;  // cand_dist[32]
   b += 128;  // mbarriers (<= 8) + spare
   b += align_up(c.dcap * 8u, 128);  // deleted-candidate queue: hi[dcap] | id[dcap]
-  b += c.staged ? align_up(c.G * c.NG * dpad * 4u, 128) : 0u;
+  b += c.staged ? align_up(c.G * c.NG * vbytes, 128) : 0u;
   return b;
 }
 
@@ -101,13 +113,15 @@ struct WarpCtx {
   uint32_t lane;
 };
 
-__device__ __forceinline__ void ctx_init(WarpCtx& c, unsigned char* base, const WalkCfg& cfg, uint32_t dpad) {
+// esize: bytes per row element (4 = fp32 rows, 2 = bf16 shadow)
+__device__ __forceinline__ void ctx_init(WarpCtx& c, unsigned char* base, const WalkCfg& cfg, uint32_t dpad,
+                                         uint32_t esize = 4u) {
   c.lane = lane_id();
   c.lcap = cfg.lcap;
   c.G = cfg.G;
   c.NG = cfg.NG;
   c.dpad = dpad;
-  c.vbytes = dpad * 4u;
+  c.vbytes = dpad * esize;
   c.hsize = cfg.hash_size;
   unsigned char* p = base;
   c.keys = (uint64_t*)p;
@@ -213,6 +227,77 @@ __device__ __forceinline__ float group_reduce(float acc) {
   return acc;
 }
 
+// ---- bf16 rows -----------------------------------------------------------------------------------------
+// A lane reads its part of a bf16 row in 16-byte chunks of 8 values (one 8-byte chunk of 4 values at
+// dpad = 32).  NQ still counts the fp32 query's float4 registers per lane (dpad == 4 * LPV * NQ), so a lane
+// holds NQ / 2 chunks; chunk j of lane `sub = lane % LPV` is elements 8 * (sub + LPV * j) .. + 7, paired with
+// the query floats in qr[2j] and qr[2j + 1].  At NQ = 1 the layout is the fp32 one.
+template <int NQ>
+struct Bf16Chunks {
+  using T = uint4;
+  static constexpr int N = NQ / 2;
+};
+template <>
+struct Bf16Chunks<1> {
+  using T = uint2;
+  static constexpr int N = 1;
+};
+template <int LPV, int NQ>
+__device__ __forceinline__ void load_query_regs_bf16(float4 (&qr)[NQ], const float* __restrict__ src, uint32_t dim,
+                                                     uint32_t lane) {
+  if constexpr (NQ == 1) {
+    load_query_regs<LPV, 1>(qr, src, dim, lane);
+  } else {
+    uint32_t sub = lane % LPV;
+#pragma unroll
+    for (int t = 0; t < NQ; ++t) {
+      uint32_t e = (sub + LPV * (t >> 1)) * 8u + 4u * (t & 1);
+      float4 v;
+      v.x = e + 0 < dim ? src[e + 0] : 0.f;
+      v.y = e + 1 < dim ? src[e + 1] : 0.f;
+      v.z = e + 2 < dim ? src[e + 2] : 0.f;
+      v.w = e + 3 < dim ? src[e + 3] : 0.f;
+      qr[t] = v;
+    }
+  }
+}
+// two packed bf16 pairs -> four floats (exact: bf16 is the top half of an fp32)
+__device__ __forceinline__ float4 bf16x4_to_f4(uint32_t a, uint32_t b) {
+  return make_float4(__uint_as_float(a << 16), __uint_as_float(a & 0xFFFF0000u), __uint_as_float(b << 16),
+                     __uint_as_float(b & 0xFFFF0000u));
+}
+template <int LPV, int NQ>
+__device__ __forceinline__ void load_vec_regs(typename Bf16Chunks<NQ>::T (&r)[Bf16Chunks<NQ>::N],
+                                              const __nv_bfloat16* __restrict__ row, uint32_t lane) {
+  using CT = typename Bf16Chunks<NQ>::T;
+  const CT* p = (const CT*)row + (lane % LPV);
+#pragma unroll
+  for (int t = 0; t < Bf16Chunks<NQ>::N; ++t) r[t] = p[LPV * t];
+}
+// widened to fp32, then the fp32 chain (fp32 products and accumulation)
+template <int NQ>
+__device__ __forceinline__ float partial_dist(const typename Bf16Chunks<NQ>::T (&v)[Bf16Chunks<NQ>::N],
+                                              const float4 (&qr)[NQ], int metric) {
+  float4 x[NQ];
+  if constexpr (NQ == 1) {
+    x[0] = bf16x4_to_f4(v[0].x, v[0].y);
+  } else {
+#pragma unroll
+    for (int j = 0; j < NQ / 2; ++j) {
+      x[2 * j] = bf16x4_to_f4(v[j].x, v[j].y);
+      x[2 * j + 1] = bf16x4_to_f4(v[j].z, v[j].w);
+    }
+  }
+  return partial_dist<NQ>(x, qr, metric);
+}
+template <class RowT>
+__device__ __forceinline__ const RowT* walk_rows(const GraphView& g) {
+  if constexpr (std::is_same<RowT, float>::value)
+    return g.vecs;
+  else
+    return g.vecs16;
+}
+
 // ---- LPV = 8: direct 128-bit loads, U steps (4 vectors each) in flight ------
 // default U: 64 registers of loads in flight (16 vectors at d <= 128)
 __host__ __device__ constexpr int eval_u(int NQ, int UDIV) {
@@ -247,8 +332,50 @@ __device__ __forceinline__ void eval_direct(WarpCtx& c, const float* __restrict_
   __syncwarp();
 }
 
+// bf16 rows: a load step carries half the bytes, so the same 64 registers of loads hold twice the vectors
+// (capped at the 32 candidates of a hop)
+__host__ __device__ constexpr int eval_u_bf16(int NQ, int UDIV) {
+  return ((NQ <= 4 ? 8 : (NQ <= 8 ? 4 : 2)) / UDIV) > 0 ? (NQ <= 4 ? 8 : (NQ <= 8 ? 4 : 2)) / UDIV : 1;
+}
+template <int NQ, int U>
+__device__ __forceinline__ void eval_direct(WarpCtx& c, const __nv_bfloat16* __restrict__ rows,
+                                            const float4 (&qr)[NQ], uint32_t m, int metric) {
+  using CT = typename Bf16Chunks<NQ>::T;
+  constexpr int NC = Bf16Chunks<NQ>::N;
+  const uint32_t sub = c.lane & 7u, grp = c.lane >> 3;
+  __syncwarp();
+#pragma unroll 1
+  for (uint32_t j0 = 0; j0 < m; j0 += 4 * U) {
+    CT v[U][NC];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (j0 + 4u * u < m) {                          // warp-uniform
+        uint32_t j = min(j0 + 4u * u + grp, m - 1u);  // clamped lanes re-read the last row (same lines)
+        const CT* p = (const CT*)(rows + (size_t)c.cand_id[j] * c.dpad) + sub;
+#pragma unroll
+        for (int t = 0; t < NC; ++t) {
+          if constexpr (NQ == 1)
+            v[u][t] = ld_nc_u2(p + 8 * t);
+          else
+            v[u][t] = ld_nc_u4(p + 8 * t);
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (j0 + 4u * u < m) {
+        uint32_t j = j0 + 4u * u + grp;
+        float acc = group_reduce<8>(partial_dist<NQ>(v[u], qr, metric));
+        if (sub == 0 && j < m) c.cand_dist[j] = metric == 0 ? acc : 1.0f - acc;
+      }
+    }
+  }
+  __syncwarp();
+}
+
 // ---- LPV = 32: TMA bulk staging ring ----------------------------------------
-__device__ __forceinline__ void issue_group(WarpCtx& c, const float* __restrict__ vecs, uint32_t r, uint32_t m) {
+template <class RowT>
+__device__ __forceinline__ void issue_group(WarpCtx& c, const RowT* __restrict__ vecs, uint32_t r, uint32_t m) {
   uint32_t buf = r % c.NG;
   uint32_t first = r * c.G;
   uint32_t cnt = min(c.G, m - first);
@@ -256,11 +383,12 @@ __device__ __forceinline__ void issue_group(WarpCtx& c, const float* __restrict_
   __syncwarp();
   if (c.lane < cnt) {
     uint32_t id = c.cand_id[first + c.lane];
-    bulk_g2s(c.stage + (size_t)(buf * c.G + c.lane) * c.dpad, vecs + (size_t)id * c.dpad, c.vbytes, &c.mbar[buf]);
+    bulk_g2s((RowT*)c.stage + (size_t)(buf * c.G + c.lane) * c.dpad, vecs + (size_t)id * c.dpad, c.vbytes,
+             &c.mbar[buf]);
   }
 }
-template <int NQ>
-__device__ __forceinline__ void eval_staged(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
+template <int NQ, class RowT>
+__device__ __forceinline__ void eval_staged(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
                                             uint32_t m, int metric) {
   const uint32_t rounds = (m + c.G - 1) / c.G;
   const uint32_t pre = min(rounds, c.NG);
@@ -279,11 +407,17 @@ __device__ __forceinline__ void eval_staged(WarpCtx& c, const float* __restrict_
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
-        const float4* s4 = (const float4*)(c.stage + (size_t)(buf * c.G + v) * c.dpad) + c.lane;
-        float4 x[NQ];
+        if constexpr (std::is_same<RowT, float>::value) {
+          const float4* s4 = (const float4*)(c.stage + (size_t)(buf * c.G + v) * c.dpad) + c.lane;
+          float4 x[NQ];
 #pragma unroll
-        for (int t = 0; t < NQ; ++t) x[t] = s4[32 * t];
-        acc[i] = partial_dist<NQ>(x, qr, metric);
+          for (int t = 0; t < NQ; ++t) x[t] = s4[32 * t];
+          acc[i] = partial_dist<NQ>(x, qr, metric);
+        } else {
+          typename Bf16Chunks<NQ>::T x[Bf16Chunks<NQ>::N];
+          load_vec_regs<32, NQ>(x, (const RowT*)c.stage + (size_t)(buf * c.G + v) * c.dpad, c.lane);
+          acc[i] = partial_dist<NQ>(x, qr, metric);
+        }
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
@@ -306,13 +440,17 @@ __device__ __forceinline__ void eval_staged(WarpCtx& c, const float* __restrict_
 
 // cand_id[0..m) -> cand_dist[0..m): distances from the register-held query.  UDIV > 1 halves (…) the
 // load batches kept in flight per warp: fewer registers, more resident warps (the "dense" walk).
-template <int LPV, int NQ, int UDIV = 1>
-__device__ __forceinline__ void eval_candidates(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
+template <int LPV, int NQ, int UDIV = 1, class RowT = float>
+__device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
                                                 uint32_t m, int metric) {
-  if (LPV == 8)
-    eval_direct<NQ, eval_u(NQ, UDIV)>(c, vecs, qr, m, metric);
-  else
+  if (LPV == 8) {
+    if constexpr (std::is_same<RowT, float>::value)
+      eval_direct<NQ, eval_u(NQ, UDIV)>(c, vecs, qr, m, metric);
+    else
+      eval_direct<NQ, eval_u_bf16(NQ, UDIV)>(c, vecs, qr, m, metric);
+  } else {
     eval_staged<NQ>(c, vecs, qr, m, metric);
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -500,7 +638,7 @@ __device__ __forceinline__ uint32_t load_row(const GraphView& g, uint32_t node, 
 
 // hnswlib searchKnn's upper-layer descent: at each level move to the closest
 // neighbour until no neighbour improves.
-template <int LPV, int NQ, int UDIV = 1>
+template <int LPV, int NQ, int UDIV = 1, class RowT = float>
 __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], uint32_t& cur,
                                                float& curdist, int from_level, int to_level_excl,
                                                WalkCounters& wc) {
@@ -517,7 +655,7 @@ __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, c
       if (nb != kInvalid) c.cand_id[__popc(mask & lanemask_lt())] = nb;
       __syncwarp();
       wc.evals += m;
-      eval_candidates<LPV, NQ, UDIV>(c, g.vecs, qr, m, g.metric);
+      eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
       float bd = c.lane < m ? c.cand_dist[c.lane] : INFINITY;
       uint32_t bl = c.lane;
 #pragma unroll
@@ -590,7 +728,7 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 
 // HASDEL = false compiles every trace of the tombstone machinery out (an index without tombstones runs
 // exactly the plain loop: the extra live registers would cost the 16-vector load batches their overlap).
-template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1>
+template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
@@ -636,13 +774,13 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       const uint32_t unsure = (HASDEL && del) ? __reduce_or_sync(0xffffffffu, (is_new && o) ? (1u << pos) : 0u) : 0u;
       __syncwarp();
       wc.evals += m;
-      eval_candidates<LPV, NQ, UDIV>(c, g.vecs, qr, m, g.metric);
+      eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
       // the speculative row has arrived by now: pull its neighbours' vectors towards L2 while this hop's
       // candidates are inserted (rows <= 1 KB only; a wrong guess costs bandwidth, not correctness)
       if (PREFETCH && LPV == 8 && c.prefetch && spec_row != kInvalid) {
-        const char* pv = (const char*)(g.vecs + (size_t)spec_row * g.dpad);
+        const char* pv = (const char*)(walk_rows<RowT>(g) + (size_t)spec_row * g.dpad);
 #pragma unroll
-        for (int b = 0; b < NQ * 8 * 16; b += 128) prefetch_l2(pv + b);
+        for (int b = 0; b < NQ * 8 * 16 * (int)sizeof(RowT) / 4; b += 128) prefetch_l2(pv + b);
       }
       uint32_t myhi = 0xFFFFFFFFu, myid = kInvalid;
       if (c.lane < m) myhi = f2ord(c.cand_dist[c.lane]), myid = c.cand_id[c.lane];

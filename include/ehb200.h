@@ -83,7 +83,10 @@ typedef struct ehb_stats {
   uint64_t hops_base;
   uint64_t dist_evals;
   uint64_t visited_overflow; /* queries whose visited table filled up          */
-  uint64_t algorithmic_bytes; /* hops_upper*4M + hops_base*8M + evals*4d + Q*4d */
+  /* fp32 search: hops_upper*4M + hops_base*8M + evals*4d + Q*4d;
+   * bf16 search: hops_upper*4M + hops_base*8M + evals*2d + Q*4d + reranked*4d, reranked = the keys the walk
+   * retained and the fp32 re-rank read (min(max(ef, k), reachable live points) per query) */
+  uint64_t algorithmic_bytes;
   /* index shape */
   uint64_t size, capacity, upper_rows;
   uint32_t dim, M, max_level, entry_point;
@@ -152,6 +155,22 @@ int ehb_index_search(ehb_index* ix, uint64_t nq, const float* queries_host, uint
                      uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
 int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k, uint32_t ef,
                          uint64_t* out_labels_dev, float* out_dists_dev, uint32_t* out_counts_dev, void* stream);
+/* The same search at a chosen precision; ehb_index_search(_dev) is exactly the _ex form with EHB_FP32, and an
+ * unknown precision fails with EHB_ERR_INVALID.  EHB_BF16 walks the same graph with hnswlib's searchKnn order and
+ * stop rule, but evaluates every distance between the fp32 query and the bf16 copy of the row (widened to fp32,
+ * fp32 accumulation); the walk keeps its whole result set (max(ef, k) entries), which is re-ranked with the
+ * exact path's canonical fp32 arithmetic over the fp32 rows.  So every returned distance is bit-identical to the
+ * exact distance of that id, ties go by internal id, and only the set the walk retains can differ from the fp32
+ * walk's.  It always runs one warp per query (the multi-warp team walk reads fp32 rows only).  Tombstones,
+ * padding, counts and cosine normalisation behave as in the fp32 search.  The first bf16 search (graph or brute
+ * force) creates the index's bf16 copy of its rows (2 * dim-padded bytes per vector), which every later add,
+ * update and compaction keeps current; an index that never runs one allocates none of it.
+ * ehb_index_last_kernel_ms covers the walk and the re-rank. */
+int ehb_index_search_ex(ehb_index* ix, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef, int precision,
+                        uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
+int ehb_index_search_ex_dev(ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k, uint32_t ef,
+                            int precision, uint64_t* out_labels_dev, float* out_dists_dev, uint32_t* out_counts_dev,
+                            void* stream);
 
 /* hnswlib BruteforceSearch (not used by the reference; the exact path named by
  * the north star).  EHB_FP32 is exact with a defined total order (distance asc,
@@ -235,6 +254,9 @@ int ehb_sharded_compact(ehb_sharded* sh); /* ehb_index_compact on every shard, c
 int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef);
 int ehb_sharded_search(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef,
                        uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
+/* ehb_index_search_ex on every shard, then the same merge (ehb_sharded_search is the EHB_FP32 form). */
+int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef,
+                          int precision, uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, int precision,
                                   uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
 
@@ -259,7 +281,8 @@ int ehb_exchange_merge_dev(ehb_exchange* ex, float* out_dists_dev, uint64_t* out
 /* The fused step for graph searches (replaces begin + ehb_index_search_dev + merge_dev): the walk kernel's
  * epilogue stores each query's top-k into every peer's receive buffer (coalesced stores over NVLink, overlapping
  * the rest of the walk) and raises per-slice flags; one kernel then waits for the peers' flags and merges.
- * shard_counts_dev ([nq], this shard's hit counts) may be NULL. */
+ * shard_counts_dev ([nq], this shard's hit counts) may be NULL.  This step walks fp32 rows only (there is no
+ * bf16 form: a bf16 walk hands its retained set to a re-rank kernel rather than to the peers). */
 int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
                             uint32_t ef, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
                             uint32_t* shard_counts_dev, void* stream);

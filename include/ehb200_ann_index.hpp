@@ -9,7 +9,8 @@
 //     same type for capacity errors, which the reference lets propagate);
 //   * approx_nearest returns the keys that exist when fewer than `num` points are
 //     stored (index.cc:42-50 pops `num` entries regardless — undefined behaviour);
-//   * a batched approx_nearest_batch() is added (docs/inference.md:14-22).
+//   * a batched approx_nearest_batch() is added (docs/inference.md:14-22), with an optional ef and precision
+//     (EHB_BF16: the graph walk over bf16 rows, re-ranked in fp32; ehb_index_search_ex).
 #pragma once
 #include <cstdint>
 #include <memory>
@@ -61,7 +62,8 @@ class ANNIndex {
   }
 
   std::vector<std::vector<std::string>> approx_nearest_batch(const std::vector<std::vector<float>>& values,
-                                                             size_t num, uint32_t ef = 0) const {
+                                                             size_t num, uint32_t ef = 0,
+                                                             int precision = EHB_FP32) const {
     std::vector<std::vector<std::string>> out(values.size());
     if (num == 0 || values.empty()) return out;
     std::vector<float> q(values.size() * dims_);
@@ -71,7 +73,8 @@ class ANNIndex {
     }
     std::vector<uint64_t> labels(values.size() * num);
     std::vector<uint32_t> counts(values.size());
-    check(ehb_index_search(ix_, values.size(), q.data(), (uint32_t)num, ef, labels.data(), nullptr, counts.data()));
+    check(ehb_index_search_ex(ix_, values.size(), q.data(), (uint32_t)num, ef, precision, labels.data(), nullptr,
+                              counts.data()));
     for (size_t i = 0; i < values.size(); ++i)
       for (uint32_t j = 0; j < counts[i]; ++j) out[i].push_back(label_to_key_.at(labels[i * num + j]));
     return out;
