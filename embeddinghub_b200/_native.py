@@ -86,6 +86,7 @@ SYMBOLS = {
     "ehb_index_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce_dev": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP, _VP]),
     "ehb_index_stats": (C.c_int, [_VP, C.POINTER(Stats)]),
+    "ehb_index_screen_stats": (C.c_int, [_VP, C.POINTER(_U64), C.POINTER(_U64)]),
     "ehb_index_last_kernel_ms": (C.c_int, [_VP, C.POINTER(C.c_float)]),
     "ehb_index_last_kernel_name": (C.c_int, [_VP, C.c_char_p, _U32]),
     "ehb_index_export_graph": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(_U32), C.POINTER(_I32)]),
@@ -282,7 +283,11 @@ class NativeIndex:
     def stats(self):
         s = Stats()
         check(lib().ehb_index_stats(self._h, C.byref(s)))
-        return {f: getattr(s, f) for f, _ in Stats._fields_}
+        out = {f: getattr(s, f) for f, _ in Stats._fields_}
+        screened, fp32_rows = C.c_uint64(), C.c_uint64()
+        check(lib().ehb_index_screen_stats(self._h, C.byref(screened), C.byref(fp32_rows)))
+        out["screened_evals"], out["fp32_row_reads"] = screened.value, fp32_rows.value
+        return out
 
     def last_kernel_ms(self):
         ms = C.c_float()

@@ -41,7 +41,34 @@ ehb::GraphView ehb_index::view() const {
   g.max_level = max_level;
   g.metric = metric == EHB_L2 ? 0 : 1;
   g.vecs16 = nullptr;
+  g.screen_c = 0.f;
   return g;
+}
+
+// The fp32 walk's bf16 screen (walk.cuh beam_search) applies to staged rows (> 1 KB, dpad <= 1536) under 1 - dot.
+// By default it runs for batches of at least kScreenMinBatchPerSm queries per SM: those keep the walk bound by DRAM
+// bandwidth, which the screen relieves; a smaller batch is bound by each warp's chain of memory round trips, to
+// which the screen adds one per hop.
+bool ehb_index::walk_screens(uint64_t nq) const {
+  if (o_walk_screen == 0 || metric == EHB_L2 || dpad * 4u <= 1024u || dpad > 128u * ehb::kScreenMaxNQ) return false;
+  return o_walk_screen > 0 || nq >= (uint64_t)ehb::kScreenMinBatchPerSm * sms;
+}
+
+// The screen is an optimisation: when the shadow does not fit next to the index, the walk runs unscreened.
+int ehb_index::try_screen_shadow() {
+  size_t fr = 0, tot = 0;
+  const uint64_t need = std::max<uint64_t>(cap, 1) * (dpad * 2ull + 4ull) + (256ull << 20);
+  bool ok = cudaMemGetInfo(&fr, &tot) == cudaSuccess && fr >= need;
+  if (ok && create_shadow() != EHB_OK) {
+    drop_shadow();
+    ok = false;
+  }
+  if (!ok) {
+    (void)cudaGetLastError();
+    ehb::g_err.clear();
+    screen_no_room = true;
+  }
+  return EHB_OK;
 }
 
 // ef_eff: beam width; smem_list: capacity of the shared-memory key list (0 for plain searches);
@@ -601,14 +628,16 @@ int ehb_index::compact() {
 
 // Searches link pending points lazily, and the first bf16 search creates the bf16 shadow; both need the writer
 // side of the lock.  Another writer may run between the unlock and the lock, so the state is checked again.
-int ehb_index::ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16) {
-  while (needs_build() || (bf16 && !shadow)) {
+int ehb_index::ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16, bool screen) {
+  auto screen_wants_shadow = [&] { return screen && !shadow && !screen_no_room; };
+  while (needs_build() || (bf16 && !shadow) || screen_wants_shadow()) {
     lk.unlock();
     int rc;
     {
       std::unique_lock<ehb::RwLock> x(rw);
       rc = build();
       if (rc == EHB_OK && bf16) rc = create_shadow();
+      if (rc == EHB_OK && screen_wants_shadow()) rc = try_screen_shadow();
     }
     lk.lock();
     if (rc != EHB_OK) return rc;
@@ -687,6 +716,7 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
   if (bf16) team = 1;                                       // the team walk reads fp32 rows only
   ehb::WalkCfg cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16);
+  const bool screen = !bf16 && team == 1 && shadow && walk_screens(nq);
   if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
   const float* q = dq;
   if (metric == EHB_COSINE) {
@@ -694,8 +724,8 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     CU(ehb::launch_pad_rows(dq, sl->q_norm.p, nq, dim, dim, true, s));
     q = sl->q_norm.p;
   }
-  CU(sl->stats.grow(nq * 4, 0, -1, s));
-  CU(sl->stat_sum.grow(4, 0, 0, s));
+  CU(sl->stats.grow(nq * ehb::kStatWords, 0, -1, s));
+  CU(sl->stat_sum.grow(ehb::kStatWords, 0, 0, s));
   if (bf16) {
     CU(sl->q_pad.grow(nq * dpad, 0, -1, s));
     CU(sl->walk_keys.grow(nq * ef_eff, 0, -1, s));
@@ -727,7 +757,13 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     } else if (pushed) {
       *pushed = true;
     }
-    CU(ehb::launch_search(view(), cfg, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, wpb, s));
+    ehb::GraphView g = view();
+    if (screen) {
+      g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
+      const double c = ehb::screen_constant(dpad);
+      g.screen_c = (double)(float)c >= c ? (float)c : std::nextafter((float)c, INFINITY);
+    }
+    CU(ehb::launch_search(g, cfg, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, wpb, s));
   }
   CU(cudaEventRecord(sl->ev1, s));
   sl->last_nq = nq;
@@ -1087,7 +1123,7 @@ int ehb_index_search_ex(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, 
   if (k == 0 || nq == 0) return EHB_OK;
   if (std::max(ef ? ef : ix->ef, k) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
   // before queueing: a waiting follower must never block a writer the leader needs
-  RET(ix->ensure_built(_g, precision == EHB_BF16));
+  RET(ix->ensure_built(_g, precision == EHB_BF16, precision == EHB_FP32 && ix->walk_screens(nq)));
   if (ix->o_combine && nq <= ehb::kCombineMaxCall)
     return search_host_combined(ix, nq, q, k, ef ? ef : ix->ef, precision, ol, od, oc);
   return search_host_direct(ix, nq, q, k, ef, precision, ol, od, oc);
@@ -1103,7 +1139,7 @@ int ehb_index_search_ex_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_
   if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (nq && (!dq || !dl)) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
-  RET(ix->ensure_built(_g, precision == EHB_BF16));
+  RET(ix->ensure_built(_g, precision == EHB_BF16, precision == EHB_FP32 && ix->walk_screens(nq)));
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = stream ? (cudaStream_t)stream : sl->stream;
@@ -1123,7 +1159,7 @@ int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint3
   ENTER_S(ix);
   if (!dq || !sink || !sink->n || !sink->labels[0]) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
-  RET(ix->ensure_built(_g));
+  RET(ix->ensure_built(_g, false, ix->walk_screens(nq)));
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = stream ? stream : sl->stream;
@@ -1164,34 +1200,50 @@ int ehb_index_search_bruteforce_dev(ehb_index* ix, uint64_t nq, const float* dq,
   return ix->bruteforce_dev(nq, dq, k, precision, dl, dd, dc, stream ? (cudaStream_t)stream : ix->stream);
 }
 
+// Caller holds last_mu: the counters of the last graph search, summed once (false when there is none)
+static int last_walk_sums(ehb_index* ix, bool* have) {
+  ehb::SearchSlot* sl = ix->last_slot;
+  *have = sl && !ix->last_was_brute && sl->last_nq;
+  if (!*have || ix->last_sum_valid) return EHB_OK;
+  CU(cudaEventSynchronize(sl->ev1));
+  CU(ehb::launch_sum_stats(sl->stats.p, (uint32_t)sl->last_nq, sl->stat_sum.p, ix->stream));
+  CU(cudaMemcpyAsync(ix->last_sum, sl->stat_sum.p, sizeof(ix->last_sum), cudaMemcpyDeviceToHost, ix->stream));
+  ix->last_reranked = 0;
+  std::vector<uint32_t> cnt(sl->last_bf16 ? sl->last_nq : 0);
+  if (sl->last_bf16)
+    CU(cudaMemcpyAsync(cnt.data(), sl->walk_counts.p, sl->last_nq * 4, cudaMemcpyDeviceToHost, ix->stream));
+  CU(cudaStreamSynchronize(ix->stream));
+  for (uint32_t c : cnt) ix->last_reranked += c;
+  ix->last_sum_valid = true;
+  return EHB_OK;
+}
+// fp32 rows the last graph walk read: every evaluation but the screened ones, plus the screen's survivors (none
+// for a bf16 walk)
+static uint64_t last_fp32_rows(const ehb_index* ix) {
+  return ix->last_slot->last_bf16 ? 0 : ix->last_sum[2] - ix->last_sum[4] + ix->last_sum[5];
+}
+
 int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
   ENTER_S(ix);
   if (!out) return fail(EHB_ERR_INVALID, "null out");
   std::memset(out, 0, sizeof(*out));
   {
     std::lock_guard<std::mutex> g(ix->last_mu);
-    ehb::SearchSlot* sl = ix->last_slot;
-    if (sl && !ix->last_was_brute && sl->last_nq) {
-      if (!ix->last_sum_valid) {
-        CU(cudaEventSynchronize(sl->ev1));
-        CU(ehb::launch_sum_stats(sl->stats.p, (uint32_t)sl->last_nq, sl->stat_sum.p, ix->stream));
-        CU(cudaMemcpyAsync(ix->last_sum, sl->stat_sum.p, 32, cudaMemcpyDeviceToHost, ix->stream));
-        ix->last_reranked = 0;
-        std::vector<uint32_t> cnt(sl->last_bf16 ? sl->last_nq : 0);
-        if (sl->last_bf16)
-          CU(cudaMemcpyAsync(cnt.data(), sl->walk_counts.p, sl->last_nq * 4, cudaMemcpyDeviceToHost, ix->stream));
-        CU(cudaStreamSynchronize(ix->stream));
-        for (uint32_t c : cnt) ix->last_reranked += c;
-        ix->last_sum_valid = true;
-      }
+    bool have = false;
+    RET(last_walk_sums(ix, &have));
+    if (have) {
+      ehb::SearchSlot* sl = ix->last_slot;
       out->queries = sl->last_nq;
       out->hops_upper = ix->last_sum[0];
       out->hops_base = ix->last_sum[1];
       out->dist_evals = ix->last_sum[2];
       out->visited_overflow = ix->last_sum[3];
-      // a bf16 walk reads 2 bytes per element, and its re-rank reads the fp32 rows of the retained keys
+      // A bf16 walk reads 2 bytes per element, and its re-rank reads the fp32 rows of the retained keys.  A
+      // screened fp32 walk reads 2 bytes per element of every screened candidate, and 4 of the fp32 rows it read.
+      const uint64_t screened = ix->last_sum[4];
       out->algorithmic_bytes = out->hops_upper * 4ull * ix->M + out->hops_base * 4ull * ix->M0 +
-                               out->dist_evals * (sl->last_bf16 ? 2ull : 4ull) * ix->dim +
+                               (sl->last_bf16 ? out->dist_evals * 2ull : last_fp32_rows(ix) * 4ull + screened * 2ull) *
+                                   ix->dim +
                                out->queries * 4ull * ix->dim + ix->last_reranked * 4ull * ix->dim;
     }
   }
@@ -1203,11 +1255,23 @@ int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
   out->max_level = ix->max_level < 0 ? 0 : (uint32_t)ix->max_level;
   out->entry_point = ix->entry;
   out->device_bytes = ix->vecs.bytes() + ix->labels.bytes() + ix->levels.bytes() + ix->deleted.bytes() +
-                      ix->links0.bytes() + ix->up_off.bytes() + ix->links_up.bytes() + ix->up_owner.bytes();
+                      ix->links0.bytes() + ix->up_off.bytes() + ix->links_up.bytes() + ix->up_owner.bytes() +
+                      ix->x_bf16.bytes() + ix->x_norm.bytes();
   out->deleted = ix->n_deleted;
   out->combined_batches = ix->combined_batches.load();
   out->combined_queries = ix->combined_queries.load();
   out->metric = (uint32_t)ix->metric;
+  return EHB_OK;
+}
+
+int ehb_index_screen_stats(ehb_index* ix, uint64_t* screened_evals, uint64_t* fp32_row_reads) {
+  ENTER_S(ix);
+  if (!screened_evals || !fp32_row_reads) return fail(EHB_ERR_INVALID, "null out");
+  std::lock_guard<std::mutex> g(ix->last_mu);
+  bool have = false;
+  RET(last_walk_sums(ix, &have));
+  *screened_evals = have ? ix->last_sum[4] : 0;
+  *fp32_row_reads = have ? last_fp32_rows(ix) : 0;
   return EHB_OK;
 }
 
@@ -1250,6 +1314,9 @@ int ehb_index_set_option(ehb_index* ix, const char* name, int64_t value) {
     ix->o_bf16_unfused = value != 0;
   } else if (o == "walk_prefetch") {
     ix->o_walk_prefetch = value != 0;
+  } else if (o == "walk_screen") {
+    ix->o_walk_screen = value < 0 ? -1 : (value ? 1 : 0);
+    ix->screen_no_room = false;
   } else if (o == "combine") {
     ix->o_combine = value != 0;
   } else {

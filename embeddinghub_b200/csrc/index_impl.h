@@ -191,6 +191,7 @@ constexpr uint32_t kCombineMaxCall = 256;  // host searches up to this many quer
 constexpr uint32_t kCombineMaxBatch = 8192;
 constexpr uint32_t kCombineLeaders = 2;    // batches in flight (copies of one overlap the walk of the other)
 constexpr uint32_t kDeletedQueue = 64;     // side queue of tombstoned candidates per walking warp
+constexpr uint32_t kScreenMinBatchPerSm = 4;  // default fp32 walk screen: batches of >= 4 queries per SM
 
 }  // namespace ehb
 
@@ -240,7 +241,7 @@ struct ehb_index {
   std::mutex last_mu;
   ehb::SearchSlot* last_slot = nullptr;  // graph search (counters + events)
   bool last_was_brute = false, timed = false;
-  unsigned long long last_sum[4] = {0, 0, 0, 0};
+  unsigned long long last_sum[ehb::kStatWords] = {};
   unsigned long long last_reranked = 0;  // keys the bf16 re-rank read (0 for an fp32 search)
   bool last_sum_valid = false;
 
@@ -283,6 +284,11 @@ struct ehb_index {
   // L2 prefetch of the speculated next hop's vectors (rows <= 1 KB).  Off: already-visited neighbours and wrong
   // guesses are fetched too, which adds DRAM traffic to a walk that is bound by DRAM traffic.
   bool o_walk_prefetch = false;
+  // fp32 walk screen (walk.cuh beam_search): -1 = automatic (walk_screens), 0 = off, 1 = on for every batch it applies
+  // to.  It needs the bf16 shadow; when there was no room for it the walk runs unscreened (screen_no_room, cleared
+  // when the option is set again).
+  int o_walk_screen = -1;
+  bool screen_no_room = false;
 
   std::default_random_engine level_rng;
 
@@ -305,7 +311,11 @@ struct ehb_index {
   int compact();
   bool needs_build() const { return n_linked != n || !pending_updates.empty(); }
   // (re-)take the writer side until the graph is built and, with bf16, the shadow exists
-  int ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16 = false);
+  // screen: the fp32 walk of this batch wants the bf16 shadow (walk_screens); it is created if it fits
+  int ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16 = false, bool screen = false);
+  // whether an fp32 one-warp walk of nq queries screens on the bf16 shadow (given that the shadow exists)
+  bool walk_screens(uint64_t nq) const;
+  int try_screen_shadow();
   int ensure_shadow(std::shared_lock<ehb::RwLock>& lk);
   int create_shadow();
   void drop_shadow();

@@ -13,7 +13,9 @@ constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved
 constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
 
 // K2 — batched k-NN graph walk (hnswlib searchKnn).  ef >= k, cfg.lcap >= ef.
-// stats: [nq][4] u32 = hops_upper, hops_base, evals, overflow.
+// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.vecs16
+// set (metric 1, rows > 1 KB) the walk screens candidates on the bf16 shadow (walk.cuh beam_search).
+constexpr uint32_t kStatWords = 8;
 cudaError_t launch_search(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
                           uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                           uint32_t warps_per_block, cudaStream_t s);
@@ -37,7 +39,8 @@ cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, ui
 // copy [n][dim] -> [n][dpad] with zero padding (and optional normalisation)
 cudaError_t launch_pad_rows(const float* in, float* out, uint64_t n, uint32_t dim, uint32_t dpad, bool normalize,
                             cudaStream_t s);
-cudaError_t launch_sum_stats(const uint32_t* stats, uint32_t nq, unsigned long long* out4, cudaStream_t s);
+// sums the per-query stats into out[6] (the overflow word counts queries)
+cudaError_t launch_sum_stats(const uint32_t* stats, uint32_t nq, unsigned long long* out, cudaStream_t s);
 
 // K1 — exact fp32 brute force with canonical arithmetic.
 struct BruteScratch {

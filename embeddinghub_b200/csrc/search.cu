@@ -81,30 +81,24 @@ cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, ui
   return launch_pad_rows(in, out, n, dim, out_stride, true, s);
 }
 
-__global__ void sum_stats_kernel(const uint32_t* __restrict__ stats, uint32_t nq, unsigned long long* out4) {
-  unsigned long long a = 0, b = 0, c = 0, d = 0;
+// per query: hops_upper, hops_base, evals, overflow flag, screened, survivors, 0, 0 -> sums (overflow: queries)
+__global__ void sum_stats_kernel(const uint32_t* __restrict__ stats, uint32_t nq, unsigned long long* out) {
+  unsigned long long a[kStatWords] = {};
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += gridDim.x * blockDim.x) {
-    uint4 s = ((const uint4*)stats)[i];
-    a += s.x, b += s.y, c += s.z, d += s.w ? 1 : 0;
+    const uint4 s = ((const uint4*)stats)[2 * i], t = ((const uint4*)stats)[2 * i + 1];
+    a[0] += s.x, a[1] += s.y, a[2] += s.z, a[3] += s.w ? 1 : 0, a[4] += t.x, a[5] += t.y;
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-    c += __shfl_xor_sync(0xffffffffu, c, o);
-    d += __shfl_xor_sync(0xffffffffu, d, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&out4[0], a);
-    atomicAdd(&out4[1], b);
-    atomicAdd(&out4[2], c);
-    atomicAdd(&out4[3], d);
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(0xffffffffu, a[j], o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&out[j], a[j]);
   }
 }
 
-cudaError_t launch_sum_stats(const uint32_t* stats, uint32_t nq, unsigned long long* out4, cudaStream_t s) {
-  cudaError_t e = cudaMemsetAsync(out4, 0, 4 * sizeof(unsigned long long), s);
+cudaError_t launch_sum_stats(const uint32_t* stats, uint32_t nq, unsigned long long* out, cudaStream_t s) {
+  cudaError_t e = cudaMemsetAsync(out, 0, kStatWords * sizeof(unsigned long long), s);
   if (e != cudaSuccess) return e;
-  if (nq) sum_stats_kernel<<<64, 256, 0, s>>>(stats, nq, out4);
+  if (nq) sum_stats_kernel<<<64, 256, 0, s>>>(stats, nq, out);
   return cudaGetLastError();
 }
 

@@ -88,7 +88,10 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   }
   if (c.lane == 0) {
     if (out_counts) out_counts[q] = found;
-    if (stats) ((uint4*)stats)[q] = make_uint4(wc.hops_upper, wc.hops_base, wc.evals, wc.overflow);
+    if (stats) {
+      ((uint4*)stats)[2 * q] = make_uint4(wc.hops_upper, wc.hops_base, wc.evals, wc.overflow);
+      ((uint4*)stats)[2 * q + 1] = make_uint4(wc.screened, wc.survivors, 0u, 0u);
+    }
   }
 }
 

@@ -176,7 +176,10 @@ __global__ void __launch_bounds__(T * 32, (T == 4 && U * NQ >= 16) ? 3 : 7) hnsw
     }
     if (lane == 0) {
       if (out_counts) out_counts[q] = found;
-      if (stats) ((uint4*)stats)[q] = make_uint4(misc[2], misc[3], misc[4], ovf_any ? 1u : 0u);
+      if (stats) {  // (the team walk does not screen)
+        ((uint4*)stats)[2 * q] = make_uint4(misc[2], misc[3], misc[4], ovf_any ? 1u : 0u);
+        ((uint4*)stats)[2 * q + 1] = make_uint4(0u, 0u, 0u, 0u);
+      }
     }
   }
 }

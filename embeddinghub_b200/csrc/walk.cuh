@@ -43,8 +43,22 @@ struct GraphView {
   uint32_t n, dim, dpad, M, M0, entry;
   int32_t max_level;
   int32_t metric;            // 0 = squared L2, 1 = 1 - dot (IP and cosine)
-  const __nv_bfloat16* vecs16;  // [n][dpad] bf16 shadow of vecs (bf16 graph search only), else nullptr
+  // [n][dpad] bf16 shadow of vecs, else nullptr.  The bf16 graph search walks it; the fp32 walk (metric 1, staged
+  // rows) screens candidates on it when it is set (beam_search).
+  const __nv_bfloat16* vecs16;
+  float screen_c;  // fp32 screen: relative error constant of the bound (screen_constant), rounded up
 };
+
+// The fp32 walk's screen (beam_search, DESIGN.md §9).  For b = RN_bf16(x) and any fp32 summation order of the
+// dpad terms, the walk's dot product P^ and the screen's dot product E^ over b satisfy
+//   |P^ - E^| <= (2^-8 + (2 + 2^-8) g) * S + A,   g = n 2^-24 / (1 - n 2^-24),  S = sum |q_i| |b_i|,
+// A covering subnormal inputs and products (flushed or not).  The screen computes S^ >= (1 - g) S in fp32 as well,
+// so the constant is divided by (1 - g), then padded by 2^-20 for the rounding of the constant itself.
+constexpr uint32_t kScreenMaxNQ = 12;  // staged rows of dpad 384 .. 1536 (LPV = 32, NQ = dpad / 128)
+__host__ __device__ inline double screen_constant(uint32_t n) {
+  const double u = 1.0 / 256.0, e = n * 0x1p-24, g = e / (1.0 - e);
+  return (u + (2.0 + u) * g) / (1.0 - g) * (1.0 + 0x1p-20);
+}
 
 struct WalkCfg {
   uint32_t lcap;       // shared-memory key list capacity (0 = none; cold paths only)
@@ -374,18 +388,23 @@ __device__ __forceinline__ void eval_direct(WarpCtx& c, const __nv_bfloat16* __r
 }
 
 // ---- LPV = 32: TMA bulk staging ring ----------------------------------------
+// group r of G rows (vbytes each) of cand_id[0..m) -> ring buffer r % NG
 template <class RowT>
-__device__ __forceinline__ void issue_group(WarpCtx& c, const RowT* __restrict__ vecs, uint32_t r, uint32_t m) {
+__device__ __forceinline__ void issue_rows(WarpCtx& c, const RowT* __restrict__ vecs, uint32_t r, uint32_t m,
+                                           uint32_t G, uint32_t vbytes) {
   uint32_t buf = r % c.NG;
-  uint32_t first = r * c.G;
-  uint32_t cnt = min(c.G, m - first);
-  if (c.lane == 0) mbar_arrive_expect_tx(&c.mbar[buf], cnt * c.vbytes);
+  uint32_t first = r * G;
+  uint32_t cnt = min(G, m - first);
+  if (c.lane == 0) mbar_arrive_expect_tx(&c.mbar[buf], cnt * vbytes);
   __syncwarp();
   if (c.lane < cnt) {
     uint32_t id = c.cand_id[first + c.lane];
-    bulk_g2s((RowT*)c.stage + (size_t)(buf * c.G + c.lane) * c.dpad, vecs + (size_t)id * c.dpad, c.vbytes,
-             &c.mbar[buf]);
+    bulk_g2s((RowT*)c.stage + (size_t)(buf * G + c.lane) * c.dpad, vecs + (size_t)id * c.dpad, vbytes, &c.mbar[buf]);
   }
+}
+template <class RowT>
+__device__ __forceinline__ void issue_group(WarpCtx& c, const RowT* __restrict__ vecs, uint32_t r, uint32_t m) {
+  issue_rows(c, vecs, r, m, c.G, c.vbytes);
 }
 template <int NQ, class RowT>
 __device__ __forceinline__ void eval_staged(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
@@ -451,6 +470,97 @@ __device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restri
   } else {
     eval_staged<NQ>(c, vecs, qr, m, metric);
   }
+}
+
+// ---- fp32 walk: the bf16 screen (LPV = 32, metric 1) -----------------------------------------------------
+template <int NQ>
+__device__ __forceinline__ float partial_abs_dot(const float4 (&v)[NQ], const float4 (&qr)[NQ]) {
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll
+  for (int t = 0; t < NQ; ++t) {
+    a0 = fmaf(fabsf(qr[t].x), fabsf(v[t].x), a0);
+    a1 = fmaf(fabsf(qr[t].y), fabsf(v[t].y), a1);
+    a2 = fmaf(fabsf(qr[t].z), fabsf(v[t].z), a2);
+    a3 = fmaf(fabsf(qr[t].w), fabsf(v[t].w), a3);
+  }
+  return (a0 + a1) + (a2 + a3);
+}
+// The bf16 shadow rows of cand_id[0..m) go through the fp32 walk's staging ring (twice the rows per group: the same
+// bytes) and are read in the fp32 lane layout (8 bytes = the 4 values of chunk lane + 32 t), so the fp32 query
+// registers serve both passes.  Per candidate the warp computes E^ (the fp32 chain over the bf16 row) and
+// S^ = sum |q| |b|, and from them L = RD(RD(1 - E^) - B), B = RU(sc S^ + babs): a lower bound on the distance
+// RN(1 - P^) of the fp32 pass (screen_constant).  A candidate with f2ord(L) >= worst_hi (the hop-start worst of a
+// full result set, which only shrinks within the hop) cannot be admitted and is dropped; a non-finite L keeps it.
+// The survivors move to the front of cand_id in their order, and their count is returned.  `unsure` (a bit per
+// cand_id position) moves with them.
+template <int NQ>
+__device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const __nv_bfloat16* __restrict__ rows,
+                                                  const float4 (&qr)[NQ], uint32_t m, float sc, float babs,
+                                                  uint32_t worst_hi, uint32_t& unsure) {
+  constexpr int SV = NQ >= 12 ? 2 : 4;  // staged rows per math step (two at dpad 1536: no spills)
+  const uint32_t G = min(2u * c.G, 32u), vbytes = c.dpad * 2u;
+  const uint32_t rounds = (m + G - 1) / G;
+  const uint32_t pre = min(rounds, c.NG);
+  fence_proxy_async();
+  for (uint32_t r = 0; r < pre; ++r) issue_rows(c, rows, r, m, G, vbytes);
+#pragma unroll 1
+  for (uint32_t r = 0; r < rounds; ++r) {
+    uint32_t buf = r % c.NG;
+    mbar_wait(&c.mbar[buf], (c.phases >> buf) & 1u);
+    c.phases ^= (1u << buf);
+    uint32_t first = r * G;
+    uint32_t cnt = min(G, m - first);
+#pragma unroll 1
+    for (uint32_t v0 = 0; v0 < cnt; v0 += SV) {
+      float e[SV], s[SV];
+#pragma unroll
+      for (int i = 0; i < SV; ++i) {
+        uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
+        const uint2* s2 = (const uint2*)((const __nv_bfloat16*)c.stage + (size_t)(buf * G + v) * c.dpad) + c.lane;
+        float4 x[NQ];
+#pragma unroll
+        for (int t = 0; t < NQ; ++t) {
+          const uint2 w = s2[32 * t];
+          x[t] = bf16x4_to_f4(w.x, w.y);
+        }
+        e[i] = partial_dist<NQ>(x, qr, 1);
+        s[i] = partial_abs_dot<NQ>(x, qr);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int i = 0; i < SV; ++i) {
+          e[i] += __shfl_xor_sync(0xffffffffu, e[i], o);
+          s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
+        }
+      }
+      if (c.lane < (uint32_t)SV && v0 + c.lane < cnt) {
+        float ea = e[0], sa = s[0];
+#pragma unroll
+        for (int i = 1; i < SV; ++i)
+          if (c.lane == (uint32_t)i) ea = e[i], sa = s[i];
+        c.cand_dist[first + v0 + c.lane] = __fsub_rd(__fsub_rd(1.0f, ea), __fmaf_ru(sc, sa, babs));
+      }
+    }
+    __syncwarp();
+    if (r + c.NG < rounds) {
+      fence_proxy_async();
+      issue_rows(c, rows, r + c.NG, m, G, vbytes);
+    }
+  }
+  __syncwarp();
+  const bool in = c.lane < m;
+  const float L = in ? c.cand_dist[c.lane] : 0.f;
+  const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
+  const bool keep = in && !(isfinite(L) && f2ord(L) >= worst_hi);
+  const uint32_t mask = __ballot_sync(0xffffffffu, keep);
+  const uint32_t pos = __popc(mask & lanemask_lt());
+  __syncwarp();
+  if (keep) c.cand_id[pos] = id;
+  if (unsure) unsure = __reduce_or_sync(0xffffffffu, (keep && ((unsure >> c.lane) & 1u)) ? (1u << pos) : 0u);
+  fence_proxy_async();  // the ring's generic reads above, before the fp32 pass's bulk copies into it
+  __syncwarp();
+  return __popc(mask);
 }
 
 // ---------------------------------------------------------------------------
@@ -616,8 +726,10 @@ __device__ __forceinline__ uint32_t list_insert(WarpCtx& c, uint64_t key, uint32
   return pos;
 }
 
+// screened: evaluations made on the bf16 shadow first (fp32 screen); survivors: those of them whose fp32 row was
+// then read.  An fp32 walk reads evals - screened + survivors fp32 rows.
 struct WalkCounters {
-  uint32_t hops_upper, hops_base, evals, overflow;
+  uint32_t hops_upper, hops_base, evals, overflow, screened, survivors;
 };
 
 // Adjacency row of `node` at `level` -> one id per lane (kInvalid beyond the row).
@@ -728,10 +840,26 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 
 // HASDEL = false compiles every trace of the tombstone machinery out (an index without tombstones runs
 // exactly the plain loop: the extra live registers would cost the 16-vector load batches their overlap).
+// The fp32 screen (staged rows up to dpad 1536, metric 1, g.vecs16 set): at a hop that starts with a full result set the hop's
+// candidates are screened on the bf16 shadow first (screen_staged), and only the survivors are evaluated in fp32
+// and offered for admission.  A dropped candidate's fp32 distance is >= the hop-start worst result, so it would
+// not have been admitted (nor queued, if tombstoned): the walk, its results and its counters stay the same.
 template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
+  // (not at dpad 2048: the screen's registers would make ptxas spill in the KPL 2 and 4 walks there)
+  constexpr bool kScreen = LPV == 32 && NQ <= kScreenMaxNQ && std::is_same<RowT, float>::value;
+  const bool screen = kScreen && g.vecs16 && g.metric == 1;  // warp-uniform
+  float babs = 0.f;  // the bound's absolute term: d (2^-125 max|q| + 2^-124) covers subnormals, flushed or not
+  if (screen) {
+    float mx = 0.f;
+#pragma unroll
+    for (int t = 0; t < NQ; ++t)
+      mx = fmaxf(mx, fmaxf(fmaxf(fabsf(qr[t].x), fabsf(qr[t].y)), fmaxf(fabsf(qr[t].z), fabsf(qr[t].w))));
+    mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
+    babs = __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f));
+  }
   hash_clear(c);
   ul_clear<KPL>(u, ef, c.lane);
   const uint8_t* __restrict__ del = (HASDEL && c.dcap) ? g.deleted : nullptr;  // warp-uniform
@@ -771,9 +899,14 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       const uint32_t pos = __popc(mask & lanemask_lt());
       if (is_new) c.cand_id[pos] = nb;
       // tombstones only: candidates (compacted positions) whose visited status is a guess
-      const uint32_t unsure = (HASDEL && del) ? __reduce_or_sync(0xffffffffu, (is_new && o) ? (1u << pos) : 0u) : 0u;
+      uint32_t unsure = (HASDEL && del) ? __reduce_or_sync(0xffffffffu, (is_new && o) ? (1u << pos) : 0u) : 0u;
       __syncwarp();
       wc.evals += m;
+      if (kScreen && screen && cnt >= ef) {
+        wc.screened += m;
+        m = screen_staged<NQ>(c, g.vecs16, qr, m, g.screen_c, babs, worst_hi, unsure);
+        wc.survivors += m;
+      }
       eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
       // the speculative row has arrived by now: pull its neighbours' vectors towards L2 while this hop's
       // candidates are inserted (rows <= 1 KB only; a wrong guess costs bandwidth, not correctness)
