@@ -50,7 +50,8 @@ ehb::GraphView ehb_index::view() const {
 // bandwidth, which the screen relieves; a smaller batch is bound by each warp's chain of memory round trips, to
 // which the screen adds one per hop.
 bool ehb_index::walk_screens(uint64_t nq) const {
-  if (o_walk_screen == 0 || metric == EHB_L2 || dpad * 4u <= 1024u || dpad > 128u * ehb::kScreenMaxNQ) return false;
+  if (o_walk_screen == 0 || metric == EHB_L2) return false;
+  if (!ehb::screen_shape(ehb::row_lpv(dpad * 4u), ehb::row_nq(dpad, dpad * 4u))) return false;
   return o_walk_screen > 0 || nq >= (uint64_t)ehb::kScreenMinBatchPerSm * sms;
 }
 
@@ -72,17 +73,17 @@ int ehb_index::try_screen_shadow() {
 }
 
 // ef_eff: beam width; smem_list: capacity of the shared-memory key list (0 for plain searches);
-// jobs: warps (queries or points) of the launch; team: warps sharing one visited table.
-ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16) const {
+// jobs: warps (queries or points) of the launch; team: warps sharing one visited table; dense: the launch runs
+// the dense form of the walk (walk_plan).
+ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16,
+                                 bool dense) const {
   ehb::WalkCfg c;
   const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);  // bytes of a row as the walk reads it
   c.lcap = smem_list;
-  c.staged = vbytes > 1024 ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
+  c.staged = ehb::row_lpv(vbytes) == 32 ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
   c.dcap = n_deleted ? ehb::kDeletedQueue : 0;
   c.prefetch = o_walk_prefetch ? 1 : 0;
-  // dense walk (search_impl.cuh): batches big enough to fill 20 warps per SM, rows <= 512 B, no tombstones
-  c.dense = (!smem_list && team == 1 && !c.staged && dpad <= 128 && !n_deleted && jobs >= 20ull * (uint64_t)sms) ? 1 : 0;
-  if (bf16 && dpad == 128 && ef_eff > 128) c.dense = 0;  // no dense bf16 form there (search_impl.cuh dense_form)
+  c.dense = dense ? 1 : 0;
   const uint32_t warp_target = c.dense ? 20u : 16u;  // resident warps per SM the visited-table sizing aims at
   uint32_t nslots = std::max(4u, std::min(32u, 24576u / vbytes));
   uint32_t ng = 2;                      // two groups: math on one overlaps the copies of the other
@@ -124,6 +125,45 @@ uint32_t ehb_index::wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16) co
   const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);
   while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, vbytes) + extra) * w > 220 * 1024) w >>= 1;
   return w;
+}
+
+// Largest batch for which the T = 4 team walk keeps its wide U: registers are no constraint while <= 3 CTAs of 128
+// threads (~125 registers each) sit on each SM of the H100's 132.
+constexpr uint64_t kTeamWideMaxQueries = 132u * 3u;
+
+ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) const {
+  ehb::WalkPlan p;
+  p.bf16 = bf16;
+  const uint32_t row_bytes = dpad * (bf16 ? 2u : 4u);
+  p.lpv = ehb::row_lpv(row_bytes);
+  p.nq = ehb::row_nq(dpad, row_bytes);
+  p.kpl = ehb::kpl_for(ef_eff);
+  p.hasdel = n_deleted != 0;
+  // Warps per query (rows <= 1 KB, ef <= 256): four while 3 CTAs of 128 threads per SM hold every query (small
+  // online batches, where one warp's serial chain of memory round trips is the bound), two while 7 CTAs of 64
+  // threads do (C2, Q=1000), else one warp per query: once the batch alone fills the SMs, the team walk's
+  // speculative expansions only add work (C5 shape, Q=10k).
+  uint32_t team = t_team;
+  if (team == 0) team = nq <= (uint64_t)sms * 3 ? 4 : (nq <= (uint64_t)sms * 7 ? 2 : 1);
+  if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
+  if (bf16) team = 1;                                       // the team walk reads fp32 rows only
+  p.T = team;
+  // Vector-load steps (4 vectors each) a team warp keeps in flight.  Registers of loads in flight per lane are
+  // sized so that 7 CTAs fit an SM (T = 2: 64, T = 3 and 4: 32), except that T = 4 keeps the full 16-vector
+  // batches when the batch is so small that registers are no constraint.
+  const bool wide = team == 2 || (team == 4 && nq <= kTeamWideMaxQueries);
+  p.U = team == 1 ? 0 : (uint32_t)(wide ? ehb::team_u_wide(p.nq) : ehb::team_u_narrow(p.nq));
+  // dense walk (search_impl.cuh): batches big enough to fill 20 warps per SM, on the shapes that have one
+  if (team > 1)
+    p.form = ehb::WalkForm::team;
+  else if (nq >= 20ull * (uint64_t)sms && ehb::dense_form(bf16, p.lpv, p.nq, p.kpl, p.hasdel))
+    p.form = ehb::WalkForm::dense;
+  else
+    p.form = ehb::WalkForm::plain;
+  p.screen = !bf16 && team == 1 && shadow && walk_screens(nq);
+  p.cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16, p.form == ehb::WalkForm::dense);
+  p.wpb = wpb_for(p.cfg, 0, bf16);
+  return p;
 }
 
 int ehb_index::ensure_capacity(uint64_t want) {
@@ -707,16 +747,8 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   const bool bf16 = precision == EHB_BF16;
   if (bf16 && sink) return fail(EHB_ERR_INVALID, "the fused shard exchange walks fp32 rows only");
   if (bf16 && !shadow) return fail(EHB_ERR_STATE, "bf16 shadow missing");
-  // Warps per query (rows <= 1 KB, ef <= 256): four while 3 CTAs of 128 threads per SM hold every query (small
-  // online batches, where one warp's serial chain of memory round trips is the bound), two while 7 CTAs of 64
-  // threads do (C2, Q=1000), else one warp per query: once the batch alone fills the SMs, the team walk's
-  // speculative expansions only add work (C5 shape, Q=10k).
-  uint32_t team = t_team;
-  if (team == 0) team = nq <= (uint64_t)sms * 3 ? 4 : (nq <= (uint64_t)sms * 7 ? 2 : 1);
-  if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
-  if (bf16) team = 1;                                       // the team walk reads fp32 rows only
-  ehb::WalkCfg cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16);
-  const bool screen = !bf16 && team == 1 && shadow && walk_screens(nq);
+  const ehb::WalkPlan plan = walk_plan(nq, ef_eff, bf16);
+  if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team;  // the team walk writes destination 0 only
   if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
   const float* q = dq;
   if (metric == EHB_COSINE) {
@@ -732,7 +764,6 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     CU(sl->walk_counts.grow(nq, 0, -1, s));
     CU(ehb::launch_pad_rows(dq, sl->q_pad.p, nq, dim, dpad, metric == EHB_COSINE, s));
   }
-  uint32_t wpb = wpb_for(cfg, 0, bf16);
   CU(cudaEventRecord(sl->ev0, s));
   if (bf16) {
     // walk the bf16 rows keeping the whole retained set, then re-rank it with the canonical fp32 chain
@@ -741,12 +772,12 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     ks.keys = sl->walk_keys.p;
     ehb::GraphView g = view();
     g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
-    CU(ehb::launch_search_bf16(g, cfg, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, wpb, s));
+    CU(ehb::launch_search(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, s));
     CU(ehb::launch_rerank(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
                           labels.p, nq, k, dl, dd, dc, s));
-  } else if (team >= 2)
-    CU(ehb::launch_search_team(team, view(), cfg.hash_size, q, (uint32_t)nq, k, ef_eff, dl, dd, dc, sl->stats.p, s));
-  else {
+  } else if (plan.form == ehb::WalkForm::team) {
+    CU(ehb::launch_search_team(plan, view(), q, (uint32_t)nq, k, ef_eff, dl, dd, dc, sl->stats.p, s));
+  } else {
     ehb::ResultSink one;
     if (!sink) {
       std::memset(&one, 0, sizeof(one));
@@ -754,31 +785,19 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
       one.dists[0] = dd;
       one.n = 1;
       sink = &one;
-    } else if (pushed) {
-      *pushed = true;
     }
     ehb::GraphView g = view();
-    if (screen) {
+    if (plan.screen) {
       g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
       const double c = ehb::screen_constant(dpad);
       g.screen_c = (double)(float)c >= c ? (float)c : std::nextafter((float)c, INFINITY);
     }
-    CU(ehb::launch_search(g, cfg, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, wpb, s));
+    CU(ehb::launch_search(plan, g, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, s));
   }
   CU(cudaEventRecord(sl->ev1, s));
   sl->last_nq = nq;
   sl->last_bf16 = bf16;
-  {
-    const uint32_t kpl = ef_eff <= 64 ? 2 : (ef_eff <= 128 ? 4 : (ef_eff <= 256 ? 8 : 16));
-    const uint32_t lpv = cfg.staged ? 32 : 8;
-    if (team >= 2)
-      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "hnsw_search_team_kernel<NQ=%u,KPL=%u,T=%u,U=%u>",
-                    dpad / (4 * lpv), kpl, team, ehb::team_eval_steps(team, dpad, (uint32_t)nq));
-    else  // (HASDEL is named only when set, so the common instantiations keep their short names)
-      std::snprintf(sl->last_kernel, sizeof(sl->last_kernel), "%s<LPV=%u,NQ=%u,KPL=%u%s%s>",
-                    cfg.dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", lpv, dpad / (4 * lpv), kpl,
-                    n_deleted ? ",HASDEL=1" : "", bf16 ? ",ROW=bf16" : "");
-  }
+  ehb::walk_kernel_name(plan, sl->last_kernel, sizeof(sl->last_kernel));
   {
     std::lock_guard<std::mutex> g(last_mu);
     last_slot = sl;

@@ -18,25 +18,16 @@
 //     does one edge at a time.
 // Results are deterministic: candidates are ordered by (distance, id) before
 // any selection, so atomic arrival order never matters.
-#include "build_impl.cuh"
+// The kernels are in build_impl.cuh, instantiated per row shape in build_inst_*.cu.
+#include "kernels.h"
 
 namespace ehb {
 
-cudaError_t launch_build_batch(EHB_BUILD_ARGS) {
+cudaError_t launch_build_batch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
+                               uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
   if (b == 0) return cudaSuccess;
-  switch (bg.g.dpad) {
-    case 32: return launch_build_d32(EHB_BUILD_PASS);
-    case 64: return launch_build_d64(EHB_BUILD_PASS);
-    case 128: return launch_build_d128(EHB_BUILD_PASS);
-    case 256: return launch_build_d256(EHB_BUILD_PASS);
-    case 384: return launch_build_d384(EHB_BUILD_PASS);
-    case 512: return launch_build_d512(EHB_BUILD_PASS);
-    case 768: return launch_build_d768(EHB_BUILD_PASS);
-    case 1024: return launch_build_d1024(EHB_BUILD_PASS);
-    case 1536: return launch_build_d1536(EHB_BUILD_PASS);
-    case 2048: return launch_build_d2048(EHB_BUILD_PASS);
-    default: return cudaErrorInvalidValue;
-  }
+  return with_dpad(bg.g.dpad,
+                   [&](auto d) { return BuildShape<decltype(d)::value>::launch(bg, cfg, ids, first, b, mode, bb, wpb, s); });
 }
 
 }  // namespace ehb

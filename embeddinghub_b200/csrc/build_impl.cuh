@@ -434,9 +434,10 @@ __global__ void __launch_bounds__(128) merge_rows_kernel(BuildGraph bg, WalkCfg 
   }
 }
 
-template <int LPV, int NQ>
-cudaError_t launch_build_t(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first, uint32_t b,
-                           int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
+template <uint32_t DPAD>
+cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
+                                     uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
+  constexpr int LPV = row_lpv(DPAD * 4u), NQ = row_nq(DPAD, DPAD * 4u);
   constexpr int KPL = 8;  // ef_construction <= 256
   cudaError_t e;
   const bool is_update = mode == kBuildUpdate;
@@ -488,20 +489,5 @@ cudaError_t launch_build_t(const BuildGraph& bg, const WalkCfg& cfg, const uint3
   km<<<(ethreads + mwpb - 1) / mwpb, 32 * mwpb, msmem, s>>>(bg, mcfg, bb, mwsm);
   return cudaGetLastError();
 }
-
-#define EHB_BUILD_ARGS                                                                                     \
-  const BuildGraph &bg, const WalkCfg &cfg, const uint32_t *ids, uint32_t first, uint32_t b, int mode, \
-      BuildBuffers &bb, uint32_t wpb, cudaStream_t s
-#define EHB_BUILD_PASS bg, cfg, ids, first, b, mode, bb, wpb, s
-cudaError_t launch_build_d32(EHB_BUILD_ARGS);
-cudaError_t launch_build_d64(EHB_BUILD_ARGS);
-cudaError_t launch_build_d128(EHB_BUILD_ARGS);
-cudaError_t launch_build_d256(EHB_BUILD_ARGS);
-cudaError_t launch_build_d384(EHB_BUILD_ARGS);
-cudaError_t launch_build_d512(EHB_BUILD_ARGS);
-cudaError_t launch_build_d768(EHB_BUILD_ARGS);
-cudaError_t launch_build_d1024(EHB_BUILD_ARGS);
-cudaError_t launch_build_d1536(EHB_BUILD_ARGS);
-cudaError_t launch_build_d2048(EHB_BUILD_ARGS);
 
 }  // namespace ehb

@@ -1,7 +1,7 @@
-// K5 instantiations (generated list of row shapes; see build_impl.cuh)
+// K5 instantiations for dpad 32 .. 128 (see build_impl.cuh)
 #include "build_impl.cuh"
 namespace ehb {
-cudaError_t launch_build_d32(EHB_BUILD_ARGS) { return launch_build_t<8, 1>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d64(EHB_BUILD_ARGS) { return launch_build_t<8, 2>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d128(EHB_BUILD_ARGS) { return launch_build_t<8, 4>(EHB_BUILD_PASS); }
+template struct BuildShape<32>;
+template struct BuildShape<64>;
+template struct BuildShape<128>;
 }  // namespace ehb

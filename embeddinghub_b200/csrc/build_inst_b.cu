@@ -1,6 +1,6 @@
-// K5 instantiations (generated list of row shapes; see build_impl.cuh)
+// K5 instantiations for dpad 256 .. 384 (see build_impl.cuh)
 #include "build_impl.cuh"
 namespace ehb {
-cudaError_t launch_build_d256(EHB_BUILD_ARGS) { return launch_build_t<8, 8>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d384(EHB_BUILD_ARGS) { return launch_build_t<32, 3>(EHB_BUILD_PASS); }
+template struct BuildShape<256>;
+template struct BuildShape<384>;
 }  // namespace ehb

@@ -1,6 +1,6 @@
-// K5 instantiations (generated list of row shapes; see build_impl.cuh)
+// K5 instantiations for dpad 512 .. 768 (see build_impl.cuh)
 #include "build_impl.cuh"
 namespace ehb {
-cudaError_t launch_build_d512(EHB_BUILD_ARGS) { return launch_build_t<32, 4>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d768(EHB_BUILD_ARGS) { return launch_build_t<32, 6>(EHB_BUILD_PASS); }
+template struct BuildShape<512>;
+template struct BuildShape<768>;
 }  // namespace ehb

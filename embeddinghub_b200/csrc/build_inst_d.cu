@@ -1,7 +1,7 @@
-// K5 instantiations (generated list of row shapes; see build_impl.cuh)
+// K5 instantiations for dpad 1024 .. 2048 (see build_impl.cuh)
 #include "build_impl.cuh"
 namespace ehb {
-cudaError_t launch_build_d1024(EHB_BUILD_ARGS) { return launch_build_t<32, 8>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d1536(EHB_BUILD_ARGS) { return launch_build_t<32, 12>(EHB_BUILD_PASS); }
-cudaError_t launch_build_d2048(EHB_BUILD_ARGS) { return launch_build_t<32, 16>(EHB_BUILD_PASS); }
+template struct BuildShape<1024>;
+template struct BuildShape<1536>;
+template struct BuildShape<2048>;
 }  // namespace ehb

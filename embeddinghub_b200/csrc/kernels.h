@@ -12,26 +12,52 @@ constexpr uint32_t kMaxEf = 512;    // register-resident list: 16 keys per lane
 constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved point, >= 1 + 32 + 32*32
 constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
 
-// K2 — batched k-NN graph walk (hnswlib searchKnn).  ef >= k, cfg.lcap >= ef.
-// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.vecs16
-// set (metric 1, rows > 1 KB) the walk screens candidates on the bf16 shadow (walk.cuh beam_search).
-constexpr uint32_t kStatWords = 8;
-cudaError_t launch_search(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
-                          uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
-                          uint32_t warps_per_block, cudaStream_t s);
-// K2 over the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation).  Writes the retained set, not results:
-// sink.keys[nq][k] gets the (ordered distance, internal id) keys nearest-first (call with k = ef to keep all of
-// them) and out_counts the retained count; launch_rerank then produces the fp32 results.
-cudaError_t launch_search_bf16(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
-                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
-                               uint32_t warps_per_block, cudaStream_t s);
+// Shapes with a dense form of the one-warp walk (search_impl.cuh): LPV = 8, NQ <= 4, no tombstones.  Over bf16 rows
+// the dense form's 96-register budget spills at dpad = 128 with KPL >= 8, so those shapes have none.
+constexpr bool dense_form(bool bf16, int LPV, int NQ, int KPL, bool HASDEL) {
+  return LPV == 8 && NQ <= 4 && !HASDEL && (!bf16 || NQ < 4 || KPL < 8);
+}
+// U (4-vector load steps a team warp keeps in flight) of the team walk's wide and narrow forms
+__host__ __device__ constexpr int team_u_wide(int NQ) { return NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2); }
+__host__ __device__ constexpr int team_u_narrow(int NQ) { return NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1); }
 
-// K2t — team walk (T warps per query, T in {2,3,4}); rows <= 1 KB and ef <= 256 only.
-cudaError_t launch_search_team(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,
-                               uint32_t k, uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
+// Which graph-walk kernel a search runs and how it is launched (ehb_index::walk_plan).  The launchers and the
+// reported kernel name read it and decide nothing themselves.
+enum class WalkForm { plain, dense, team };
+struct WalkPlan {
+  bool bf16;           // the walk reads the bf16 shadow g.vecs16 (else the fp32 rows)
+  int lpv, nq, kpl;    // row shape (walk.cuh row_lpv / row_nq) and result-set entries per lane (kpl_for)
+  bool hasdel;         // the index has tombstones
+  WalkForm form;
+  uint32_t T, U;       // team form: warps per query (2..4) and load steps in flight; 1 and 0 otherwise
+  bool screen;         // the fp32 walk screens candidates on the bf16 shadow (g.vecs16 set by the caller)
+  WalkCfg cfg;
+  uint32_t wpb;        // warps per block of the one-warp forms
+};
+// the name of the kernel the plan launches, e.g. hnsw_search_kernel<LPV=32,NQ=6,KPL=4>
+void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes);
+
+// K2 — batched k-NN graph walk (hnswlib searchKnn), one warp per query, plain or dense form.  ef >= k.
+// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.vecs16
+// set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the bf16 shadow (walk.cuh beam_search).
+// With p.bf16 the walk reads the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation) and writes the retained
+// set, not results: sink.keys[nq][k] gets the (ordered distance, internal id) keys nearest-first (call with k = ef
+// to keep all of them) and out_counts the retained count; launch_rerank then produces the fp32 results.
+constexpr uint32_t kStatWords = 8;
+cudaError_t launch_search(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                          uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, cudaStream_t s);
+// K2 for rows of DPAD floats of type RowT (search_impl.cuh; instantiated per shape in search_inst_*.cu)
+template <uint32_t DPAD, class RowT>
+struct SearchShape {
+  static cudaError_t launch(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                            uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
+                            cudaStream_t s);
+};
+
+// K2t — team walk (p.T warps per query); fp32 rows <= 1 KB and ef <= 256 only.
+cudaError_t launch_search_team(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                               uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
                                uint32_t* stats, cudaStream_t s);
-// the U (4-vector load steps in flight) that launch_search_team instantiates for this shape
-uint32_t team_eval_steps(uint32_t T, uint32_t dpad, uint32_t nq);
 
 // row-wise L2 normalisation (hnswlib cosine convention), canonical arithmetic.
 cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, uint32_t out_stride, uint64_t n,
@@ -128,6 +154,12 @@ enum BuildMode : int {
 };
 cudaError_t launch_build_batch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
                                uint32_t b, int mode, BuildBuffers& bb, uint32_t warps_per_block, cudaStream_t s);
+// K5 for rows of DPAD floats (build_impl.cuh; instantiated per shape in build_inst_*.cu)
+template <uint32_t DPAD>
+struct BuildShape {
+  static cudaError_t launch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first, uint32_t b,
+                            int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s);
+};
 
 // K6 — compaction (ehb_index_compact).  Row ids follow the edge_row convention: < cap a level-0 row, >= cap an
 // upper row.

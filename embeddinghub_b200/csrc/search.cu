@@ -3,43 +3,31 @@
 // ANNIndex::approx_nearest (embeddinghub/embeddingstore/index.cc:39-52).
 // The kernel template lives in search_impl.cuh; one translation unit per group
 // of row shapes (search_inst_*.cu) keeps the build parallel.
-#include "search_impl.cuh"
+#include <cstdio>
+
+#include "kernels.h"
 
 namespace ehb {
 
-cudaError_t launch_search(EHB_SEARCH_ARGS) {
+cudaError_t launch_search(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                          uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, cudaStream_t s) {
   if (nq == 0) return cudaSuccess;
-  switch (g.dpad) {
-    case 32: return launch_search_d32(EHB_SEARCH_PASS);
-    case 64: return launch_search_d64(EHB_SEARCH_PASS);
-    case 128: return launch_search_d128(EHB_SEARCH_PASS);
-    case 256: return launch_search_d256(EHB_SEARCH_PASS);
-    case 384: return launch_search_d384(EHB_SEARCH_PASS);
-    case 512: return launch_search_d512(EHB_SEARCH_PASS);
-    case 768: return launch_search_d768(EHB_SEARCH_PASS);
-    case 1024: return launch_search_d1024(EHB_SEARCH_PASS);
-    case 1536: return launch_search_d1536(EHB_SEARCH_PASS);
-    case 2048: return launch_search_d2048(EHB_SEARCH_PASS);
-    default: return cudaErrorInvalidValue;
-  }
+  if (p.bf16 && (!g.vecs16 || !sink.keys)) return cudaErrorInvalidValue;
+  return with_dpad(g.dpad, [&](auto d) {
+    constexpr uint32_t D = decltype(d)::value;
+    return p.bf16 ? SearchShape<D, __nv_bfloat16>::launch(p, g, queries, nq, k, ef, sink, out_counts, stats, s)
+                  : SearchShape<D, float>::launch(p, g, queries, nq, k, ef, sink, out_counts, stats, s);
+  });
 }
 
-cudaError_t launch_search_bf16(EHB_SEARCH_ARGS) {
-  if (nq == 0) return cudaSuccess;
-  if (!g.vecs16 || !sink.keys) return cudaErrorInvalidValue;
-  switch (g.dpad) {
-    case 32: return launch_search_bf16_d32(EHB_SEARCH_PASS);
-    case 64: return launch_search_bf16_d64(EHB_SEARCH_PASS);
-    case 128: return launch_search_bf16_d128(EHB_SEARCH_PASS);
-    case 256: return launch_search_bf16_d256(EHB_SEARCH_PASS);
-    case 384: return launch_search_bf16_d384(EHB_SEARCH_PASS);
-    case 512: return launch_search_bf16_d512(EHB_SEARCH_PASS);
-    case 768: return launch_search_bf16_d768(EHB_SEARCH_PASS);
-    case 1024: return launch_search_bf16_d1024(EHB_SEARCH_PASS);
-    case 1536: return launch_search_bf16_d1536(EHB_SEARCH_PASS);
-    case 2048: return launch_search_bf16_d2048(EHB_SEARCH_PASS);
-    default: return cudaErrorInvalidValue;
-  }
+// (HASDEL and ROW are named only when set, so the common instantiations keep their short names)
+void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes) {
+  if (p.form == WalkForm::team)
+    std::snprintf(out, out_bytes, "hnsw_search_team_kernel<NQ=%d,KPL=%d,T=%u,U=%u>", p.nq, p.kpl, p.T, p.U);
+  else
+    std::snprintf(out, out_bytes, "%s<LPV=%d,NQ=%d,KPL=%d%s%s>",
+                  p.form == WalkForm::dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", p.lpv, p.nq, p.kpl,
+                  p.hasdel ? ",HASDEL=1" : "", p.bf16 ? ",ROW=bf16" : "");
 }
 
 // ---------------------------------------------------------------------------

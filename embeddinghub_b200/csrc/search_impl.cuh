@@ -109,16 +109,10 @@ __global__ void __launch_bounds__(128, kWalkMinBlocks<RowT>)
   search_body<LPV, NQ, KPL, HASDEL, 1, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
-// Shapes with a dense form (LPV = 8, NQ <= 4, no tombstones).  Over bf16 rows the 96-register budget spills at
-// dpad = 128 with KPL >= 8, so those shapes keep the default form (ehb_index::walk_cfg agrees).
-template <class RowT>
-__host__ __device__ constexpr bool dense_form(int NQ, int KPL) {
-  return std::is_same<RowT, float>::value || NQ < 4 || KPL < 8;
-}
-
 // "Dense" form for big batches of short rows (LPV = 8, d <= 128): 8 vectors in flight per warp instead of 16
 // and a 96-register budget -> 20 resident warps per SM instead of 16 (the visited table shrinks to match,
-// api.cu walk_cfg): with many queries in flight, more warps hide more of each hop's memory latency.
+// api.cu walk_cfg): with many queries in flight, more warps hide more of each hop's memory latency.  Only the
+// shapes of kernels.h dense_form have one.
 template <int LPV, int NQ, int KPL, class RowT>
 __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, WalkCfg cfg,
                                                                    const float* __restrict__ queries, uint32_t nq,
@@ -129,66 +123,43 @@ __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, 
   search_body<LPV, NQ, KPL, false, 2, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
-template <int LPV, int NQ, int KPL, bool HASDEL, class RowT>
-cudaError_t launch_search_t(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
-                            uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t wpb,
+template <int LPV, int NQ, int KPL, class RowT>
+cudaError_t launch_search_t(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                            uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                             cudaStream_t s) {
-  uint32_t wsm = warp_smem_bytes(cfg, g.dpad * (uint32_t)sizeof(RowT));
+  constexpr bool kBf16 = !std::is_same<RowT, float>::value;
+  const uint32_t wpb = p.wpb;
+  uint32_t wsm = warp_smem_bytes(p.cfg, g.dpad * (uint32_t)sizeof(RowT));
   size_t smem = (size_t)wsm * wpb;
   dim3 grid((nq + wpb - 1) / wpb), block(32 * wpb);
   void (*kern)(GraphView, WalkCfg, const float*, uint32_t, uint32_t, uint32_t, const ResultSink, uint32_t*, uint32_t*,
-               uint32_t) = hnsw_search_kernel<LPV, NQ, KPL, HASDEL, RowT>;
-  if constexpr (LPV == 8 && NQ <= 4 && !HASDEL && dense_form<RowT>(NQ, KPL)) {
-    if (cfg.dense) kern = hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
+               uint32_t) = p.hasdel ? hnsw_search_kernel<LPV, NQ, KPL, true, RowT>
+                                    : hnsw_search_kernel<LPV, NQ, KPL, false, RowT>;
+  if (p.form == WalkForm::dense) {
+    if (!dense_form(kBf16, LPV, NQ, KPL, p.hasdel)) return cudaErrorInvalidValue;
+    if constexpr (dense_form(kBf16, LPV, NQ, KPL, false)) kern = hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
   }
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kern<<<grid, block, smem, s>>>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wsm);
+  kern<<<grid, block, smem, s>>>(g, p.cfg, queries, nq, k, ef, sink, out_counts, stats, wsm);
   return cudaGetLastError();
 }
 
-template <int LPV, int NQ, class RowT = float>
-cudaError_t launch_search_kpl(const GraphView& g, const WalkCfg& cfg, const float* queries, uint32_t nq, uint32_t k,
-                              uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t wpb,
-                              cudaStream_t s) {
+template <uint32_t DPAD, class RowT>
+cudaError_t SearchShape<DPAD, RowT>::launch(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq,
+                                            uint32_t k, uint32_t ef, const ResultSink& sink, uint32_t* out_counts,
+                                            uint32_t* stats, cudaStream_t s) {
+  constexpr int LPV = row_lpv(DPAD * sizeof(RowT)), NQ = row_nq(DPAD, DPAD * sizeof(RowT));
+  if (p.lpv != LPV || p.nq != NQ || p.form == WalkForm::team) return cudaErrorInvalidValue;
   // (Keeping a whole 2M-neighbour hop in flight per batch needs about 168 registers, which costs occupancy;
   //  batches stay at 16 vectors.)
-#define EHB_KPL(K)                                                                                          \
-  return g.deleted                                                                                          \
-             ? launch_search_t<LPV, NQ, K, true, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s) \
-             : launch_search_t<LPV, NQ, K, false, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s)
-  if (ef <= 64) EHB_KPL(2);
-  if (ef <= 128) EHB_KPL(4);
-  if (ef <= 256) EHB_KPL(8);
-  EHB_KPL(16);
-#undef EHB_KPL
+  switch (p.kpl) {
+    case 2: return launch_search_t<LPV, NQ, 2, RowT>(p, g, queries, nq, k, ef, sink, out_counts, stats, s);
+    case 4: return launch_search_t<LPV, NQ, 4, RowT>(p, g, queries, nq, k, ef, sink, out_counts, stats, s);
+    case 8: return launch_search_t<LPV, NQ, 8, RowT>(p, g, queries, nq, k, ef, sink, out_counts, stats, s);
+    case 16: return launch_search_t<LPV, NQ, 16, RowT>(p, g, queries, nq, k, ef, sink, out_counts, stats, s);
+    default: return cudaErrorInvalidValue;
+  }
 }
-
-#define EHB_SEARCH_ARGS                                                                                  \
-  const GraphView &g, const WalkCfg &cfg, const float *queries, uint32_t nq, uint32_t k, uint32_t ef,    \
-      const ResultSink &sink, uint32_t *out_counts, uint32_t *stats, uint32_t wpb, cudaStream_t s
-#define EHB_SEARCH_PASS g, cfg, queries, nq, k, ef, sink, out_counts, stats, wpb, s
-
-cudaError_t launch_search_d32(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d64(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d128(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d256(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d384(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d512(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d768(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d1024(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d1536(EHB_SEARCH_ARGS);
-cudaError_t launch_search_d2048(EHB_SEARCH_ARGS);
-// the bf16 walk (search_inst_bf16_*.cu)
-cudaError_t launch_search_bf16_d32(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d64(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d128(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d256(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d384(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d512(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d768(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d1024(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d1536(EHB_SEARCH_ARGS);
-cudaError_t launch_search_bf16_d2048(EHB_SEARCH_ARGS);
 
 }  // namespace ehb

@@ -1,7 +1,7 @@
-// K2 instantiations (generated list of row shapes; see search_impl.cuh)
+// K2 instantiations over fp32 rows of dpad 32 .. 128 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_d32(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 1>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d64(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 2>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d128(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 4>(EHB_SEARCH_PASS); }
+template struct SearchShape<32, float>;
+template struct SearchShape<64, float>;
+template struct SearchShape<128, float>;
 }  // namespace ehb

@@ -1,6 +1,6 @@
-// K2 instantiations (generated list of row shapes; see search_impl.cuh)
+// K2 instantiations over fp32 rows of dpad 256 .. 384 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_d256(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 8>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d384(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 3>(EHB_SEARCH_PASS); }
+template struct SearchShape<256, float>;
+template struct SearchShape<384, float>;
 }  // namespace ehb

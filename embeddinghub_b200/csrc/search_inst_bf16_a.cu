@@ -1,7 +1,7 @@
-// K2 instantiations over bf16 rows (row shapes of the bf16 walk; see search_impl.cuh and walk.cuh)
+// K2 instantiations over the bf16 shadow of dpad 32 .. 128 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_bf16_d32(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 1, __nv_bfloat16>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_bf16_d64(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 2, __nv_bfloat16>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_bf16_d128(EHB_SEARCH_ARGS) { return launch_search_kpl<8, 4, __nv_bfloat16>(EHB_SEARCH_PASS); }
+template struct SearchShape<32, __nv_bfloat16>;
+template struct SearchShape<64, __nv_bfloat16>;
+template struct SearchShape<128, __nv_bfloat16>;
 }  // namespace ehb

@@ -1,6 +1,6 @@
-// K2 instantiations over bf16 rows (row shapes of the bf16 walk; see search_impl.cuh and walk.cuh)
+// K2 instantiations over the bf16 shadow of dpad 768 .. 1024 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_bf16_d768(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 6, __nv_bfloat16>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_bf16_d1024(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 8, __nv_bfloat16>(EHB_SEARCH_PASS); }
+template struct SearchShape<768, __nv_bfloat16>;
+template struct SearchShape<1024, __nv_bfloat16>;
 }  // namespace ehb

@@ -1,6 +1,6 @@
-// K2 instantiations (generated list of row shapes; see search_impl.cuh)
+// K2 instantiations over fp32 rows of dpad 512 .. 768 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_d512(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 4>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d768(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 6>(EHB_SEARCH_PASS); }
+template struct SearchShape<512, float>;
+template struct SearchShape<768, float>;
 }  // namespace ehb

@@ -1,7 +1,7 @@
-// K2 instantiations (generated list of row shapes; see search_impl.cuh)
+// K2 instantiations over fp32 rows of dpad 1024 .. 2048 (see search_impl.cuh)
 #include "search_impl.cuh"
 namespace ehb {
-cudaError_t launch_search_d1024(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 8>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d1536(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 12>(EHB_SEARCH_PASS); }
-cudaError_t launch_search_d2048(EHB_SEARCH_ARGS) { return launch_search_kpl<32, 16>(EHB_SEARCH_PASS); }
+template struct SearchShape<1024, float>;
+template struct SearchShape<1536, float>;
+template struct SearchShape<2048, float>;
 }  // namespace ehb

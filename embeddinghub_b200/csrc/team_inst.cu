@@ -3,53 +3,35 @@
 
 namespace ehb {
 
-// Vector-load steps (4 vectors each) a team warp keeps in flight: the U template argument of K2t.  Registers of
-// loads in flight per lane are sized so that 7 CTAs fit an SM (T = 2: 64, T = 3 and 4: 32), except that T = 4
-// keeps the full 16-vector batches when the batch is so small that registers are no constraint (<= 3 CTAs of 128
-// threads per SM of the H100's 132 at ~125 registers).
-constexpr uint32_t kTeamWideMaxQueries = 132u * 3u;
-__host__ __device__ constexpr int team_u_wide(int NQ) { return NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2); }
-__host__ __device__ constexpr int team_u_narrow(int NQ) { return NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1); }
-static bool team_wide(uint32_t T, uint32_t nq) { return T == 2 || (T >= 4 && nq <= kTeamWideMaxQueries); }
-
-uint32_t team_eval_steps(uint32_t T, uint32_t dpad, uint32_t nq) {
-  const int NQ = (int)(dpad / 32u);
-  return (uint32_t)(team_wide(T, nq) ? team_u_wide(NQ) : team_u_narrow(NQ));
-}
-
 template <int NQ, int T, int U>
-static cudaError_t team_kpl(const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq, uint32_t k,
+static cudaError_t team_kpl(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
                             uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
                             uint32_t* stats, cudaStream_t s) {
-  if (ef <= 64) return launch_team_t<NQ, 2, T, U>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-  if (ef <= 128) return launch_team_t<NQ, 4, T, U>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-  return launch_team_t<NQ, 8, T, U>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-}
-
-template <int NQ>
-static cudaError_t team_t(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,
-                          uint32_t k, uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
-                          uint32_t* stats, cudaStream_t s) {
-  constexpr int U2 = team_u_wide(NQ), U4 = team_u_narrow(NQ);
-  if (T >= 4 && team_wide(T, nq))
-    return team_kpl<NQ, 4, U2>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-  if (T >= 4) return team_kpl<NQ, 4, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-  if (T == 3) return team_kpl<NQ, 3, U4>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-  return team_kpl<NQ, 2, U2>(g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-}
-
-// ef <= 256, dpad in {32, 64, 128, 256}
-cudaError_t launch_search_team(uint32_t T, const GraphView& g, uint32_t hash_size, const float* queries, uint32_t nq,
-                               uint32_t k, uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
-                               uint32_t* stats, cudaStream_t s) {
-  if (nq == 0) return cudaSuccess;
-  switch (g.dpad) {
-    case 32: return team_t<1>(T, g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-    case 64: return team_t<2>(T, g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-    case 128: return team_t<4>(T, g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
-    case 256: return team_t<8>(T, g, hash_size, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+  const uint32_t hs = p.cfg.hash_size;
+  switch (p.kpl) {
+    case 2: return launch_team_t<NQ, 2, T, U>(g, hs, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    case 4: return launch_team_t<NQ, 4, T, U>(g, hs, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    case 8: return launch_team_t<NQ, 8, T, U>(g, hs, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
     default: return cudaErrorInvalidValue;
   }
+}
+
+cudaError_t launch_search_team(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                               uint32_t ef, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,
+                               uint32_t* stats, cudaStream_t s) {
+  if (nq == 0) return cudaSuccess;
+  if (p.form != WalkForm::team || p.bf16 || p.lpv != 8) return cudaErrorInvalidValue;
+  return with_dpad<256>(g.dpad, [&](auto d) {
+    constexpr int NQ = row_nq(decltype(d)::value, decltype(d)::value * 4u);
+    constexpr uint32_t UW = team_u_wide(NQ), UN = team_u_narrow(NQ);
+    // the (T, U) pairs ehb_index::walk_plan chooses: T = 2 and 4 with the wide U, T = 3 and 4 with the narrow one
+    const uint32_t T = p.T, U = p.U;
+    if (T == 2 && U == UW) return team_kpl<NQ, 2, UW>(p, g, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    if (T == 3 && U == UN) return team_kpl<NQ, 3, UN>(p, g, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    if (T == 4 && U == UW) return team_kpl<NQ, 4, UW>(p, g, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    if (T == 4 && U == UN) return team_kpl<NQ, 4, UN>(p, g, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);
+    return cudaErrorInvalidValue;
+  });
 }
 
 }  // namespace ehb

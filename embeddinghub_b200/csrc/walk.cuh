@@ -54,7 +54,6 @@ struct GraphView {
 //   |P^ - E^| <= (2^-8 + (2 + 2^-8) g) * S + A,   g = n 2^-24 / (1 - n 2^-24),  S = sum |q_i| |b_i|,
 // A covering subnormal inputs and products (flushed or not).  The screen computes S^ >= (1 - g) S in fp32 as well,
 // so the constant is divided by (1 - g), then padded by 2^-20 for the rounding of the constant itself.
-constexpr uint32_t kScreenMaxNQ = 12;  // staged rows of dpad 384 .. 1536 (LPV = 32, NQ = dpad / 128)
 __host__ __device__ inline double screen_constant(uint32_t n) {
   const double u = 1.0 / 256.0, e = n * 0x1p-24, g = e / (1.0 - e);
   return (u + (2.0 + u) * g) / (1.0 - g) * (1.0 + 0x1p-20);
@@ -90,13 +89,40 @@ struct ResultSink {
 
 __host__ __device__ inline uint32_t align_up(uint32_t x, uint32_t a) { return (x + a - 1) / a * a; }
 
-// Supported padded row lengths: LPV=8 -> NQ in {1,2,4,8}; LPV=32 -> NQ in {3,4,6,8,12,16}.
-__host__ __device__ inline uint32_t pad_dim(uint32_t dim) {
-  const uint32_t sizes[10] = {32, 64, 128, 256, 384, 512, 768, 1024, 1536, 2048};
-  for (int i = 0; i < 10; ++i)
-    if (dim <= sizes[i]) return sizes[i];
+// ---- Row shapes ------------------------------------------------------------------------------------------
+// The padded row lengths (floats) the walk supports, ascending.  A row of `row_bytes` as the walk reads it
+// (dpad * 4 for fp32 rows, dpad * 2 for the bf16 shadow) is loaded directly by LPV = 8 lanes per vector up to
+// 1 KB, and staged through the TMA ring and read by LPV = 32 lanes above; a lane holds NQ float4 chunks of the
+// fp32 query (dpad == 4 * LPV * NQ).
+constexpr uint32_t kPadDims[] = {32, 64, 128, 256, 384, 512, 768, 1024, 1536, 2048};
+constexpr uint32_t kNumPadDims = sizeof(kPadDims) / sizeof(kPadDims[0]);
+__host__ __device__ constexpr int row_lpv(uint32_t row_bytes) { return row_bytes > 1024 ? 32 : 8; }
+__host__ __device__ constexpr int row_nq(uint32_t dpad, uint32_t row_bytes) {
+  return (int)(dpad / (4u * (uint32_t)row_lpv(row_bytes)));
+}
+// register-resident result set entries per lane for a beam of ef (<= 512)
+constexpr int kpl_for(uint32_t ef) { return ef <= 64 ? 2 : (ef <= 128 ? 4 : (ef <= 256 ? 8 : 16)); }
+
+inline uint32_t pad_dim(uint32_t dim) {
+  for (uint32_t d : kPadDims)
+    if (dim <= d) return d;
   return 0;
 }
+
+// Calls f(std::integral_constant<uint32_t, DPAD>{}) for the padded row length DPAD == dpad; any other dpad, or one
+// above MaxDpad, is cudaErrorInvalidValue.
+template <uint32_t MaxDpad = 2048, uint32_t I = 0, class F>
+cudaError_t with_dpad(uint32_t dpad, F&& f) {
+  if constexpr (I == kNumPadDims || kPadDims[I] > MaxDpad)
+    return cudaErrorInvalidValue;
+  else
+    return dpad == kPadDims[I] ? f(std::integral_constant<uint32_t, kPadDims[I]>{})
+                               : with_dpad<MaxDpad, I + 1>(dpad, f);
+}
+
+// The fp32 walk's screen applies to staged fp32 rows of dpad 384 .. 1536 (not at dpad 2048: the screen's registers
+// would make ptxas spill in the KPL 2 and 4 walks there).
+__host__ __device__ constexpr bool screen_shape(int LPV, int NQ) { return LPV == 32 && NQ <= 12; }
 
 // Per-warp shared-memory slice; every region offset is a multiple of 128 B.  vbytes: bytes of one row as the
 // walk reads it (dpad * 4 for fp32 rows, dpad * 2 for the bf16 shadow); it sizes the TMA staging ring.
@@ -848,8 +874,7 @@ template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, cl
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
-  // (not at dpad 2048: the screen's registers would make ptxas spill in the KPL 2 and 4 walks there)
-  constexpr bool kScreen = LPV == 32 && NQ <= kScreenMaxNQ && std::is_same<RowT, float>::value;
+  constexpr bool kScreen = screen_shape(LPV, NQ) && std::is_same<RowT, float>::value;
   const bool screen = kScreen && g.vecs16 && g.metric == 1;  // warp-uniform
   float babs = 0.f;  // the bound's absolute term: d (2^-125 max|q| + 2^-124) covers subnormals, flushed or not
   if (screen) {
