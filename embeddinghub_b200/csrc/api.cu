@@ -152,7 +152,7 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
   // sized so that 7 CTAs fit an SM (T = 2: 64, T = 3 and 4: 32), except that T = 4 keeps the full 16-vector
   // batches when the batch is so small that registers are no constraint.
   const bool wide = team == 2 || (team == 4 && nq <= kTeamWideMaxQueries);
-  p.U = team == 1 ? 0 : (uint32_t)(wide ? ehb::team_u_wide(p.nq) : ehb::team_u_narrow(p.nq));
+  p.U = team == 1 ? 0 : (uint32_t)ehb::eval_u(p.nq, wide ? 1 : 2);
   // dense walk (search_impl.cuh): batches big enough to fill 20 warps per SM, on the shapes that have one
   if (team > 1)
     p.form = ehb::WalkForm::team;

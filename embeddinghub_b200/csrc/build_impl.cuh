@@ -111,15 +111,7 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
   uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
   for (int level = min(level_p, top); level >= 0; --level) {
     beam_search<LPV, NQ, KPL, false, HASDEL>(c, g, qr, ul, cur, curdist, level, bg.efc, is_update ? p : kInvalid, wc);
-    // ascending dump into the shared-memory list the selection heuristic walks
-    c.cnt = 0;
-    for (;;) {
-      uint64_t key = ul_extract_min<KPL>(ul, c.lane);
-      if (key == kMaxKey) break;
-      if (c.lane == 0) c.keys[c.cnt] = key;
-      c.cnt++;
-    }
-    __syncwarp();
+    ul_extract_all<KPL>(c, ul);  // the list the selection heuristic walks
     if (c.cnt == 0) continue;
     uint32_t nsel = heuristic_select<LPV, NQ>(c, g, g.M, a);
     uint32_t width = level == 0 ? g.M0 : g.M;
@@ -193,14 +185,7 @@ __device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g,
       ul_insert<KPL>(u, hj, ij, keep, cnt, worst_hi, c.lane);
     }
   }
-  c.cnt = 0;
-  for (;;) {
-    uint64_t key = ul_extract_min<KPL>(u, c.lane);
-    if (key == kMaxKey) break;
-    if (c.lane == 0) c.keys[c.cnt] = key;
-    c.cnt++;
-  }
-  __syncwarp();
+  ul_extract_all<KPL>(c, u);
   return heuristic_select<LPV, NQ>(c, g, Mmax, a);
 }
 

@@ -17,9 +17,6 @@ constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persi
 constexpr bool dense_form(bool bf16, int LPV, int NQ, int KPL, bool HASDEL) {
   return LPV == 8 && NQ <= 4 && !HASDEL && (!bf16 || NQ < 4 || KPL < 8);
 }
-// U (4-vector load steps a team warp keeps in flight) of the team walk's wide and narrow forms
-__host__ __device__ constexpr int team_u_wide(int NQ) { return NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2); }
-__host__ __device__ constexpr int team_u_narrow(int NQ) { return NQ <= 2 ? 4 : (NQ <= 4 ? 2 : 1); }
 
 // Which graph-walk kernel a search runs and how it is launched (ehb_index::walk_plan).  The launchers and the
 // reported kernel name read it and decide nothing themselves.

@@ -19,10 +19,7 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   WarpCtx c;
   ctx_init(c, smem + (size_t)w * warp_smem, cfg, g.dpad, (uint32_t)sizeof(RowT));
   float4 qr[NQ];
-  if constexpr (kKeys)
-    load_query_regs_bf16<LPV, NQ>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
-  else
-    load_query_regs<LPV, NQ>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
+  load_query_regs<LPV, NQ, RowT>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
   WalkCounters wc = {0, 0, 0, 0};
   UList<KPL> ul;
   ul_clear<KPL>(ul, ef, c.lane);

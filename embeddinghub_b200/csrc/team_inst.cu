@@ -23,7 +23,7 @@ cudaError_t launch_search_team(const WalkPlan& p, const GraphView& g, const floa
   if (p.form != WalkForm::team || p.bf16 || p.lpv != 8) return cudaErrorInvalidValue;
   return with_dpad<256>(g.dpad, [&](auto d) {
     constexpr int NQ = row_nq(decltype(d)::value, decltype(d)::value * 4u);
-    constexpr uint32_t UW = team_u_wide(NQ), UN = team_u_narrow(NQ);
+    constexpr uint32_t UW = eval_u(NQ, 1), UN = eval_u(NQ, 2);  // wide and narrow U
     // the (T, U) pairs ehb_index::walk_plan chooses: T = 2 and 4 with the wide U, T = 3 and 4 with the narrow one
     const uint32_t T = p.T, U = p.U;
     if (T == 2 && U == UW) return team_kpl<NQ, 2, UW>(p, g, queries, nq, k, ef, out_labels, out_dists, out_counts, stats, s);

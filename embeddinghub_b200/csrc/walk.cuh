@@ -212,16 +212,47 @@ __device__ __forceinline__ bool hash_insert(WarpCtx& c, uint32_t id, uint32_t& o
 }
 
 // ---------------------------------------------------------------------------
-// Query / vector registers: lane `sub = lane % LPV` holds float4 chunks
-// sub + LPV*t, t < NQ  (dpad == 4 * LPV * NQ exactly).
+// Lane chunks: how a lane holds its share of a row.  Lane `sub = lane % LPV`
+// holds the fp32 query as NQ float4 registers (dpad == 4 * LPV * NQ exactly)
+// and reads a row of RowT in chunks of W consecutive values: chunk j covers
+// elements W * (sub + LPV * j) .. + W - 1 and pairs with the V = W / 4 query
+// registers qr[j * V] .. qr[j * V + V - 1].  The chunk kinds:
+//   fp32 rows, W = 4: float4;
+//   bf16 rows, W = 8: uint4 (the walk, NQ >= 2);
+//   bf16 rows, W = 4: uint2 (the walk at NQ = 1, and the fp32 walk's screen at every NQ).
 // ---------------------------------------------------------------------------
-template <int LPV, int NQ>
+template <class RowT, int NQ, int W = (std::is_same<RowT, float>::value || NQ == 1) ? 4 : 8>
+struct LaneChunks {
+  static_assert(W == 4 || (W == 8 && !std::is_same<RowT, float>::value), "no such chunk");
+  using T = std::conditional_t<std::is_same<RowT, float>::value, float4, std::conditional_t<W == 8, uint4, uint2>>;
+  static constexpr int V = W / 4;   // query registers per chunk
+  static constexpr int N = NQ / V;  // chunks per lane
+};
+__device__ __forceinline__ float4 ld_chunk(const float4* p) { return ld_nc_f4(p); }
+__device__ __forceinline__ uint4 ld_chunk(const uint4* p) { return ld_nc_u4(p); }
+__device__ __forceinline__ uint2 ld_chunk(const uint2* p) { return ld_nc_u2(p); }
+// two packed bf16 pairs -> four floats (exact: bf16 is the top half of an fp32)
+__device__ __forceinline__ float4 bf16x4_to_f4(uint32_t a, uint32_t b) {
+  return make_float4(__uint_as_float(a << 16), __uint_as_float(a & 0xFFFF0000u), __uint_as_float(b << 16),
+                     __uint_as_float(b & 0xFFFF0000u));
+}
+// chunk -> its V float4s of row values
+__device__ __forceinline__ void widen(const float4& v, float4* x) { x[0] = v; }
+__device__ __forceinline__ void widen(const uint4& v, float4* x) {
+  x[0] = bf16x4_to_f4(v.x, v.y);
+  x[1] = bf16x4_to_f4(v.z, v.w);
+}
+__device__ __forceinline__ void widen(const uint2& v, float4* x) { x[0] = bf16x4_to_f4(v.x, v.y); }
+
+// the fp32 query in the lane layout of RowT rows (zero past dim)
+template <int LPV, int NQ, class RowT = float>
 __device__ __forceinline__ void load_query_regs(float4 (&qr)[NQ], const float* __restrict__ src, uint32_t dim,
                                                 uint32_t lane) {
+  constexpr int V = LaneChunks<RowT, NQ>::V;
   uint32_t sub = lane % LPV;
 #pragma unroll
   for (int t = 0; t < NQ; ++t) {
-    uint32_t e = (sub + LPV * t) * 4u;
+    uint32_t e = (sub + LPV * (t / V)) * 4u * V + 4u * (t % V);
     float4 v;
     v.x = e + 0 < dim ? src[e + 0] : 0.f;
     v.y = e + 1 < dim ? src[e + 1] : 0.f;
@@ -230,11 +261,13 @@ __device__ __forceinline__ void load_query_regs(float4 (&qr)[NQ], const float* _
     qr[t] = v;
   }
 }
-template <int LPV, int NQ>
-__device__ __forceinline__ void load_vec_regs(float4 (&r)[NQ], const float* __restrict__ row, uint32_t lane) {
-  const float4* r4 = (const float4*)row + (lane % LPV);
+// a lane's chunks of one row (fp32 rows: the row's values, which the build kernels also use as a query)
+template <int LPV, int NQ, class RowT, class C = LaneChunks<RowT, NQ>>
+__device__ __forceinline__ void load_vec_regs(typename C::T (&r)[C::N], const RowT* __restrict__ row,
+                                              uint32_t lane) {
+  const typename C::T* p = (const typename C::T*)row + (lane % LPV);
 #pragma unroll
-  for (int t = 0; t < NQ; ++t) r[t] = r4[LPV * t];
+  for (int t = 0; t < C::N; ++t) r[t] = p[LPV * t];
 }
 
 template <int NQ>
@@ -267,67 +300,12 @@ __device__ __forceinline__ float group_reduce(float acc) {
   return acc;
 }
 
-// ---- bf16 rows -----------------------------------------------------------------------------------------
-// A lane reads its part of a bf16 row in 16-byte chunks of 8 values (one 8-byte chunk of 4 values at
-// dpad = 32).  NQ still counts the fp32 query's float4 registers per lane (dpad == 4 * LPV * NQ), so a lane
-// holds NQ / 2 chunks; chunk j of lane `sub = lane % LPV` is elements 8 * (sub + LPV * j) .. + 7, paired with
-// the query floats in qr[2j] and qr[2j + 1].  At NQ = 1 the layout is the fp32 one.
-template <int NQ>
-struct Bf16Chunks {
-  using T = uint4;
-  static constexpr int N = NQ / 2;
-};
-template <>
-struct Bf16Chunks<1> {
-  using T = uint2;
-  static constexpr int N = 1;
-};
-template <int LPV, int NQ>
-__device__ __forceinline__ void load_query_regs_bf16(float4 (&qr)[NQ], const float* __restrict__ src, uint32_t dim,
-                                                     uint32_t lane) {
-  if constexpr (NQ == 1) {
-    load_query_regs<LPV, 1>(qr, src, dim, lane);
-  } else {
-    uint32_t sub = lane % LPV;
-#pragma unroll
-    for (int t = 0; t < NQ; ++t) {
-      uint32_t e = (sub + LPV * (t >> 1)) * 8u + 4u * (t & 1);
-      float4 v;
-      v.x = e + 0 < dim ? src[e + 0] : 0.f;
-      v.y = e + 1 < dim ? src[e + 1] : 0.f;
-      v.z = e + 2 < dim ? src[e + 2] : 0.f;
-      v.w = e + 3 < dim ? src[e + 3] : 0.f;
-      qr[t] = v;
-    }
-  }
-}
-// two packed bf16 pairs -> four floats (exact: bf16 is the top half of an fp32)
-__device__ __forceinline__ float4 bf16x4_to_f4(uint32_t a, uint32_t b) {
-  return make_float4(__uint_as_float(a << 16), __uint_as_float(a & 0xFFFF0000u), __uint_as_float(b << 16),
-                     __uint_as_float(b & 0xFFFF0000u));
-}
-template <int LPV, int NQ>
-__device__ __forceinline__ void load_vec_regs(typename Bf16Chunks<NQ>::T (&r)[Bf16Chunks<NQ>::N],
-                                              const __nv_bfloat16* __restrict__ row, uint32_t lane) {
-  using CT = typename Bf16Chunks<NQ>::T;
-  const CT* p = (const CT*)row + (lane % LPV);
-#pragma unroll
-  for (int t = 0; t < Bf16Chunks<NQ>::N; ++t) r[t] = p[LPV * t];
-}
-// widened to fp32, then the fp32 chain (fp32 products and accumulation)
-template <int NQ>
-__device__ __forceinline__ float partial_dist(const typename Bf16Chunks<NQ>::T (&v)[Bf16Chunks<NQ>::N],
-                                              const float4 (&qr)[NQ], int metric) {
+// a lane's chunks of a row widened to fp32, then the fp32 chain (fp32 products and accumulation)
+template <int NQ, class RowT, class C = LaneChunks<RowT, NQ>>
+__device__ __forceinline__ float chunk_dist(const typename C::T (&v)[C::N], const float4 (&qr)[NQ], int metric) {
   float4 x[NQ];
-  if constexpr (NQ == 1) {
-    x[0] = bf16x4_to_f4(v[0].x, v[0].y);
-  } else {
 #pragma unroll
-    for (int j = 0; j < NQ / 2; ++j) {
-      x[2 * j] = bf16x4_to_f4(v[j].x, v[j].y);
-      x[2 * j + 1] = bf16x4_to_f4(v[j].z, v[j].w);
-    }
-  }
+  for (int j = 0; j < C::N; ++j) widen(v[j], x + j * C::V);
   return partial_dist<NQ>(x, qr, metric);
 }
 template <class RowT>
@@ -338,74 +316,37 @@ __device__ __forceinline__ const RowT* walk_rows(const GraphView& g) {
     return g.vecs16;
 }
 
-// ---- LPV = 8: direct 128-bit loads, U steps (4 vectors each) in flight ------
-// default U: 64 registers of loads in flight (16 vectors at d <= 128)
-__host__ __device__ constexpr int eval_u(int NQ, int UDIV) {
-  return ((NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2)) / UDIV) > 0 ? (NQ <= 2 ? 8 : (NQ <= 4 ? 4 : 2)) / UDIV : 1;
+// ---- LPV = 8: direct loads, U steps (4 vectors each) in flight --------------
+// U for N chunks per lane: 64 registers of loads in flight (16 vectors of fp32 rows at d <= 128; a bf16 chunk
+// carries twice the values, so the same registers hold twice the vectors, capped at the 32 candidates of a hop).
+// UDIV > 1 divides it (the dense walk and the team walk's narrow form).
+__host__ __device__ constexpr int eval_u(int N, int UDIV) {
+  return ((N <= 2 ? 8 : (N <= 4 ? 4 : 2)) / UDIV) > 0 ? (N <= 2 ? 8 : (N <= 4 ? 4 : 2)) / UDIV : 1;
 }
-template <int NQ, int U = eval_u(NQ, 1)>
-__device__ __forceinline__ void eval_direct(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
+// (the default U is the one of fp32 rows)
+template <int NQ, int U = eval_u(NQ, 1), class RowT = float>
+__device__ __forceinline__ void eval_direct(WarpCtx& c, const RowT* __restrict__ rows, const float4 (&qr)[NQ],
                                             uint32_t m, int metric) {
+  using C = LaneChunks<RowT, NQ>;
   const uint32_t sub = c.lane & 7u, grp = c.lane >> 3;
   __syncwarp();
 #pragma unroll 1
   for (uint32_t j0 = 0; j0 < m; j0 += 4 * U) {
-    float4 v[U][NQ];
+    typename C::T v[U][C::N];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (j0 + 4u * u < m) {                          // warp-uniform
         uint32_t j = min(j0 + 4u * u + grp, m - 1u);  // clamped lanes re-read the last row (same lines)
-        const float4* p = (const float4*)(vecs + (size_t)c.cand_id[j] * c.dpad) + sub;
+        const typename C::T* p = (const typename C::T*)(rows + (size_t)c.cand_id[j] * c.dpad) + sub;
 #pragma unroll
-        for (int t = 0; t < NQ; ++t) v[u][t] = ld_nc_f4(p + 8 * t);
+        for (int t = 0; t < C::N; ++t) v[u][t] = ld_chunk(p + 8 * t);
       }
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (j0 + 4u * u < m) {
         uint32_t j = j0 + 4u * u + grp;
-        float acc = group_reduce<8>(partial_dist<NQ>(v[u], qr, metric));
-        if (sub == 0 && j < m) c.cand_dist[j] = metric == 0 ? acc : 1.0f - acc;
-      }
-    }
-  }
-  __syncwarp();
-}
-
-// bf16 rows: a load step carries half the bytes, so the same 64 registers of loads hold twice the vectors
-// (capped at the 32 candidates of a hop)
-__host__ __device__ constexpr int eval_u_bf16(int NQ, int UDIV) {
-  return ((NQ <= 4 ? 8 : (NQ <= 8 ? 4 : 2)) / UDIV) > 0 ? (NQ <= 4 ? 8 : (NQ <= 8 ? 4 : 2)) / UDIV : 1;
-}
-template <int NQ, int U>
-__device__ __forceinline__ void eval_direct(WarpCtx& c, const __nv_bfloat16* __restrict__ rows,
-                                            const float4 (&qr)[NQ], uint32_t m, int metric) {
-  using CT = typename Bf16Chunks<NQ>::T;
-  constexpr int NC = Bf16Chunks<NQ>::N;
-  const uint32_t sub = c.lane & 7u, grp = c.lane >> 3;
-  __syncwarp();
-#pragma unroll 1
-  for (uint32_t j0 = 0; j0 < m; j0 += 4 * U) {
-    CT v[U][NC];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (j0 + 4u * u < m) {                          // warp-uniform
-        uint32_t j = min(j0 + 4u * u + grp, m - 1u);  // clamped lanes re-read the last row (same lines)
-        const CT* p = (const CT*)(rows + (size_t)c.cand_id[j] * c.dpad) + sub;
-#pragma unroll
-        for (int t = 0; t < NC; ++t) {
-          if constexpr (NQ == 1)
-            v[u][t] = ld_nc_u2(p + 8 * t);
-          else
-            v[u][t] = ld_nc_u4(p + 8 * t);
-        }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (j0 + 4u * u < m) {
-        uint32_t j = j0 + 4u * u + grp;
-        float acc = group_reduce<8>(partial_dist<NQ>(v[u], qr, metric));
+        float acc = group_reduce<8>(chunk_dist<NQ, RowT>(v[u], qr, metric));
         if (sub == 0 && j < m) c.cand_dist[j] = metric == 0 ? acc : 1.0f - acc;
       }
     }
@@ -452,17 +393,9 @@ __device__ __forceinline__ void eval_staged(WarpCtx& c, const RowT* __restrict__
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
-        if constexpr (std::is_same<RowT, float>::value) {
-          const float4* s4 = (const float4*)(c.stage + (size_t)(buf * c.G + v) * c.dpad) + c.lane;
-          float4 x[NQ];
-#pragma unroll
-          for (int t = 0; t < NQ; ++t) x[t] = s4[32 * t];
-          acc[i] = partial_dist<NQ>(x, qr, metric);
-        } else {
-          typename Bf16Chunks<NQ>::T x[Bf16Chunks<NQ>::N];
-          load_vec_regs<32, NQ>(x, (const RowT*)c.stage + (size_t)(buf * c.G + v) * c.dpad, c.lane);
-          acc[i] = partial_dist<NQ>(x, qr, metric);
-        }
+        typename LaneChunks<RowT, NQ>::T x[LaneChunks<RowT, NQ>::N];
+        load_vec_regs<32, NQ>(x, (const RowT*)c.stage + (size_t)(buf * c.G + v) * c.dpad, c.lane);
+        acc[i] = chunk_dist<NQ, RowT>(x, qr, metric);
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
@@ -488,14 +421,10 @@ __device__ __forceinline__ void eval_staged(WarpCtx& c, const RowT* __restrict__
 template <int LPV, int NQ, int UDIV = 1, class RowT = float>
 __device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
                                                 uint32_t m, int metric) {
-  if (LPV == 8) {
-    if constexpr (std::is_same<RowT, float>::value)
-      eval_direct<NQ, eval_u(NQ, UDIV)>(c, vecs, qr, m, metric);
-    else
-      eval_direct<NQ, eval_u_bf16(NQ, UDIV)>(c, vecs, qr, m, metric);
-  } else {
+  if (LPV == 8)
+    eval_direct<NQ, eval_u(LaneChunks<RowT, NQ>::N, UDIV)>(c, vecs, qr, m, metric);
+  else
     eval_staged<NQ>(c, vecs, qr, m, metric);
-  }
 }
 
 // ---- fp32 walk: the bf16 screen (LPV = 32, metric 1) -----------------------------------------------------
@@ -512,7 +441,7 @@ __device__ __forceinline__ float partial_abs_dot(const float4 (&v)[NQ], const fl
   return (a0 + a1) + (a2 + a3);
 }
 // The bf16 shadow rows of cand_id[0..m) go through the fp32 walk's staging ring (twice the rows per group: the same
-// bytes) and are read in the fp32 lane layout (8 bytes = the 4 values of chunk lane + 32 t), so the fp32 query
+// bytes) and are read in W = 4 chunks (uint2), the fp32 rows' lane layout, so the fp32 query
 // registers serve both passes.  Per candidate the warp computes E^ (the fp32 chain over the bf16 row) and
 // S^ = sum |q| |b|, and from them L = RD(RD(1 - E^) - B), B = RU(sc S^ + babs): a lower bound on the distance
 // RN(1 - P^) of the fp32 pass (screen_constant).  A candidate with f2ord(L) >= worst_hi (the hop-start worst of a
@@ -542,13 +471,12 @@ __device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const __nv_bfloat1
 #pragma unroll
       for (int i = 0; i < SV; ++i) {
         uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
-        const uint2* s2 = (const uint2*)((const __nv_bfloat16*)c.stage + (size_t)(buf * G + v) * c.dpad) + c.lane;
+        using C = LaneChunks<__nv_bfloat16, NQ, 4>;
+        const typename C::T* s2 =
+            (const typename C::T*)((const __nv_bfloat16*)c.stage + (size_t)(buf * G + v) * c.dpad) + c.lane;
         float4 x[NQ];
 #pragma unroll
-        for (int t = 0; t < NQ; ++t) {
-          const uint2 w = s2[32 * t];
-          x[t] = bf16x4_to_f4(w.x, w.y);
-        }
+        for (int t = 0; t < C::N; ++t) widen(s2[32 * t], x + t);  // each chunk widened as it is read
         e[i] = partial_dist<NQ>(x, qr, 1);
         s[i] = partial_abs_dot<NQ>(x, qr);
       }
@@ -720,6 +648,18 @@ __device__ __forceinline__ uint64_t ul_extract_min(UList<KPL>& u, uint32_t lane)
     }
   }
   return out;
+}
+// Empties the set into the shared-memory key list c.keys[0..c.cnt) in ascending order.
+template <int KPL>
+__device__ __forceinline__ void ul_extract_all(WarpCtx& c, UList<KPL>& u) {
+  c.cnt = 0;
+  for (;;) {
+    uint64_t key = ul_extract_min<KPL>(u, c.lane);
+    if (key == kMaxKey) break;
+    if (c.lane == 0) c.keys[c.cnt] = key;
+    c.cnt++;
+  }
+  __syncwarp();
 }
 
 // ---------------------------------------------------------------------------
