@@ -9,10 +9,15 @@ OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(SRCS))
 LIB       := embeddinghub_b200/libehb200.so
 
 all: $(LIB) oracle tests/cpp/ann_index_cases tests/cpp/concurrent_search tests/cpp/sharded_two_dev tests/cpp/rwlock_stress \
-     tests/cpp/libbf16_probe.so tests/cpp/ann_index_bf16
+     tests/cpp/libbf16_probe.so tests/cpp/libi8_probe.so tests/cpp/ann_index_bf16
 
 # test-only extern "C" wrappers around the K3 launchers of the shipped library (run by tests/test_gpu_bf16_gemm.py)
 tests/cpp/libbf16_probe.so: tests/cpp/bf16_probe.cu $(CSRC)/kernels.h $(LIB)
+	$(NVCC) $(ARCH) -O2 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC,-Wall -shared -I$(CSRC) $< \
+	  -Lembeddinghub_b200 -lehb200 -Xlinker -rpath,'$$ORIGIN/../../embeddinghub_b200' -o $@
+
+# test-only extern "C" wrapper around the int8 screen-copy conversion (run by tests/test_gpu_walk_screen_int8.py)
+tests/cpp/libi8_probe.so: tests/cpp/i8_probe.cu $(CSRC)/kernels.h $(LIB)
 	$(NVCC) $(ARCH) -O2 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC,-Wall -shared -I$(CSRC) $< \
 	  -Lembeddinghub_b200 -lehb200 -Xlinker -rpath,'$$ORIGIN/../../embeddinghub_b200' -o $@
 

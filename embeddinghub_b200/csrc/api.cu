@@ -41,11 +41,12 @@ ehb::GraphView ehb_index::view() const {
   g.max_level = max_level;
   g.metric = metric == EHB_L2 ? 0 : 1;
   g.vecs16 = nullptr;
-  g.screen_c = 0.f;
+  g.codes8 = nullptr;
+  g.terms8 = nullptr;
   return g;
 }
 
-// The fp32 walk's bf16 screen (walk.cuh beam_search) applies to staged rows (> 1 KB, dpad <= 1536) under 1 - dot.
+// The fp32 walk's int8 screen (walk.cuh beam_search) applies to staged rows (> 1 KB, dpad <= 1536) under 1 - dot.
 // By default it runs for batches of at least kScreenMinBatchPerSm queries per SM: those keep the walk bound by DRAM
 // bandwidth, which the screen relieves; a smaller batch is bound by each warp's chain of memory round trips, to
 // which the screen adds one per hop.
@@ -55,14 +56,22 @@ bool ehb_index::walk_screens(uint64_t nq) const {
   return o_walk_screen > 0 || nq >= (uint64_t)ehb::kScreenMinBatchPerSm * sms;
 }
 
-// The screen is an optimisation: when the shadow does not fit next to the index, the walk runs unscreened.
-int ehb_index::try_screen_shadow() {
+// The screen is an optimisation: when its copy does not fit next to the index, the walk runs unscreened.
+int ehb_index::try_screen_copy() {
   size_t fr = 0, tot = 0;
-  const uint64_t need = std::max<uint64_t>(cap, 1) * (dpad * 2ull + 4ull) + (256ull << 20);
+  const uint64_t need = std::max<uint64_t>(cap, 1) * (dpad + sizeof(float4)) + (256ull << 20);
   bool ok = cudaMemGetInfo(&fr, &tot) == cudaSuccess && fr >= need;
-  if (ok && create_shadow() != EHB_OK) {
-    drop_shadow();
-    ok = false;
+  if (ok) {
+    cudaError_t e = x_i8.grow(std::max<uint64_t>(cap, 1) * dpad, 0, -1, stream);
+    if (e == cudaSuccess) e = x_i8t.grow(std::max<uint64_t>(cap, 1), 0, -1, stream);
+    if (e == cudaSuccess) e = ehb::launch_to_i8(vecs.p, dpad, x_i8.p, x_i8t.p, n, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    screen_copy = e == cudaSuccess;
+    if (!screen_copy) {
+      x_i8.release();
+      x_i8t.release();
+      ok = false;
+    }
   }
   if (!ok) {
     (void)cudaGetLastError();
@@ -160,7 +169,7 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
     p.form = ehb::WalkForm::dense;
   else
     p.form = ehb::WalkForm::plain;
-  p.screen = !bf16 && team == 1 && shadow && walk_screens(nq);
+  p.screen = !bf16 && team == 1 && screen_copy && walk_screens(nq);
   p.cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16, p.form == ehb::WalkForm::dense);
   p.wpb = wpb_for(p.cfg, 0, bf16);
   return p;
@@ -181,12 +190,16 @@ int ehb_index::ensure_capacity(uint64_t want) {
     CU(x_bf16.grow(nc * dpad, n * dpad, -1, stream));
     CU(x_norm.grow(nc, n, -1, stream));
   }
+  if (screen_copy) {
+    CU(x_i8.grow(nc * dpad, n * dpad, -1, stream));
+    CU(x_i8t.grow(nc, n, -1, stream));
+  }
   cap = nc;
   return EHB_OK;
 }
 
-// ---- bf16 shadow ----------------------------------------------------------------------------------------
-// Writer side.  Sized like vecs (capacity rows), so adds within the capacity never reallocate it.
+// ---- copies derived from the rows (index_impl.h) -----------------------------------------------------------
+// Writer side.  Sized like vecs (capacity rows), so adds within the capacity never reallocate them.
 int ehb_index::create_shadow() {
   if (shadow) return EHB_OK;
   CU(x_bf16.grow(std::max<uint64_t>(cap, 1) * dpad, 0, -1, stream));
@@ -197,15 +210,20 @@ int ehb_index::create_shadow() {
   return EHB_OK;
 }
 
-void ehb_index::drop_shadow() {
+void ehb_index::drop_derived() {
   x_bf16.release();
   x_norm.release();
   shadow = false;
+  x_i8.release();
+  x_i8t.release();
+  screen_copy = false;
 }
 
-int ehb_index::shadow_rows(uint64_t first, uint64_t cnt) {
-  if (!shadow || cnt == 0) return EHB_OK;
-  CU(ehb::launch_to_bf16(vecs.p + first * dpad, dpad, x_bf16.p + first * dpad, x_norm.p + first, cnt, dpad, stream));
+int ehb_index::derive_rows(uint64_t first, uint64_t cnt) {
+  if (cnt == 0) return EHB_OK;
+  if (shadow)
+    CU(ehb::launch_to_bf16(vecs.p + first * dpad, dpad, x_bf16.p + first * dpad, x_norm.p + first, cnt, dpad, stream));
+  if (screen_copy) CU(ehb::launch_to_i8(vecs.p + first * dpad, dpad, x_i8.p + first * dpad, x_i8t.p + first, cnt, stream));
   return EHB_OK;
 }
 
@@ -250,7 +268,7 @@ void ehb_index::reset_content() {
   h_deleted.clear();
   pending_updates.clear();
   identity_labels = true;
-  drop_shadow();
+  drop_derived();
 }
 
 // ---- ingest ---------------------------------------------------------------------------------------
@@ -340,7 +358,7 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
       }
       if (contiguous_new) {
         CU(ehb::launch_pad_rows(dsrc, vecs.p + first_new * dpad, m, dim, dpad, metric == EHB_COSINE, stream));
-        RET(shadow_rows(first_new, m));
+        RET(derive_rows(first_new, m));
       } else {
         // rows go to arbitrary ids: one launch per run of consecutive destinations
         uint64_t i = 0;
@@ -349,7 +367,7 @@ int ehb_index::add_rows(uint64_t cnt, const float* src, bool src_is_device, cons
           while (j < m && dst[j] == dst[j - 1] + 1) ++j;
           CU(ehb::launch_pad_rows(dsrc + i * dim, vecs.p + (uint64_t)dst[i] * dpad, j - i, dim, dpad,
                                   metric == EHB_COSINE, stream));
-          RET(shadow_rows(dst[i], j - i));
+          RET(derive_rows(dst[i], j - i));
           i = j;
         }
       }
@@ -631,7 +649,7 @@ int ehb_index::compact() {
   uint64_t lo = 0;
   while (lo < nn && inv[lo] == lo) ++lo;  // rows below the first tombstone stay where they are
   CU(ehb::launch_compact_move_rows(vecs.p, dpad, d_inv.p, lo, nn, stage.p, stage_rows, s));
-  RET(shadow_rows(lo, nn - lo));  // the survivors' rows moved: re-convert them in their new places
+  RET(derive_rows(lo, nn - lo));  // the survivors' rows moved: re-derive them in their new places
   CU(cudaMemcpyAsync(labels.p, labels_new.data(), nn * 8, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(levels.p, levels_new.data(), nn, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(up_off.p, up_off_new.data(), nn * 4, cudaMemcpyHostToDevice, s));
@@ -666,18 +684,19 @@ int ehb_index::compact() {
   return build();
 }
 
-// Searches link pending points lazily, and the first bf16 search creates the bf16 shadow; both need the writer
-// side of the lock.  Another writer may run between the unlock and the lock, so the state is checked again.
+// Searches link pending points lazily, the first bf16 search creates the bf16 shadow and the first screened search
+// the int8 screen copy; all need the writer side of the lock.  Another writer may run between the unlock and the
+// lock, so the state is checked again.
 int ehb_index::ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16, bool screen) {
-  auto screen_wants_shadow = [&] { return screen && !shadow && !screen_no_room; };
-  while (needs_build() || (bf16 && !shadow) || screen_wants_shadow()) {
+  auto screen_wants_copy = [&] { return screen && !screen_copy && !screen_no_room; };
+  while (needs_build() || (bf16 && !shadow) || screen_wants_copy()) {
     lk.unlock();
     int rc;
     {
       std::unique_lock<ehb::RwLock> x(rw);
       rc = build();
       if (rc == EHB_OK && bf16) rc = create_shadow();
-      if (rc == EHB_OK && screen_wants_shadow()) rc = try_screen_shadow();
+      if (rc == EHB_OK && screen_wants_copy()) rc = try_screen_copy();
     }
     lk.lock();
     if (rc != EHB_OK) return rc;
@@ -788,9 +807,8 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     }
     ehb::GraphView g = view();
     if (plan.screen) {
-      g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
-      const double c = ehb::screen_constant(dpad);
-      g.screen_c = (double)(float)c >= c ? (float)c : std::nextafter((float)c, INFINITY);
+      g.codes8 = x_i8.p;
+      g.terms8 = x_i8t.p;
     }
     CU(ehb::launch_search(plan, g, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, s));
   }
@@ -1258,11 +1276,13 @@ int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
       out->dist_evals = ix->last_sum[2];
       out->visited_overflow = ix->last_sum[3];
       // A bf16 walk reads 2 bytes per element, and its re-rank reads the fp32 rows of the retained keys.  A
-      // screened fp32 walk reads 2 bytes per element of every screened candidate, and 4 of the fp32 rows it read.
+      // screened fp32 walk reads 1 byte per element and the 16 bytes of per-row terms of every screened candidate,
+      // and 4 bytes per element of the fp32 rows it read.
       const uint64_t screened = ix->last_sum[4];
       out->algorithmic_bytes = out->hops_upper * 4ull * ix->M + out->hops_base * 4ull * ix->M0 +
-                               (sl->last_bf16 ? out->dist_evals * 2ull : last_fp32_rows(ix) * 4ull + screened * 2ull) *
-                                   ix->dim +
+                               (sl->last_bf16 ? out->dist_evals * 2ull * ix->dim
+                                              : last_fp32_rows(ix) * 4ull * ix->dim +
+                                                    screened * (ix->dim + (uint64_t)sizeof(float4))) +
                                out->queries * 4ull * ix->dim + ix->last_reranked * 4ull * ix->dim;
     }
   }
@@ -1275,7 +1295,7 @@ int ehb_index_stats(ehb_index* ix, ehb_stats* out) {
   out->entry_point = ix->entry;
   out->device_bytes = ix->vecs.bytes() + ix->labels.bytes() + ix->levels.bytes() + ix->deleted.bytes() +
                       ix->links0.bytes() + ix->up_off.bytes() + ix->links_up.bytes() + ix->up_owner.bytes() +
-                      ix->x_bf16.bytes() + ix->x_norm.bytes();
+                      ix->x_bf16.bytes() + ix->x_norm.bytes() + ix->x_i8.bytes() + ix->x_i8t.bytes();
   out->deleted = ix->n_deleted;
   out->combined_batches = ix->combined_batches.load();
   out->combined_queries = ix->combined_queries.load();

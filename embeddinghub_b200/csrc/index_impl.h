@@ -261,14 +261,21 @@ struct ehb_index {
   ehb::DevBuf<float> q_norm2, bf_thr;
   ehb::DevBuf<uint64_t> bf_cbuf;
   ehb::DevBuf<uint32_t> bf_ccount;
-  // The bf16 shadow of the base rows ([cap][dpad] bf16 + squared norms of the rounded rows), read by the bf16
-  // graph walk and the bf16 brute force.  The first bf16 search creates it (writer side of `rw`); from then on
-  // every mutation keeps rows [0, n) equal to bf16(vecs) under the writer lock: add_rows converts the rows it
-  // wrote, ensure_capacity grows it with vecs, compact re-converts the survivors, load / import / reset drop it.
-  // An index that never runs a bf16 search allocates none of it.
+  // Copies derived from the base rows, sized like vecs (capacity rows).  Each is created on the writer side of `rw`
+  // by the first search that needs it, and from then on every mutation keeps rows [0, n) equal to a function of
+  // vecs under the writer lock: add_rows and compact call derive_rows for the rows they wrote or moved,
+  // ensure_capacity grows the copies with vecs, load / import / reset call drop_derived.  An index allocates only the
+  // copies its searches used.
+  //  - The bf16 shadow ([cap][dpad] bf16 + squared norms of the rounded rows): the bf16 graph walk and the bf16 brute
+  //    force.  Created by the first bf16 search.
+  //  - The int8 screen copy ([cap][dpad] int8 codes + [cap] per-row terms, launch_to_i8): the fp32 walk's screen.
+  //    Created by the first screened search when it fits (try_screen_copy).
   ehb::DevBuf<uint16_t> x_bf16;
   ehb::DevBuf<float> x_norm;
   bool shadow = false;
+  ehb::DevBuf<int8_t> x_i8;
+  ehb::DevBuf<float4> x_i8t;
+  bool screen_copy = false;
 
   // build scratch
   ehb::DevBuf<uint32_t> b_edge_row, b_edge_src, b_row_cnt, b_row_fill, b_row_start, b_touched, b_seg_src, b_counters,
@@ -285,8 +292,8 @@ struct ehb_index {
   // guesses are fetched too, which adds DRAM traffic to a walk that is bound by DRAM traffic.
   bool o_walk_prefetch = false;
   // fp32 walk screen (walk.cuh beam_search): -1 = automatic (walk_screens), 0 = off, 1 = on for every batch it applies
-  // to.  It needs the bf16 shadow; when there was no room for it the walk runs unscreened (screen_no_room, cleared
-  // when the option is set again).
+  // to.  It needs the int8 screen copy; when there was no room for it the walk runs unscreened (screen_no_room,
+  // cleared when the option is set again).
   int o_walk_screen = -1;
   bool screen_no_room = false;
 
@@ -314,15 +321,15 @@ struct ehb_index {
   int compact();
   bool needs_build() const { return n_linked != n || !pending_updates.empty(); }
   // (re-)take the writer side until the graph is built and, with bf16, the shadow exists
-  // screen: the fp32 walk of this batch wants the bf16 shadow (walk_screens); it is created if it fits
+  // screen: the fp32 walk of this batch wants the int8 screen copy (walk_screens); it is created if it fits
   int ensure_built(std::shared_lock<ehb::RwLock>& lk, bool bf16 = false, bool screen = false);
-  // whether an fp32 one-warp walk of nq queries screens on the bf16 shadow (given that the shadow exists)
+  // whether an fp32 one-warp walk of nq queries screens on the int8 copy (given that the copy exists)
   bool walk_screens(uint64_t nq) const;
-  int try_screen_shadow();
+  int try_screen_copy();
   int ensure_shadow(std::shared_lock<ehb::RwLock>& lk);
   int create_shadow();
-  void drop_shadow();
-  int shadow_rows(uint64_t first, uint64_t cnt);  // re-convert rows [first, first + cnt) when the shadow exists
+  int derive_rows(uint64_t first, uint64_t cnt);  // re-derive rows [first, first + cnt) of every copy that exists
+  void drop_derived();
   int acquire_slot(ehb::SearchSlot** out);
   void release_slot(ehb::SearchSlot* sl, cudaStream_t used);
   // sink (optional): extra destinations + slice flags for the sharded exchange; *pushed tells whether the

@@ -160,7 +160,7 @@ int adopt_host_tables(ehb_index* ix, uint64_t n, uint64_t upper_rows, std::vecto
   ix->up_rows = upper_rows;
   ix->entry = entry;
   ix->max_level = n ? max_level : -1;
-  ix->drop_shadow();
+  ix->drop_derived();
   ix->pending_updates.clear();
   return EHB_OK;
 }

@@ -27,7 +27,7 @@ struct WalkPlan {
   bool hasdel;         // the index has tombstones
   WalkForm form;
   uint32_t T, U;       // team form: warps per query (2..4) and load steps in flight; 1 and 0 otherwise
-  bool screen;         // the fp32 walk screens candidates on the bf16 shadow (g.vecs16 set by the caller)
+  bool screen;         // the fp32 walk screens candidates on the int8 screen copy (g.codes8 / g.terms8 set by the caller)
   WalkCfg cfg;
   uint32_t wpb;        // warps per block of the one-warp forms
 };
@@ -35,8 +35,8 @@ struct WalkPlan {
 void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes);
 
 // K2 — batched k-NN graph walk (hnswlib searchKnn), one warp per query, plain or dense form.  ef >= k.
-// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.vecs16
-// set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the bf16 shadow (walk.cuh beam_search).
+// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.codes8
+// set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the int8 screen copy (walk.cuh beam_search).
 // With p.bf16 the walk reads the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation) and writes the retained
 // set, not results: sink.keys[nq][k] gets the (ordered distance, internal id) keys nearest-first (call with k = ef
 // to keep all of them) and out_counts the retained count; launch_rerank then produces the fp32 results.
@@ -62,6 +62,10 @@ cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, ui
 // copy [n][dim] -> [n][dpad] with zero padding (and optional normalisation)
 cudaError_t launch_pad_rows(const float* in, float* out, uint64_t n, uint32_t dim, uint32_t dpad, bool normalize,
                             cudaStream_t s);
+// the int8 screen copy of fp32 rows [n][dpad] (GraphView::codes8 / terms8): per row, s = RN(max |x_i| / 127),
+// codes RN(x_i / s) clamped to [-127, 127], and terms (s, max |r_i|, |r|_2, |x|_2) rounded up, r = x - s c computed
+// in double.  An all-zero row has s = 0 and zero terms; a row with a non-finite value or a subnormal s gets NaN terms.
+cudaError_t launch_to_i8(const float* in, uint32_t dpad, int8_t* codes, float4* terms, uint64_t n, cudaStream_t s);
 // sums the per-query stats into out[6] (the overflow word counts queries)
 cudaError_t launch_sum_stats(const uint32_t* stats, uint32_t nq, unsigned long long* out, cudaStream_t s);
 

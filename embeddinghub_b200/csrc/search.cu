@@ -69,6 +69,64 @@ cudaError_t launch_normalize(const float* in, uint32_t in_stride, float* out, ui
   return launch_pad_rows(in, out, n, dim, out_stride, true, s);
 }
 
+// One warp per row.  The residual r = x - s c is exact in double (s has 24 significant bits, c 7, and x and s c are
+// within 31 binades of each other whenever c != 0), so max |r| is exact; the sums of squares are rounded up by far
+// more than their double rounding error before they are rounded up to fp32.
+__global__ void to_i8_rows_kernel(const float* __restrict__ in, uint32_t dpad, int8_t* __restrict__ codes,
+                                  float4* __restrict__ terms, uint64_t n) {
+  const uint64_t row = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const uint32_t lane = threadIdx.x & 31;
+  if (row >= n) return;
+  const float* src = in + row * dpad;
+  float mx = 0.f;
+  bool finite = true;
+  for (uint32_t i = 4 * lane; i < dpad; i += 128) {
+    const float4 v = *(const float4*)(src + i);
+    finite = finite && isfinite(v.x) && isfinite(v.y) && isfinite(v.z) && isfinite(v.w);
+    mx = fmaxf(mx, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+  finite = __all_sync(0xffffffffu, finite);
+  mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
+  const float s = (float)((double)mx / 127.0);
+  const bool bad = !finite || (s != 0.f && s < 0x1p-126f);  // never rejected: NaN terms
+  const double sd = s;
+  double rinf = 0.0, r2 = 0.0, x2 = 0.0;
+  for (uint32_t i = 4 * lane; i < dpad; i += 128) {
+    const float4 v = *(const float4*)(src + i);
+    const float xv[4] = {v.x, v.y, v.z, v.w};
+    uint32_t packed = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const double x = xv[j];
+      const double c = bad || s == 0.f ? 0.0 : fmin(fmax(rint(x / sd), -127.0), 127.0);
+      const double r = x - sd * c;
+      rinf = fmax(rinf, fabs(r));
+      r2 = fma(r, r, r2);
+      x2 = fma(x, x, x2);
+      packed |= (uint32_t)(uint8_t)(int8_t)c << (8 * j);
+    }
+    *(uint32_t*)(codes + row * dpad + i) = packed;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    rinf = fmax(rinf, __shfl_xor_sync(0xffffffffu, rinf, o));
+    r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+    x2 += __shfl_xor_sync(0xffffffffu, x2, o);
+  }
+  if (lane == 0) {
+    const double up = 1.0 + 0x1p-30;
+    terms[row] = bad ? make_float4(NAN, NAN, NAN, NAN)
+                     : make_float4(s, __double2float_ru(rinf), __double2float_ru(sqrt(r2) * up),
+                                   __double2float_ru(sqrt(x2) * up));
+  }
+}
+
+cudaError_t launch_to_i8(const float* in, uint32_t dpad, int8_t* codes, float4* terms, uint64_t n, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  to_i8_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, s>>>(in, dpad, codes, terms, n);
+  return cudaGetLastError();
+}
+
 // per query: hops_upper, hops_base, evals, overflow flag, screened, survivors, 0, 0 -> sums (overflow: queries)
 __global__ void sum_stats_kernel(const uint32_t* __restrict__ stats, uint32_t nq, unsigned long long* out) {
   unsigned long long a[kStatWords] = {};

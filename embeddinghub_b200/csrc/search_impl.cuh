@@ -94,12 +94,13 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
 
 // Register budget of the default form: ptxas chooses (16 vectors in flight per warp).  An explicit
 // minBlocksPerSM changes its heuristics, and a register cap below what the 16 loads in flight need serialises
-// the load batches — so none is given for fp32 rows.  Over bf16 rows the default heuristics leave a few bytes of
-// spills in some shapes; minBlocksPerSM = 1 lets ptxas take the registers instead.
-template <class RowT>
-constexpr int kWalkMinBlocks = std::is_same<RowT, float>::value ? 0 : 1;
+// the load batches — so none is given for fp32 rows that are not screened.  Over bf16 rows, and in the screened fp32
+// walks, the default heuristics leave a few bytes of spills in some shapes; minBlocksPerSM = 1 lets ptxas take the
+// registers instead (a staged walk's occupancy is set by its shared memory, a few warps per SM, not by registers).
+template <class RowT, int LPV, int NQ>
+constexpr int kWalkMinBlocks = std::is_same<RowT, float>::value && !screen_shape(LPV, NQ) ? 0 : 1;
 template <int LPV, int NQ, int KPL, bool HASDEL, class RowT>
-__global__ void __launch_bounds__(128, kWalkMinBlocks<RowT>)
+__global__ void __launch_bounds__(128, (kWalkMinBlocks<RowT, LPV, NQ>))
     hnsw_search_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries, uint32_t nq, uint32_t k, uint32_t ef,
                        const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts,
                        uint32_t* __restrict__ stats, uint32_t warp_smem) {

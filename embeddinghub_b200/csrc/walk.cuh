@@ -43,21 +43,14 @@ struct GraphView {
   uint32_t n, dim, dpad, M, M0, entry;
   int32_t max_level;
   int32_t metric;            // 0 = squared L2, 1 = 1 - dot (IP and cosine)
-  // [n][dpad] bf16 shadow of vecs, else nullptr.  The bf16 graph search walks it; the fp32 walk (metric 1, staged
-  // rows) screens candidates on it when it is set (beam_search).
+  // [n][dpad] bf16 shadow of vecs, else nullptr.  The bf16 graph search walks it.
   const __nv_bfloat16* vecs16;
-  float screen_c;  // fp32 screen: relative error constant of the bound (screen_constant), rounded up
+  // The int8 screen copy of vecs (launch_to_i8), else nullptr: the fp32 walk (metric 1, staged rows) screens
+  // candidates on it when it is set (beam_search).  codes8: [n][dpad] c = RN(x / s) in [-127, 127];
+  // terms8: [n] (s, >= max |r_i|, >= |r|_2, >= |x|_2) with r = x - s c (all NaN: the row is never rejected).
+  const int8_t* codes8;
+  const float4* terms8;
 };
-
-// The fp32 walk's screen (beam_search, DESIGN.md §9).  For b = RN_bf16(x) and any fp32 summation order of the
-// dpad terms, the walk's dot product P^ and the screen's dot product E^ over b satisfy
-//   |P^ - E^| <= (2^-8 + (2 + 2^-8) g) * S + A,   g = n 2^-24 / (1 - n 2^-24),  S = sum |q_i| |b_i|,
-// A covering subnormal inputs and products (flushed or not).  The screen computes S^ >= (1 - g) S in fp32 as well,
-// so the constant is divided by (1 - g), then padded by 2^-20 for the rounding of the constant itself.
-__host__ __device__ inline double screen_constant(uint32_t n) {
-  const double u = 1.0 / 256.0, e = n * 0x1p-24, g = e / (1.0 - e);
-  return (u + (2.0 + u) * g) / (1.0 - g) * (1.0 + 0x1p-20);
-}
 
 struct WalkCfg {
   uint32_t lcap;       // shared-memory key list capacity (0 = none; cold paths only)
@@ -120,8 +113,7 @@ cudaError_t with_dpad(uint32_t dpad, F&& f) {
                                : with_dpad<MaxDpad, I + 1>(dpad, f);
 }
 
-// The fp32 walk's screen applies to staged fp32 rows of dpad 384 .. 1536 (not at dpad 2048: the screen's registers
-// would make ptxas spill in the KPL 2 and 4 walks there).
+// The fp32 walk's screen applies to staged fp32 rows of dpad 384 .. 1536 (dpad 2048: DESIGN.md §9).
 __host__ __device__ constexpr bool screen_shape(int LPV, int NQ) { return LPV == 32 && NQ <= 12; }
 
 // Per-warp shared-memory slice; every region offset is a multiple of 128 B.  vbytes: bytes of one row as the
@@ -132,7 +124,7 @@ __host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t v
   b += align_up(c.hash_size * 4u, 128);
   b += 128;  // cand_id[32]
   b += 128;  // cand_dist[32]
-  b += 128;  // mbarriers (<= 8) + spare
+  b += 128;  // mbarriers (<= 8) + the fp32 screen's per-query terms (ScreenQuery)
   b += align_up(c.dcap * 8u, 128);  // deleted-candidate queue: hi[dcap] | id[dcap]
   b += c.staged ? align_up(c.G * c.NG * vbytes, 128) : 0u;
   return b;
@@ -219,12 +211,15 @@ __device__ __forceinline__ bool hash_insert(WarpCtx& c, uint32_t id, uint32_t& o
 // registers qr[j * V] .. qr[j * V + V - 1].  The chunk kinds:
 //   fp32 rows, W = 4: float4;
 //   bf16 rows, W = 8: uint4 (the walk, NQ >= 2);
-//   bf16 rows, W = 4: uint2 (the walk at NQ = 1, and the fp32 walk's screen at every NQ).
+//   bf16 rows, W = 4: uint2 (the walk at NQ = 1);
+//   int8 rows, W = 4: uint32_t (the fp32 walk's screen, every NQ).
 // ---------------------------------------------------------------------------
-template <class RowT, int NQ, int W = (std::is_same<RowT, float>::value || NQ == 1) ? 4 : 8>
+template <class RowT, int NQ, int W = (std::is_same<RowT, __nv_bfloat16>::value && NQ > 1) ? 8 : 4>
 struct LaneChunks {
-  static_assert(W == 4 || (W == 8 && !std::is_same<RowT, float>::value), "no such chunk");
-  using T = std::conditional_t<std::is_same<RowT, float>::value, float4, std::conditional_t<W == 8, uint4, uint2>>;
+  static_assert(W == 4 || (W == 8 && std::is_same<RowT, __nv_bfloat16>::value), "no such chunk");
+  using T = std::conditional_t<std::is_same<RowT, float>::value, float4,
+                               std::conditional_t<std::is_same<RowT, int8_t>::value, uint32_t,
+                                                  std::conditional_t<W == 8, uint4, uint2>>>;
   static constexpr int V = W / 4;   // query registers per chunk
   static constexpr int N = NQ / V;  // chunks per lane
 };
@@ -243,6 +238,15 @@ __device__ __forceinline__ void widen(const uint4& v, float4* x) {
   x[1] = bf16x4_to_f4(v.z, v.w);
 }
 __device__ __forceinline__ void widen(const uint2& v, float4* x) { x[0] = bf16x4_to_f4(v.x, v.y); }
+// four int8 codes -> four floats, exactly: byte k + 128 is placed in the low mantissa bits of 2^23, and
+// (2^23 + b + 128) - (2^23 + 128) = b is exact in fp32 (a byte permute and an add per value)
+__device__ __forceinline__ void widen(const uint32_t& v, float4* x) {
+  const uint32_t u = v ^ 0x80808080u;
+  x[0] = make_float4(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7540)) - 8388736.0f,
+                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7541)) - 8388736.0f,
+                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7542)) - 8388736.0f,
+                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7543)) - 8388736.0f);
+}
 
 // the fp32 query in the lane layout of RowT rows (zero past dim)
 template <int LPV, int NQ, class RowT = float>
@@ -427,37 +431,36 @@ __device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restri
     eval_staged<NQ>(c, vecs, qr, m, metric);
 }
 
-// ---- fp32 walk: the bf16 screen (LPV = 32, metric 1) -----------------------------------------------------
+// ---- fp32 walk: the int8 screen (LPV = 32, metric 1) -----------------------------------------------------
+// Per-query terms of the screen's bound (beam_search): l1 >= |q|_1, l2 >= |q|_2, a: the walk chain's subnormal term.
+// They live in shared memory behind the mbarriers: held in registers through the walk, they cost spills.
+struct ScreenQuery {
+  float l1, l2, a;
+};
+__device__ __forceinline__ ScreenQuery* screen_query(const WarpCtx& c) { return (ScreenQuery*)(c.mbar + 8); }
+// The int8 codes of cand_id[0..m) go through the fp32 walk's staging ring (four times the rows per group, at most
+// 32: the same bytes) and are read in W = 4 chunks (one u32 of four codes), the fp32 rows' lane layout, so the fp32
+// query registers serve both passes.  Per candidate the warp computes E^ (the fp32 chain over the codes) and, with
+// the row's terms (s, rinf, r2, nx), L = RD(RD(1 - RU(s E^)) - M),
+//   M = RU(gam l2 (2 nx + r2) + min(l1 rinf, l2 r2) + a + s as),  gam = dpad 2^-24 / (1 - dpad 2^-24),
+// as = dpad 2^-118 (the screen chain's subnormal term per unit of scale: codes are integers of magnitude <= 127,
+// so only q and the partial results can be subnormal): a lower bound on the distance RN(1 - P^) of the fp32 pass (DESIGN.md §9).  A candidate with f2ord(L) >= worst_hi
+// (the hop-start worst of a full result set, which only shrinks within the hop) cannot be admitted and is dropped;
+// a non-finite L keeps it.  The survivors move to the front of cand_id in their order, and their count is returned.
+// `unsure` (a bit per cand_id position) moves with them.
 template <int NQ>
-__device__ __forceinline__ float partial_abs_dot(const float4 (&v)[NQ], const float4 (&qr)[NQ]) {
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-  for (int t = 0; t < NQ; ++t) {
-    a0 = fmaf(fabsf(qr[t].x), fabsf(v[t].x), a0);
-    a1 = fmaf(fabsf(qr[t].y), fabsf(v[t].y), a1);
-    a2 = fmaf(fabsf(qr[t].z), fabsf(v[t].z), a2);
-    a3 = fmaf(fabsf(qr[t].w), fabsf(v[t].w), a3);
-  }
-  return (a0 + a1) + (a2 + a3);
-}
-// The bf16 shadow rows of cand_id[0..m) go through the fp32 walk's staging ring (twice the rows per group: the same
-// bytes) and are read in W = 4 chunks (uint2), the fp32 rows' lane layout, so the fp32 query
-// registers serve both passes.  Per candidate the warp computes E^ (the fp32 chain over the bf16 row) and
-// S^ = sum |q| |b|, and from them L = RD(RD(1 - E^) - B), B = RU(sc S^ + babs): a lower bound on the distance
-// RN(1 - P^) of the fp32 pass (screen_constant).  A candidate with f2ord(L) >= worst_hi (the hop-start worst of a
-// full result set, which only shrinks within the hop) cannot be admitted and is dropped; a non-finite L keeps it.
-// The survivors move to the front of cand_id in their order, and their count is returned.  `unsure` (a bit per
-// cand_id position) moves with them.
-template <int NQ>
-__device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const __nv_bfloat16* __restrict__ rows,
-                                                  const float4 (&qr)[NQ], uint32_t m, float sc, float babs,
+__device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], uint32_t m,
                                                   uint32_t worst_hi, uint32_t& unsure) {
-  constexpr int SV = NQ >= 12 ? 2 : 4;  // staged rows per math step (two at dpad 1536: no spills)
-  const uint32_t G = min(2u * c.G, 32u), vbytes = c.dpad * 2u;
+  using C = LaneChunks<int8_t, NQ>;
+  constexpr int SV = 4;  // staged rows per math step
+  const uint32_t G = min(4u * c.G, 32u), vbytes = c.dpad;
   const uint32_t rounds = (m + G - 1) / G;
   const uint32_t pre = min(rounds, c.NG);
+  const bool in = c.lane < m;
   fence_proxy_async();
-  for (uint32_t r = 0; r < pre; ++r) issue_rows(c, rows, r, m, G, vbytes);
+  for (uint32_t r = 0; r < pre; ++r) issue_rows(c, g.codes8, r, m, G, vbytes);
+  // lane j's candidate's row terms, read after the pass (holding them in registers through it costs spills)
+  if (in) prefetch_l2(g.terms8 + c.cand_id[c.lane]);
 #pragma unroll 1
   for (uint32_t r = 0; r < rounds; ++r) {
     uint32_t buf = r % c.NG;
@@ -467,45 +470,50 @@ __device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const __nv_bfloat1
     uint32_t cnt = min(G, m - first);
 #pragma unroll 1
     for (uint32_t v0 = 0; v0 < cnt; v0 += SV) {
-      float e[SV], s[SV];
+      float e[SV];
 #pragma unroll
       for (int i = 0; i < SV; ++i) {
         uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
-        using C = LaneChunks<__nv_bfloat16, NQ, 4>;
-        const typename C::T* s2 =
-            (const typename C::T*)((const __nv_bfloat16*)c.stage + (size_t)(buf * G + v) * c.dpad) + c.lane;
+        const typename C::T* s4 = (const typename C::T*)((const int8_t*)c.stage + (size_t)(buf * G + v) * c.dpad) +
+                                  c.lane;
         float4 x[NQ];
 #pragma unroll
-        for (int t = 0; t < C::N; ++t) widen(s2[32 * t], x + t);  // each chunk widened as it is read
+        for (int t = 0; t < C::N; ++t) widen(s4[32 * t], x + t);
         e[i] = partial_dist<NQ>(x, qr, 1);
-        s[i] = partial_abs_dot<NQ>(x, qr);
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-        for (int i = 0; i < SV; ++i) {
-          e[i] += __shfl_xor_sync(0xffffffffu, e[i], o);
-          s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
-        }
+        for (int i = 0; i < SV; ++i) e[i] += __shfl_xor_sync(0xffffffffu, e[i], o);
       }
       if (c.lane < (uint32_t)SV && v0 + c.lane < cnt) {
-        float ea = e[0], sa = s[0];
+        float ea = e[0];
 #pragma unroll
         for (int i = 1; i < SV; ++i)
-          if (c.lane == (uint32_t)i) ea = e[i], sa = s[i];
-        c.cand_dist[first + v0 + c.lane] = __fsub_rd(__fsub_rd(1.0f, ea), __fmaf_ru(sc, sa, babs));
+          if (c.lane == (uint32_t)i) ea = e[i];
+        c.cand_dist[first + v0 + c.lane] = ea;
       }
     }
     __syncwarp();
     if (r + c.NG < rounds) {
       fence_proxy_async();
-      issue_rows(c, rows, r + c.NG, m, G, vbytes);
+      issue_rows(c, g.codes8, r + c.NG, m, G, vbytes);
     }
   }
   __syncwarp();
-  const bool in = c.lane < m;
-  const float L = in ? c.cand_dist[c.lane] : 0.f;
+  float L = 0.f;
   const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
+  if (in) {
+    const float4 tm = ld_nc_f4(g.terms8 + id);
+    const ScreenQuery sq = *screen_query(c);
+    const float e = (float)c.dpad * 0x1p-24f;  // exact, and so is 1 - e (dpad <= 2048)
+    const float gam = __fdiv_ru(e, 1.0f - e), as = __fmul_ru((float)c.dpad, 0x1p-118f);
+    const float se = __fmul_ru(tm.x, c.cand_dist[c.lane]);
+    float mg = __fmul_ru(__fmul_ru(gam, sq.l2), __fmaf_ru(2.0f, tm.w, tm.z));
+    mg = __fadd_ru(mg, fminf(__fmul_ru(sq.l1, tm.y), __fmul_ru(sq.l2, tm.z)));
+    mg = __fadd_ru(mg, __fmaf_ru(tm.x, as, sq.a));
+    L = __fsub_rd(__fsub_rd(1.0f, se), mg);
+  }
   const bool keep = in && !(isfinite(L) && f2ord(L) >= worst_hi);
   const uint32_t mask = __ballot_sync(0xffffffffu, keep);
   const uint32_t pos = __popc(mask & lanemask_lt());
@@ -692,8 +700,8 @@ __device__ __forceinline__ uint32_t list_insert(WarpCtx& c, uint64_t key, uint32
   return pos;
 }
 
-// screened: evaluations made on the bf16 shadow first (fp32 screen); survivors: those of them whose fp32 row was
-// then read.  An fp32 walk reads evals - screened + survivors fp32 rows.
+// screened: evaluations made on the int8 screen copy first (fp32 screen); survivors: those of them whose fp32 row
+// was then read.  An fp32 walk reads evals - screened + survivors fp32 rows.
 struct WalkCounters {
   uint32_t hops_upper, hops_base, evals, overflow, screened, survivors;
 };
@@ -806,24 +814,38 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 
 // HASDEL = false compiles every trace of the tombstone machinery out (an index without tombstones runs
 // exactly the plain loop: the extra live registers would cost the 16-vector load batches their overlap).
-// The fp32 screen (staged rows up to dpad 1536, metric 1, g.vecs16 set): at a hop that starts with a full result set the hop's
-// candidates are screened on the bf16 shadow first (screen_staged), and only the survivors are evaluated in fp32
-// and offered for admission.  A dropped candidate's fp32 distance is >= the hop-start worst result, so it would
+// The fp32 screen (staged rows up to dpad 1536, metric 1, g.codes8 set): at a hop that starts with a full result set
+// the hop's candidates are screened on the int8 copy first (screen_staged), and only the survivors are evaluated in
+// fp32 and offered for admission.  A dropped candidate's fp32 distance is >= the hop-start worst result, so it would
 // not have been admitted (nor queued, if tombstoned): the walk, its results and its counters stay the same.
 template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
   constexpr bool kScreen = screen_shape(LPV, NQ) && std::is_same<RowT, float>::value;
-  const bool screen = kScreen && g.vecs16 && g.metric == 1;  // warp-uniform
-  float babs = 0.f;  // the bound's absolute term: d (2^-125 max|q| + 2^-124) covers subnormals, flushed or not
+  const bool screen = kScreen && g.codes8 && g.metric == 1;  // warp-uniform
   if (screen) {
-    float mx = 0.f;
+    float mx = 0.f, l1 = 0.f, l2 = 0.f;
 #pragma unroll
-    for (int t = 0; t < NQ; ++t)
-      mx = fmaxf(mx, fmaxf(fmaxf(fabsf(qr[t].x), fabsf(qr[t].y)), fmaxf(fabsf(qr[t].z), fabsf(qr[t].w))));
+    for (int t = 0; t < NQ; ++t) {
+      const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        mx = fmaxf(mx, fabsf(v[j]));
+        l1 = __fadd_ru(l1, fabsf(v[j]));
+        l2 = __fmaf_ru(v[j], v[j], l2);
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {  // sums of non-negative terms rounded up: upper bounds
+      l1 = __fadd_ru(l1, __shfl_xor_sync(0xffffffffu, l1, o));
+      l2 = __fadd_ru(l2, __shfl_xor_sync(0xffffffffu, l2, o));
+    }
     mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
-    babs = __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f));
+    // the walk chain's subnormal inputs and products, flushed or not: d (2^-125 max|q| + 2^-124)
+    if (c.lane == 0)
+      *screen_query(c) = {l1, __fsqrt_ru(l2), __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f))};
+    __syncwarp();
   }
   hash_clear(c);
   ul_clear<KPL>(u, ef, c.lane);
@@ -869,7 +891,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       wc.evals += m;
       if (kScreen && screen && cnt >= ef) {
         wc.screened += m;
-        m = screen_staged<NQ>(c, g.vecs16, qr, m, g.screen_c, babs, worst_hi, unsure);
+        m = screen_staged<NQ>(c, g, qr, m, worst_hi, unsure);
         wc.survivors += m;
       }
       eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);

@@ -83,8 +83,8 @@ typedef struct ehb_stats {
   uint64_t hops_base;
   uint64_t dist_evals;
   uint64_t visited_overflow; /* queries whose visited table filled up          */
-  /* fp32 search: hops_upper*4M + hops_base*8M + fp32_rows*4d + screened*2d + Q*4d, where screened = the
-   * evaluations the walk's bf16 screen made and fp32_rows = evals - screened + the screen's survivors (both from
+  /* fp32 search: hops_upper*4M + hops_base*8M + fp32_rows*4d + screened*(d+16) + Q*4d, where screened = the
+   * evaluations the walk's int8 screen made and fp32_rows = evals - screened + the screen's survivors (both from
    * ehb_index_screen_stats; an unscreened walk has screened = 0 and fp32_rows = evals);
    * bf16 search: hops_upper*4M + hops_base*8M + evals*2d + Q*4d + reranked*4d, reranked = the keys the walk
    * retained and the fp32 re-rank read (min(max(ef, k), reachable live points) per query) */
@@ -92,7 +92,7 @@ typedef struct ehb_stats {
   /* index shape */
   uint64_t size, capacity, upper_rows;
   uint32_t dim, M, max_level, entry_point;
-  uint64_t device_bytes;      /* every device array of the index, the bf16 copy of its rows included      */
+  uint64_t device_bytes;      /* every device array of the index, the bf16 and int8 copies of its rows included */
   uint64_t deleted;           /* tombstones (ehb_index_remove); `size` counts them, like hnswlib   */
   uint64_t combined_batches;  /* batched launches issued by the combining queue of ehb_index_search */
   uint64_t combined_queries;  /* queries those launches carried                                     */
@@ -186,8 +186,8 @@ int ehb_index_search_bruteforce_dev(ehb_index* ix, uint64_t nq, const float* que
                                     void* stream);
 
 int ehb_index_stats(ehb_index* ix, ehb_stats* out);
-/* Counters of the fp32 walk's bf16 screen in the most recent graph search (option "walk_screen"):
- * screened_evals = distance evaluations made on the bf16 copy first, fp32_row_reads = fp32 rows the walk read
+/* Counters of the fp32 walk's int8 screen in the most recent graph search (option "walk_screen"):
+ * screened_evals = distance evaluations made on the int8 copy first (dim code bytes + 16 bytes of per-row terms each), fp32_row_reads = fp32 rows the walk read
  * (evaluations that were not screened plus the screened ones that could still be admitted).  Both count within
  * ehb_stats.dist_evals; a bf16 search reads no fp32 rows in its walk, and 0, 0 is returned before any graph search. */
 int ehb_index_screen_stats(ehb_index* ix, uint64_t* screened_evals, uint64_t* fp32_row_reads);
@@ -302,11 +302,12 @@ int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a pe
  *   "combine"       1 (default): concurrent host searches of <= 256 queries share batched launches
  *   "walk_prefetch" 1: L2-prefetch the speculated next hop's vectors (default 0: it also fetches rows the walk
  *                   never evaluates, extra DRAM traffic for a DRAM-bound walk)
- *   "walk_screen"   the fp32 walk's bf16 screen, for inner product and cosine with 256 < dim <= 1536: once the result set is full, a hop's candidates are first evaluated on the bf16
+ *   "walk_screen"   the fp32 walk's int8 screen, for inner product and cosine with 256 < dim <= 1536: once the
+ *                   result set is full, a hop's candidates are first evaluated on a per-row-scaled int8
  *                   copy of their rows with a rigorous error bound, and only those that could still be admitted
  *                   are read in fp32.  Results, counts and the hop / evaluation counters are exactly those of the
  *                   unscreened walk.  -1 (default): on for batches of at least 4 queries per SM; 0: off; 1: on for
- *                   every batch.  The screen needs the bf16 copy of the rows (2 * dim-padded bytes per vector): a
+ *                   every batch.  The screen needs the int8 copy of the rows (dim-padded + 16 bytes per vector): a
  *                   search it applies to creates it when it fits in free device memory, else the walk runs
  *                   unscreened.
  * ABI change with the sm_90a build: "gemm_2cta" (a two-SM cta_group::2 form of the bf16 GEMM that only

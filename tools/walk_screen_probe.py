@@ -1,11 +1,11 @@
-"""Measures the fp32 walk's bf16 screen (option "walk_screen") against the unscreened walk and prints one JSON line
+"""Measures the fp32 walk's int8 screen (option "walk_screen") against the unscreened walk and prints one JSON line
 per shape.
 
 For each shape the index is built once; then searches with the screen off (0) and at its default (-1) alternate
 in one process, with the L2 flushed before every timed call, and the best of --reps device-event times
 (ehb_index_last_kernel_ms) is kept for each.  Reported per setting: time, queries/s, algorithmic bytes (ehb_stats)
-and their share of the 3.35 TB/s data-sheet HBM bandwidth, the share of evaluations that read an fp32 row and the
-share that were screened (ehb_index_screen_stats), and whether labels, distance bits, counts and the hop /
+and their share of the 3.35 TB/s data-sheet HBM bandwidth, the share of evaluations that read an fp32 row, the
+share that were screened and the share of screened candidates that survived the screen (ehb_index_screen_stats), and whether labels, distance bits, counts and the hop /
 evaluation / overflow counters are identical.  For shapes the screen applies to, --small-batches also times the
 screen forced on (1) against off at batches of a few queries per SM, where the default leaves it off.  The card
 name and power limit are read in the same run.
@@ -62,7 +62,7 @@ def timed(ix, flush, q, k, ef, opts, reps):
     """Alternates the option values; returns {value: (best ms, result, stats)}."""
     best = {o: float("inf") for o in opts}
     res, st = {}, {}
-    for o in opts:                                           # warm-up (the first screened search creates the shadow)
+    for o in opts:                                           # warm-up (the first screened search creates the int8 copy)
         ix.set_option("walk_screen", o)
         ix.search(q, k, ef=ef)
     for _ in range(reps):
@@ -81,6 +81,8 @@ def describe(ms, st, nq):
     return {"ms": round(ms, 3), "qps": round(nq / ms * 1e3), "algorithmic_GB": round(ab / 1e9, 3),
             "hbm_share": round(ab / (ms * 1e-3) / HBM, 3), "fp32_read_share": round(st["fp32_row_reads"] / ev, 4),
             "screened_share": round(st["screened_evals"] / ev, 4),
+            "survivor_share": round((st["fp32_row_reads"] - st["dist_evals"] + st["screened_evals"])
+                                    / max(st["screened_evals"], 1), 4),
             "dist_evals_per_query": round(st["dist_evals"] / nq, 1)}
 
 
