@@ -459,8 +459,11 @@ __device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const GraphView& g
   const bool in = c.lane < m;
   fence_proxy_async();
   for (uint32_t r = 0; r < pre; ++r) issue_rows(c, g.codes8, r, m, G, vbytes);
-  // lane j's candidate's row terms, read after the pass (holding them in registers through it costs spills)
-  if (in) prefetch_l2(g.terms8 + c.cand_id[c.lane]);
+  // lane j's candidate's row terms, loaded together with the codes: they arrive during the pass, so the bound
+  // after it waits on no second round trip
+  const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
+  float4 tm = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (in) tm = ld_nc_f4(g.terms8 + id);
 #pragma unroll 1
   for (uint32_t r = 0; r < rounds; ++r) {
     uint32_t buf = r % c.NG;
@@ -502,9 +505,7 @@ __device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const GraphView& g
   }
   __syncwarp();
   float L = 0.f;
-  const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
   if (in) {
-    const float4 tm = ld_nc_f4(g.terms8 + id);
     const ScreenQuery sq = *screen_query(c);
     const float e = (float)c.dpad * 0x1p-24f;  // exact, and so is 1 - e (dpad <= 2048)
     const float gam = __fdiv_ru(e, 1.0f - e), as = __fmul_ru((float)c.dpad, 0x1p-118f);
@@ -520,9 +521,46 @@ __device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const GraphView& g
   __syncwarp();
   if (keep) c.cand_id[pos] = id;
   if (unsure) unsure = __reduce_or_sync(0xffffffffu, (keep && ((unsure >> c.lane) & 1u)) ? (1u << pos) : 0u);
-  fence_proxy_async();  // the ring's generic reads above, before the fp32 pass's bulk copies into it
+  fence_proxy_async();  // the ring's generic reads above, before the next bulk copies into it
   __syncwarp();
   return __popc(mask);
+}
+
+// The screen's survivors cand_id[0..m) -> cand_dist[0..m) (metric 1): their fp32 rows are loaded straight into
+// registers, SB rows per batch, instead of through the TMA ring, which then carries only int8 rows.  A lane holds
+// the chunks eval_staged reads from the ring (lane l: chunks l, l + 32, ...), and the fp32 chain and the shuffle
+// reduction are eval_staged's, so the distances have the same bits.
+template <int NQ>
+__device__ __forceinline__ void eval_survivors(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
+                                               uint32_t m) {
+  constexpr int SB = NQ <= 24 ? 24 / NQ : 1;  // 24 float4 registers of rows in flight per lane
+#pragma unroll 1
+  for (uint32_t v0 = 0; v0 < m; v0 += SB) {
+    float4 x[SB][NQ];
+#pragma unroll
+    for (int i = 0; i < SB; ++i) {
+      const uint32_t v = min(v0 + (uint32_t)i, m - 1u);  // clamped repeats are discarded below
+      const float4* p = (const float4*)(vecs + (size_t)c.cand_id[v] * c.dpad) + c.lane;
+#pragma unroll
+      for (int t = 0; t < NQ; ++t) x[i][t] = ld_nc_f4(p + 32 * t);
+    }
+    float acc[SB];
+#pragma unroll
+    for (int i = 0; i < SB; ++i) acc[i] = chunk_dist<NQ, float>(x[i], qr, 1);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+      for (int i = 0; i < SB; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+    }
+    if (c.lane < (uint32_t)SB && v0 + c.lane < m) {
+      float a = acc[0];
+#pragma unroll
+      for (int i = 1; i < SB; ++i)
+        if (c.lane == (uint32_t)i) a = acc[i];
+      c.cand_dist[v0 + c.lane] = 1.0f - a;
+    }
+  }
+  __syncwarp();
 }
 
 // ---------------------------------------------------------------------------
@@ -893,8 +931,10 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
         wc.screened += m;
         m = screen_staged<NQ>(c, g, qr, m, worst_hi, unsure);
         wc.survivors += m;
+        eval_survivors<NQ>(c, g.vecs, qr, m);
+      } else {
+        eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
       }
-      eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
       // the speculative row has arrived by now: pull its neighbours' vectors towards L2 while this hop's
       // candidates are inserted (rows <= 1 KB only; a wrong guess costs bandwidth, not correctness)
       if (PREFETCH && LPV == 8 && c.prefetch && spec_row != kInvalid) {

@@ -10,7 +10,9 @@ screens) records the fp32 inner product, the hop-start worst distance, and wheth
 A candidate is kept when L < worst.  The fp32 rounding of the chains is not modelled (it moves L by far less than
 the bounds).  Prints one JSON line: evaluations per query, the screened share, each screen's survivor share, and
 the projected algorithmic bytes per query of the row reads (dim bytes + 16 bytes of per-row terms per int8-screened
-evaluation, 2 dim per bf16-screened one, 4 dim per fp32 row read).
+evaluation, 2 dim per bf16-screened one, 4 dim per fp32 row read).  It also reports the share of screened hops whose
+next node the int8 bounds prove: spec, the closest unexpanded result before the hop's candidates, is expanded next
+when every int8 survivor has L > dist(spec) (no survivor can then come before it or evict it).
 
   python tools/walk_screen_int8_survival.py [--n 200000] [--dim 768] [--queries 300] [--ef 128] [--threads 8]
 """
@@ -54,8 +56,9 @@ def int8_copy(x):
 
 
 def walk(g, x, q, ef, visit):
-    """hnswlib searchKnn (no deletions) under 1 - dot; visit(worst or None, ids, dists) sees each base-layer hop's
-    new candidates with the hop-start worst distance when the result set was full"""
+    """hnswlib searchKnn (no deletions) under 1 - dot; visit(worst or None, spec, ids, dists) sees each base-layer
+    hop's new candidates with the hop-start worst distance when the result set was full, and the distance of the
+    closest unexpanded result at the hop's start (None when there is none)"""
     links0, up_off, links_up = g["links0"], g["up_off"], g["links_up"]
     dist = lambda ids: 1.0 - x[ids] @ q
     cur = int(g["entry"])
@@ -85,7 +88,8 @@ def walk(g, x, q, ef, visit):
             continue
         visited.update(ids.tolist())
         ds = dist(ids)
-        visit(lower if len(top) == ef else None, ids, ds)
+        spec = cand[0][0] if cand and cand[0][0] <= lower else None  # an entry beyond lower was evicted
+        visit(lower if len(top) == ef else None, spec, ids, ds)
         for i, dd in zip(ids.tolist(), ds.tolist()):
             if len(top) < ef or lower > dd:
                 heapq.heappush(cand, (dd, i))
@@ -119,14 +123,14 @@ def main():
     gam = dpad * 2.0 ** -24 / (1 - dpad * 2.0 ** -24)
     cb = bf16_constant(dpad)
     qs = np.random.default_rng(4321).standard_normal((a.queries, d), dtype=np.float32)
-    tot = {"evals": 0, "screened": 0, "bf16_kept": 0, "int8_kept": 0, "admissible": 0}
+    tot = {"evals": 0, "screened": 0, "bf16_kept": 0, "int8_kept": 0, "admissible": 0, "hops": 0, "proven": 0}
     margins = {"bf16": [], "int8": []}
     for q in qs:
         qd = q.astype(np.float64)
         q1, q2 = np.abs(qd).sum(), np.linalg.norm(qd)
         A = dpad * (2.0 ** -125 * np.abs(qd).max() + 2.0 ** -124)
 
-        def visit(worst, ids, ds):
+        def visit(worst, spec, ids, ds):
             tot["evals"] += len(ids)
             if worst is None:
                 return
@@ -138,6 +142,8 @@ def main():
             tot["bf16_kept"] += int((lb < worst).sum())
             tot["int8_kept"] += int((li < worst).sum())
             tot["admissible"] += int((ds < worst).sum())
+            tot["hops"] += 1
+            tot["proven"] += int(spec is not None and bool(np.all(li[li < worst] > spec)))
             margins["bf16"].append(mb)
             margins["int8"].append(mi)
 
@@ -158,7 +164,8 @@ def main():
         "fp32_rows_per_eval_bf16": round((unscreened + sc * kb) / ev, 4),
         "fp32_rows_per_eval_int8": round((unscreened + sc * ki) / ev, 4),
         "row_bytes_per_query_bf16": round(bytes_bf16), "row_bytes_per_query_int8": round(bytes_int8),
-        "row_bytes_ratio": round(bytes_int8 / bytes_bf16, 4)}))
+        "row_bytes_ratio": round(bytes_int8 / bytes_bf16, 4),
+        "int8_proven_next_share": round(tot["proven"] / max(tot["hops"], 1), 4)}))
 
 
 if __name__ == "__main__":
