@@ -83,9 +83,10 @@ int ehb_index::try_screen_copy() {
 
 // ef_eff: beam width; smem_list: capacity of the shared-memory key list (0 for plain searches);
 // jobs: warps (queries or points) of the launch; team: warps sharing one visited table; dense: the launch runs
-// the dense form of the walk (walk_plan).
+// the dense form of the walk (walk_plan); screen: the launch runs a screened fp32 walk, which reads its rows straight
+// into registers and has no TMA ring (its G and NG are unused).
 ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16,
-                                 bool dense) const {
+                                 bool dense, bool screen) const {
   ehb::WalkCfg c;
   const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);  // bytes of a row as the walk reads it
   c.lcap = smem_list;
@@ -126,6 +127,10 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
   // stay inside the 227 KB per-block limit
   while (ehb::warp_smem_bytes(c, vbytes) + 256 > 200 * 1024 && c.hash_size > 512)
     c.hash_size = ehb::align_up(c.hash_size / 2, 32);
+  // A screened walk keeps the visited table sized as above, for five staged warps per SM, so that it revisits and
+  // counts exactly what the unscreened walk does; without the ring that table still leaves room for the ten warps its
+  // 200 registers allow at dpad <= 768 (search_impl.cuh; at C3: 5,152 entries, 21 KB per warp).
+  if (screen) c.staged = 0;
   return c;
 }
 
@@ -170,7 +175,7 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
   else
     p.form = ehb::WalkForm::plain;
   p.screen = !bf16 && team == 1 && screen_copy && walk_screens(nq);
-  p.cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16, p.form == ehb::WalkForm::dense);
+  p.cfg = walk_cfg(ef_eff, 0, nq * team, team, bf16, p.form == ehb::WalkForm::dense, p.screen);
   p.wpb = wpb_for(p.cfg, 0, bf16);
   return p;
 }

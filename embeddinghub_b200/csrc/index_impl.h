@@ -302,9 +302,9 @@ struct ehb_index {
   ~ehb_index();
 
   ehb::GraphView view() const;
-  // bf16: the walk reads the bf16 shadow (rows of dpad * 2 bytes)
+  // bf16: the walk reads the bf16 shadow (rows of dpad * 2 bytes); screen: a screened fp32 walk (no TMA ring)
   ehb::WalkCfg walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16 = false,
-                        bool dense = false) const;
+                        bool dense = false, bool screen = false) const;
   uint32_t wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16 = false) const;
   // every choice of the graph-walk kernel for a search of nq queries with beam ef_eff (the shadow exists if bf16)
   ehb::WalkPlan walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) const;

@@ -27,7 +27,8 @@ struct WalkPlan {
   bool hasdel;         // the index has tombstones
   WalkForm form;
   uint32_t T, U;       // team form: warps per query (2..4) and load steps in flight; 1 and 0 otherwise
-  bool screen;         // the fp32 walk screens candidates on the int8 screen copy (g.codes8 / g.terms8 set by the caller)
+  bool screen;         // the fp32 walk screens candidates on the int8 screen copy (g.codes8 / g.terms8 set by the caller);
+                       // its cfg then has no TMA ring (staged = 0): rows go straight into registers
   WalkCfg cfg;
   uint32_t wpb;        // warps per block of the one-warp forms
 };

@@ -16,6 +16,7 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   const uint32_t q = blockIdx.x * (blockDim.x >> 5) + w;
   if (q >= nq) return;
   constexpr bool kKeys = !std::is_same<RowT, float>::value;
+  constexpr bool kScreen = !kKeys && screen_shape(LPV, NQ);  // can run a screened plan (no ring)
   WarpCtx c;
   ctx_init(c, smem + (size_t)w * warp_smem, cfg, g.dpad, (uint32_t)sizeof(RowT));
   float4 qr[NQ];
@@ -27,12 +28,12 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
     uint32_t cur = g.entry;
     if (c.lane == 0) c.cand_id[0] = cur;
     __syncwarp();
-    eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, 1, g.metric);
+    eval_candidates<LPV, NQ, UDIV, RowT, kScreen>(c, walk_rows<RowT>(g), qr, 1, g.metric);
     float curdist = c.cand_dist[0];
     __syncwarp();
     wc.evals = 1;
-    greedy_descent<LPV, NQ, UDIV, RowT>(c, g, qr, cur, curdist, g.max_level, 0, wc);
-    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV, RowT>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc);
+    greedy_descent<LPV, NQ, UDIV, RowT, kScreen>(c, g, qr, cur, curdist, g.max_level, 0, wc);
+    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV, RowT, kScreen>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc);
   }
   // nearest-first output: extract the k closest in ascending order into registers (element i -> lane i & 31,
   // slot i >> 5), then store them to every destination of the sink with coalesced stores
@@ -94,17 +95,32 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
 
 // Register budget of the default form: ptxas chooses (16 vectors in flight per warp).  An explicit
 // minBlocksPerSM changes its heuristics, and a register cap below what the 16 loads in flight need serialises
-// the load batches — so none is given for fp32 rows that are not screened.  Over bf16 rows, and in the screened fp32
-// walks, the default heuristics leave a few bytes of spills in some shapes; minBlocksPerSM = 1 lets ptxas take the
-// registers instead (a staged walk's occupancy is set by its shared memory, a few warps per SM, not by registers).
-template <class RowT, int LPV, int NQ>
-constexpr int kWalkMinBlocks = std::is_same<RowT, float>::value && !screen_shape(LPV, NQ) ? 0 : 1;
+// the load batches — so none is given for fp32 rows.  Over bf16 rows the default heuristics leave a few bytes of
+// spills in some shapes; minBlocksPerSM = 1 lets ptxas take the registers instead (a staged walk's occupancy is set by
+// its shared memory, a few warps per SM, not by registers).  The fp32 shapes that can screen launch
+// hnsw_search_screen_kernel instead.
+template <class RowT>
+constexpr int kWalkMinBlocks = std::is_same<RowT, float>::value ? 0 : 1;
 template <int LPV, int NQ, int KPL, bool HASDEL, class RowT>
-__global__ void __launch_bounds__(128, (kWalkMinBlocks<RowT, LPV, NQ>))
+__global__ void __launch_bounds__(128, (kWalkMinBlocks<RowT>))
     hnsw_search_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries, uint32_t nq, uint32_t k, uint32_t ef,
                        const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts,
                        uint32_t* __restrict__ stats, uint32_t warp_smem) {
   search_body<LPV, NQ, KPL, HASDEL, 1, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
+}
+
+// The one-warp walk over fp32 rows of the shapes that can screen (screen_shape).  A screened plan has no ring, so
+// registers, not shared memory, set its occupancy: 200 registers allow ten one-warp blocks per SM, and no
+// instantiation up to dpad 768 with KPL <= 8 spills with them (ptxas left alone takes 255, eight blocks; a 168-register
+// cap, twelve, spills hundreds of bytes).  Wider rows (48 query registers at dpad 1536) and KPL = 16 keep 255.
+template <int NQ, int KPL>
+constexpr int kScreenWalkRegs = NQ <= 6 && KPL <= 8 ? 200 : 255;
+template <int LPV, int NQ, int KPL, bool HASDEL>
+__global__ void __maxnreg__((kScreenWalkRegs<NQ, KPL>))
+    hnsw_search_screen_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries, uint32_t nq, uint32_t k,
+                              uint32_t ef, const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts,
+                              uint32_t* __restrict__ stats, uint32_t warp_smem) {
+  search_body<LPV, NQ, KPL, HASDEL, 1, float>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
 // "Dense" form for big batches of short rows (LPV = 8, d <= 128): 8 vectors in flight per warp instead of 16
@@ -121,22 +137,33 @@ __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, 
   search_body<LPV, NQ, KPL, false, 2, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
+using WalkKernel = void (*)(GraphView, WalkCfg, const float*, uint32_t, uint32_t, uint32_t, const ResultSink,
+                           uint32_t*, uint32_t*, uint32_t);
+// the kernel the plan launches (nullptr: the plan asks for a dense form the shape does not have)
+template <int LPV, int NQ, int KPL, class RowT>
+WalkKernel walk_kernel(const WalkPlan& p) {
+  constexpr bool kBf16 = !std::is_same<RowT, float>::value;
+  if (p.form == WalkForm::dense) {
+    if constexpr (dense_form(kBf16, LPV, NQ, KPL, false))
+      if (!p.hasdel) return hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
+    return nullptr;
+  }
+  if constexpr (std::is_same<RowT, float>::value && screen_shape(LPV, NQ))
+    return p.hasdel ? hnsw_search_screen_kernel<LPV, NQ, KPL, true> : hnsw_search_screen_kernel<LPV, NQ, KPL, false>;
+  else
+    return p.hasdel ? hnsw_search_kernel<LPV, NQ, KPL, true, RowT> : hnsw_search_kernel<LPV, NQ, KPL, false, RowT>;
+}
+
 template <int LPV, int NQ, int KPL, class RowT>
 cudaError_t launch_search_t(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
                             uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                             cudaStream_t s) {
-  constexpr bool kBf16 = !std::is_same<RowT, float>::value;
   const uint32_t wpb = p.wpb;
   uint32_t wsm = warp_smem_bytes(p.cfg, g.dpad * (uint32_t)sizeof(RowT));
   size_t smem = (size_t)wsm * wpb;
   dim3 grid((nq + wpb - 1) / wpb), block(32 * wpb);
-  void (*kern)(GraphView, WalkCfg, const float*, uint32_t, uint32_t, uint32_t, const ResultSink, uint32_t*, uint32_t*,
-               uint32_t) = p.hasdel ? hnsw_search_kernel<LPV, NQ, KPL, true, RowT>
-                                    : hnsw_search_kernel<LPV, NQ, KPL, false, RowT>;
-  if (p.form == WalkForm::dense) {
-    if (!dense_form(kBf16, LPV, NQ, KPL, p.hasdel)) return cudaErrorInvalidValue;
-    if constexpr (dense_form(kBf16, LPV, NQ, KPL, false)) kern = hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
-  }
+  const WalkKernel kern = walk_kernel<LPV, NQ, KPL, RowT>(p);
+  if (!kern) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   kern<<<grid, block, smem, s>>>(g, p.cfg, queries, nq, k, ef, sink, out_counts, stats, wsm);

@@ -140,6 +140,7 @@ struct WarpCtx {
   uint32_t* dq_id;
   float* stage;
   uint32_t lcap, hsize, G, NG, dpad, vbytes, dcap, prefetch;
+  uint32_t staged;  // the TMA staging ring is allocated (else LPV = 32 rows are read straight into registers)
   uint32_t phases;  // one parity bit per staging group
   uint32_t cnt;     // live entries in keys[] (shared-memory list only)
   uint32_t lane;
@@ -168,6 +169,7 @@ __device__ __forceinline__ void ctx_init(WarpCtx& c, unsigned char* base, const 
   p += 128;
   c.dcap = cfg.dcap;
   c.prefetch = cfg.prefetch;
+  c.staged = cfg.staged;
   c.dq_hi = (uint32_t*)p;
   c.dq_id = c.dq_hi + cfg.dcap;
   p += align_up(cfg.dcap * 8u, 128);
@@ -211,15 +213,13 @@ __device__ __forceinline__ bool hash_insert(WarpCtx& c, uint32_t id, uint32_t& o
 // registers qr[j * V] .. qr[j * V + V - 1].  The chunk kinds:
 //   fp32 rows, W = 4: float4;
 //   bf16 rows, W = 8: uint4 (the walk, NQ >= 2);
-//   bf16 rows, W = 4: uint2 (the walk at NQ = 1);
-//   int8 rows, W = 4: uint32_t (the fp32 walk's screen, every NQ).
+//   bf16 rows, W = 4: uint2 (the walk at NQ = 1).
+// (The fp32 walk's int8 screen reads its codes in the same layout, a u32 of four codes per chunk: screen_regs.)
 // ---------------------------------------------------------------------------
 template <class RowT, int NQ, int W = (std::is_same<RowT, __nv_bfloat16>::value && NQ > 1) ? 8 : 4>
 struct LaneChunks {
   static_assert(W == 4 || (W == 8 && std::is_same<RowT, __nv_bfloat16>::value), "no such chunk");
-  using T = std::conditional_t<std::is_same<RowT, float>::value, float4,
-                               std::conditional_t<std::is_same<RowT, int8_t>::value, uint32_t,
-                                                  std::conditional_t<W == 8, uint4, uint2>>>;
+  using T = std::conditional_t<std::is_same<RowT, float>::value, float4, std::conditional_t<W == 8, uint4, uint2>>;
   static constexpr int V = W / 4;   // query registers per chunk
   static constexpr int N = NQ / V;  // chunks per lane
 };
@@ -238,15 +238,6 @@ __device__ __forceinline__ void widen(const uint4& v, float4* x) {
   x[1] = bf16x4_to_f4(v.z, v.w);
 }
 __device__ __forceinline__ void widen(const uint2& v, float4* x) { x[0] = bf16x4_to_f4(v.x, v.y); }
-// four int8 codes -> four floats, exactly: byte k + 128 is placed in the low mantissa bits of 2^23, and
-// (2^23 + b + 128) - (2^23 + 128) = b is exact in fp32 (a byte permute and an add per value)
-__device__ __forceinline__ void widen(const uint32_t& v, float4* x) {
-  const uint32_t u = v ^ 0x80808080u;
-  x[0] = make_float4(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7540)) - 8388736.0f,
-                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7541)) - 8388736.0f,
-                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7542)) - 8388736.0f,
-                     __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7543)) - 8388736.0f);
-}
 
 // the fp32 query in the lane layout of RowT rows (zero past dim)
 template <int LPV, int NQ, class RowT = float>
@@ -420,120 +411,16 @@ __device__ __forceinline__ void eval_staged(WarpCtx& c, const RowT* __restrict__
   __syncwarp();
 }
 
-// cand_id[0..m) -> cand_dist[0..m): distances from the register-held query.  UDIV > 1 halves (…) the
-// load batches kept in flight per warp: fewer registers, more resident warps (the "dense" walk).
-template <int LPV, int NQ, int UDIV = 1, class RowT = float>
-__device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
-                                                uint32_t m, int metric) {
-  if (LPV == 8)
-    eval_direct<NQ, eval_u(LaneChunks<RowT, NQ>::N, UDIV)>(c, vecs, qr, m, metric);
-  else
-    eval_staged<NQ>(c, vecs, qr, m, metric);
-}
-
-// ---- fp32 walk: the int8 screen (LPV = 32, metric 1) -----------------------------------------------------
-// Per-query terms of the screen's bound (beam_search): l1 >= |q|_1, l2 >= |q|_2, a: the walk chain's subnormal term.
-// They live in shared memory behind the mbarriers: held in registers through the walk, they cost spills.
-struct ScreenQuery {
-  float l1, l2, a;
-};
-__device__ __forceinline__ ScreenQuery* screen_query(const WarpCtx& c) { return (ScreenQuery*)(c.mbar + 8); }
-// The int8 codes of cand_id[0..m) go through the fp32 walk's staging ring (four times the rows per group, at most
-// 32: the same bytes) and are read in W = 4 chunks (one u32 of four codes), the fp32 rows' lane layout, so the fp32
-// query registers serve both passes.  Per candidate the warp computes E^ (the fp32 chain over the codes) and, with
-// the row's terms (s, rinf, r2, nx), L = RD(RD(1 - RU(s E^)) - M),
-//   M = RU(gam l2 (2 nx + r2) + min(l1 rinf, l2 r2) + a + s as),  gam = dpad 2^-24 / (1 - dpad 2^-24),
-// as = dpad 2^-118 (the screen chain's subnormal term per unit of scale: codes are integers of magnitude <= 127,
-// so only q and the partial results can be subnormal): a lower bound on the distance RN(1 - P^) of the fp32 pass (DESIGN.md §9).  A candidate with f2ord(L) >= worst_hi
-// (the hop-start worst of a full result set, which only shrinks within the hop) cannot be admitted and is dropped;
-// a non-finite L keeps it.  The survivors move to the front of cand_id in their order, and their count is returned.
-// `unsure` (a bit per cand_id position) moves with them.
+// ---- LPV = 32 without the ring: rows straight into registers ----------------------------------------------
+// The walks that screen (WalkCfg::staged == 0) read fp32 rows this way, SB rows per batch (24 float4 registers per
+// lane: eight rows at dpad 384 down to two at 1536; loading the next batch during this one's math would double them,
+// and the kernel would spill at its 200-register budget).  A lane holds the chunks eval_staged reads from the ring
+// (lane l: chunks l, l + 32, ...), and the fp32 chain and the shuffle reduction are eval_staged's, so the distances
+// have the same bits.
 template <int NQ>
-__device__ __forceinline__ uint32_t screen_staged(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], uint32_t m,
-                                                  uint32_t worst_hi, uint32_t& unsure) {
-  using C = LaneChunks<int8_t, NQ>;
-  constexpr int SV = 4;  // staged rows per math step
-  const uint32_t G = min(4u * c.G, 32u), vbytes = c.dpad;
-  const uint32_t rounds = (m + G - 1) / G;
-  const uint32_t pre = min(rounds, c.NG);
-  const bool in = c.lane < m;
-  fence_proxy_async();
-  for (uint32_t r = 0; r < pre; ++r) issue_rows(c, g.codes8, r, m, G, vbytes);
-  // lane j's candidate's row terms, loaded together with the codes: they arrive during the pass, so the bound
-  // after it waits on no second round trip
-  const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
-  float4 tm = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (in) tm = ld_nc_f4(g.terms8 + id);
-#pragma unroll 1
-  for (uint32_t r = 0; r < rounds; ++r) {
-    uint32_t buf = r % c.NG;
-    mbar_wait(&c.mbar[buf], (c.phases >> buf) & 1u);
-    c.phases ^= (1u << buf);
-    uint32_t first = r * G;
-    uint32_t cnt = min(G, m - first);
-#pragma unroll 1
-    for (uint32_t v0 = 0; v0 < cnt; v0 += SV) {
-      float e[SV];
-#pragma unroll
-      for (int i = 0; i < SV; ++i) {
-        uint32_t v = min(v0 + (uint32_t)i, cnt - 1u);  // clamped repeats are discarded below
-        const typename C::T* s4 = (const typename C::T*)((const int8_t*)c.stage + (size_t)(buf * G + v) * c.dpad) +
-                                  c.lane;
-        float4 x[NQ];
-#pragma unroll
-        for (int t = 0; t < C::N; ++t) widen(s4[32 * t], x + t);
-        e[i] = partial_dist<NQ>(x, qr, 1);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-        for (int i = 0; i < SV; ++i) e[i] += __shfl_xor_sync(0xffffffffu, e[i], o);
-      }
-      if (c.lane < (uint32_t)SV && v0 + c.lane < cnt) {
-        float ea = e[0];
-#pragma unroll
-        for (int i = 1; i < SV; ++i)
-          if (c.lane == (uint32_t)i) ea = e[i];
-        c.cand_dist[first + v0 + c.lane] = ea;
-      }
-    }
-    __syncwarp();
-    if (r + c.NG < rounds) {
-      fence_proxy_async();
-      issue_rows(c, g.codes8, r + c.NG, m, G, vbytes);
-    }
-  }
-  __syncwarp();
-  float L = 0.f;
-  if (in) {
-    const ScreenQuery sq = *screen_query(c);
-    const float e = (float)c.dpad * 0x1p-24f;  // exact, and so is 1 - e (dpad <= 2048)
-    const float gam = __fdiv_ru(e, 1.0f - e), as = __fmul_ru((float)c.dpad, 0x1p-118f);
-    const float se = __fmul_ru(tm.x, c.cand_dist[c.lane]);
-    float mg = __fmul_ru(__fmul_ru(gam, sq.l2), __fmaf_ru(2.0f, tm.w, tm.z));
-    mg = __fadd_ru(mg, fminf(__fmul_ru(sq.l1, tm.y), __fmul_ru(sq.l2, tm.z)));
-    mg = __fadd_ru(mg, __fmaf_ru(tm.x, as, sq.a));
-    L = __fsub_rd(__fsub_rd(1.0f, se), mg);
-  }
-  const bool keep = in && !(isfinite(L) && f2ord(L) >= worst_hi);
-  const uint32_t mask = __ballot_sync(0xffffffffu, keep);
-  const uint32_t pos = __popc(mask & lanemask_lt());
-  __syncwarp();
-  if (keep) c.cand_id[pos] = id;
-  if (unsure) unsure = __reduce_or_sync(0xffffffffu, (keep && ((unsure >> c.lane) & 1u)) ? (1u << pos) : 0u);
-  fence_proxy_async();  // the ring's generic reads above, before the next bulk copies into it
-  __syncwarp();
-  return __popc(mask);
-}
-
-// The screen's survivors cand_id[0..m) -> cand_dist[0..m) (metric 1): their fp32 rows are loaded straight into
-// registers, SB rows per batch, instead of through the TMA ring, which then carries only int8 rows.  A lane holds
-// the chunks eval_staged reads from the ring (lane l: chunks l, l + 32, ...), and the fp32 chain and the shuffle
-// reduction are eval_staged's, so the distances have the same bits.
-template <int NQ>
-__device__ __forceinline__ void eval_survivors(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
-                                               uint32_t m) {
-  constexpr int SB = NQ <= 24 ? 24 / NQ : 1;  // 24 float4 registers of rows in flight per lane
+__device__ __forceinline__ void eval_regs(WarpCtx& c, const float* __restrict__ vecs, const float4 (&qr)[NQ],
+                                          uint32_t m, int metric) {
+  constexpr int SB = NQ <= 24 ? 24 / NQ : 1;
 #pragma unroll 1
   for (uint32_t v0 = 0; v0 < m; v0 += SB) {
     float4 x[SB][NQ];
@@ -546,7 +433,7 @@ __device__ __forceinline__ void eval_survivors(WarpCtx& c, const float* __restri
     }
     float acc[SB];
 #pragma unroll
-    for (int i = 0; i < SB; ++i) acc[i] = chunk_dist<NQ, float>(x[i], qr, 1);
+    for (int i = 0; i < SB; ++i) acc[i] = chunk_dist<NQ, float>(x[i], qr, metric);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
@@ -557,10 +444,106 @@ __device__ __forceinline__ void eval_survivors(WarpCtx& c, const float* __restri
 #pragma unroll
       for (int i = 1; i < SB; ++i)
         if (c.lane == (uint32_t)i) a = acc[i];
-      c.cand_dist[v0 + c.lane] = 1.0f - a;
+      c.cand_dist[v0 + c.lane] = metric == 0 ? a : 1.0f - a;
     }
   }
   __syncwarp();
+}
+
+// cand_id[0..m) -> cand_dist[0..m): distances from the register-held query.  UDIV > 1 halves (…) the
+// load batches kept in flight per warp: fewer registers, more resident warps (the "dense" walk).  SCREEN: the
+// instantiation can run a screened plan, which has no ring (c.staged == 0) and reads its rows into registers.
+template <int LPV, int NQ, int UDIV = 1, class RowT = float, bool SCREEN = false>
+__device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
+                                                uint32_t m, int metric) {
+  if (LPV == 8) {
+    eval_direct<NQ, eval_u(LaneChunks<RowT, NQ>::N, UDIV)>(c, vecs, qr, m, metric);
+  } else {
+    if constexpr (SCREEN) {
+      if (!c.staged) {  // warp-uniform
+        eval_regs<NQ>(c, vecs, qr, m, metric);
+        return;
+      }
+    }
+    eval_staged<NQ>(c, vecs, qr, m, metric);
+  }
+}
+
+// ---- fp32 walk: the int8 screen (LPV = 32, metric 1, no ring) ---------------------------------------------
+// The query as integers k = RN(q / sq) with |k| <= kQMax, packed in two signed byte planes k = 128 h + l
+// (h in [-64, 64], l in [-64, 63]) in the codes' lane layout.  kQMax keeps every partial sum of K = sum k_i c_i inside
+// int32 at dpad 1536: kQMax * 127 * 1536 < 2^31.
+constexpr int kQMax = 8191;
+// Per-query terms of the screen's bound (beam_search): l1 >= |q|_1, l2 >= |q|_2, a: the walk chain's subnormal term,
+// en >= |e|_2 for e = q - sq k, and sq.  They live in shared memory behind the mbarriers: held in registers through
+// the walk, they cost spills.
+struct ScreenQuery {
+  float l1, l2, a, en, sq;
+};
+__device__ __forceinline__ ScreenQuery* screen_query(const WarpCtx& c) { return (ScreenQuery*)(c.mbar + 8); }
+// Per candidate of cand_id[0..m) the warp loads the codes straight into registers (RB rows per batch: 96 registers
+// of codes per lane, 32 rows at dpad 384 down to 8 at 1536; loading the next batch during this one's math would
+// double them, and the kernel would spill at its 200-register budget)
+// and computes K = sum k_i c_i exactly, with two dp4a per u32 of codes and one int32 warp reduction.  With the row's
+// terms (s, rinf, r2, nx) it forms L = RD(RD(1 - RU(s sq K)) - M'),
+//   M' = RU(gam l2 nx + min(l1 rinf, l2 r2) + en (nx + r2) + a),  gam = dpad 2^-24 / (1 - dpad 2^-24):
+// a lower bound on the distance RN(1 - P^) of the fp32 pass (DESIGN.md §9).  A candidate with f2ord(L) >= worst_hi
+// (the hop-start worst of a full result set, which only shrinks within the hop) cannot be admitted and is dropped;
+// a non-finite L keeps it.  The survivors move to the front of cand_id in their order, and their count is returned.
+// `unsure` (a bit per cand_id position) moves with them.
+template <int NQ>
+__device__ __forceinline__ uint32_t screen_regs(WarpCtx& c, const GraphView& g, const uint32_t (&qh)[NQ],
+                                                const uint32_t (&ql)[NQ], uint32_t m, uint32_t worst_hi,
+                                                uint32_t& unsure) {
+  constexpr int RB = 96 / NQ;
+  const bool in = c.lane < m;
+  const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
+  // lane j's candidate's row terms, loaded together with the codes
+  float4 tm = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (in) tm = ld_nc_f4(g.terms8 + id);
+  int K = 0;  // lane j: K of candidate j
+#pragma unroll 1
+  for (uint32_t v0 = 0; v0 < m; v0 += RB) {
+    uint32_t x[RB][NQ];
+#pragma unroll
+    for (int i = 0; i < RB; ++i) {
+      const uint32_t* p = (const uint32_t*)(g.codes8 + (size_t)c.cand_id[min(v0 + (uint32_t)i, m - 1u)] * c.dpad) +
+                          c.lane;  // clamped repeats are discarded below
+#pragma unroll
+      for (int t = 0; t < NQ; ++t) x[i][t] = ld_nc_u32(p + 32 * t);
+    }
+#pragma unroll
+    for (int i = 0; i < RB; ++i) {
+      int h = 0, l = 0;
+#pragma unroll
+      for (int t = 0; t < NQ; ++t) {
+        h = __dp4a((int)x[i][t], (int)qh[t], h);
+        l = __dp4a((int)x[i][t], (int)ql[t], l);
+      }
+      const int kv = __reduce_add_sync(0xffffffffu, 128 * h + l);
+      if (c.lane == v0 + (uint32_t)i) K = kv;
+    }
+  }
+  float L = 0.f;
+  if (in) {
+    const ScreenQuery sq = *screen_query(c);
+    const float e = (float)c.dpad * 0x1p-24f;  // exact, and so is 1 - e (dpad <= 2048)
+    const float gam = __fdiv_ru(e, 1.0f - e);
+    // s, sq >= 0: RU(RU(s RU(K)) sq) >= s sq K whatever the sign of K
+    const float se = __fmul_ru(__fmul_ru(tm.x, __int2float_ru(K)), sq.sq);
+    float mg = __fmul_ru(__fmul_ru(gam, sq.l2), tm.w);
+    mg = __fadd_ru(mg, fminf(__fmul_ru(sq.l1, tm.y), __fmul_ru(sq.l2, tm.z)));
+    mg = __fadd_ru(mg, __fmaf_ru(sq.en, __fadd_ru(tm.w, tm.z), sq.a));
+    L = __fsub_rd(__fsub_rd(1.0f, se), mg);
+  }
+  const bool keep = in && !(isfinite(L) && f2ord(L) >= worst_hi);
+  const uint32_t mask = __ballot_sync(0xffffffffu, keep);
+  const uint32_t pos = __popc(mask & lanemask_lt());
+  __syncwarp();
+  if (keep) c.cand_id[pos] = id;
+  if (unsure) unsure = __reduce_or_sync(0xffffffffu, (keep && ((unsure >> c.lane) & 1u)) ? (1u << pos) : 0u);
+  __syncwarp();
+  return __popc(mask);
 }
 
 // ---------------------------------------------------------------------------
@@ -762,7 +745,7 @@ __device__ __forceinline__ uint32_t load_row(const GraphView& g, uint32_t node, 
 
 // hnswlib searchKnn's upper-layer descent: at each level move to the closest
 // neighbour until no neighbour improves.
-template <int LPV, int NQ, int UDIV = 1, class RowT = float>
+template <int LPV, int NQ, int UDIV = 1, class RowT = float, bool SCREEN = false>
 __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], uint32_t& cur,
                                                float& curdist, int from_level, int to_level_excl,
                                                WalkCounters& wc) {
@@ -779,7 +762,7 @@ __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, c
       if (nb != kInvalid) c.cand_id[__popc(mask & lanemask_lt())] = nb;
       __syncwarp();
       wc.evals += m;
-      eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
+      eval_candidates<LPV, NQ, UDIV, RowT, SCREEN>(c, walk_rows<RowT>(g), qr, m, g.metric);
       float bd = c.lane < m ? c.cand_dist[c.lane] : INFINITY;
       uint32_t bl = c.lane;
 #pragma unroll
@@ -852,16 +835,18 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 
 // HASDEL = false compiles every trace of the tombstone machinery out (an index without tombstones runs
 // exactly the plain loop: the extra live registers would cost the 16-vector load batches their overlap).
-// The fp32 screen (staged rows up to dpad 1536, metric 1, g.codes8 set): at a hop that starts with a full result set
-// the hop's candidates are screened on the int8 copy first (screen_staged), and only the survivors are evaluated in
-// fp32 and offered for admission.  A dropped candidate's fp32 distance is >= the hop-start worst result, so it would
-// not have been admitted (nor queued, if tombstoned): the walk, its results and its counters stay the same.
-template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float>
+// The fp32 screen (SCREEN instantiations: fp32 rows of dpad 384 .. 1536; metric 1, g.codes8 set, no ring): at a hop
+// that starts with a full result set the hop's candidates are screened on the int8 copy first (screen_regs), and only
+// the survivors are evaluated in fp32 and offered for admission.  A dropped candidate's fp32 distance is >= the
+// hop-start worst result, so it would not have been admitted (nor queued, if tombstoned): the walk, its results and
+// its counters stay the same.
+template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float, bool SCREEN = false>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
-  constexpr bool kScreen = screen_shape(LPV, NQ) && std::is_same<RowT, float>::value;
-  const bool screen = kScreen && g.codes8 && g.metric == 1;  // warp-uniform
+  static_assert(!SCREEN || (screen_shape(LPV, NQ) && std::is_same<RowT, float>::value), "no screen for this shape");
+  const bool screen = SCREEN && g.codes8 && g.metric == 1;  // warp-uniform
+  uint32_t qh[NQ], ql[NQ];  // the screen's integer query planes (kQMax)
   if (screen) {
     float mx = 0.f, l1 = 0.f, l2 = 0.f;
 #pragma unroll
@@ -880,9 +865,34 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       l2 = __fadd_ru(l2, __shfl_xor_sync(0xffffffffu, l2, o));
     }
     mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
+    // k = RN(q / sq) clamped to +-kQMax, and e = q - sq k, exact in double (sq k has at most 38 significant bits and
+    // lies within 14 binades of q when k != 0).  A zero, tiny or non-finite max |q| gets sq = 0: k = 0 and e = q (a
+    // NaN or infinite element then makes en non-finite, and every candidate is kept).
+    float sq = mx / (float)kQMax;
+    if (!(sq >= 0x1p-126f && sq <= 0x1.fffffep127f)) sq = 0.f;
+    double e2 = 0.0;
+#pragma unroll
+    for (int t = 0; t < NQ; ++t) {
+      const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
+      uint32_t h = 0, l = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int k = sq != 0.f ? max(-kQMax, min(kQMax, __float2int_rn(v[j] / sq))) : 0;
+        const double e = (double)v[j] - (double)sq * (double)k;
+        e2 = __fma_ru(e, e, e2);
+        const int kh = (k + 64) >> 7;  // floor: k - 128 kh in [-64, 63]
+        h |= (uint32_t)(kh & 0xFF) << (8 * j);
+        l |= (uint32_t)((k - 128 * kh) & 0xFF) << (8 * j);
+      }
+      qh[t] = h;
+      ql[t] = l;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) e2 = __dadd_ru(e2, __shfl_xor_sync(0xffffffffu, e2, o));
     // the walk chain's subnormal inputs and products, flushed or not: d (2^-125 max|q| + 2^-124)
     if (c.lane == 0)
-      *screen_query(c) = {l1, __fsqrt_ru(l2), __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f))};
+      *screen_query(c) = {l1, __fsqrt_ru(l2), __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f)),
+                          __double2float_ru(__dsqrt_ru(e2)), sq};
     __syncwarp();
   }
   hash_clear(c);
@@ -927,13 +937,13 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       uint32_t unsure = (HASDEL && del) ? __reduce_or_sync(0xffffffffu, (is_new && o) ? (1u << pos) : 0u) : 0u;
       __syncwarp();
       wc.evals += m;
-      if (kScreen && screen && cnt >= ef) {
+      if (SCREEN && screen && cnt >= ef) {
         wc.screened += m;
-        m = screen_staged<NQ>(c, g, qr, m, worst_hi, unsure);
+        m = screen_regs<NQ>(c, g, qh, ql, m, worst_hi, unsure);
         wc.survivors += m;
-        eval_survivors<NQ>(c, g.vecs, qr, m);
+        eval_regs<NQ>(c, g.vecs, qr, m, 1);
       } else {
-        eval_candidates<LPV, NQ, UDIV>(c, walk_rows<RowT>(g), qr, m, g.metric);
+        eval_candidates<LPV, NQ, UDIV, RowT, SCREEN>(c, walk_rows<RowT>(g), qr, m, g.metric);
       }
       // the speculative row has arrived by now: pull its neighbours' vectors towards L2 while this hop's
       // candidates are inserted (rows <= 1 KB only; a wrong guess costs bandwidth, not correctness)

@@ -234,8 +234,9 @@ int ehb_merge_topk_packed_dev(uint32_t G, uint64_t nq, uint32_t k, const void* p
 int ehb_index_set_search_width(ehb_index* ix, uint32_t warps_per_query);
 
 /* Search tuning knobs (advanced; 0 = automatic).  stage_slots: vectors staged
- * per TMA group; stage_groups: groups in flight per warp; hash_bits: log2 of the
- * per-warp visited table. */
+ * per TMA group; stage_groups: groups in flight per warp (neither applies to a
+ * screened fp32 walk, which has no TMA ring); hash_bits: log2 of the per-warp
+ * visited table. */
 int ehb_index_set_tuning(ehb_index* ix, uint32_t stage_slots, uint32_t stage_groups, uint32_t hash_bits,
                          uint32_t warps_per_block);
 
