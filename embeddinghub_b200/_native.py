@@ -120,6 +120,7 @@ SYMBOLS = {
     "ehb_exchange_begin": (C.c_int, [_VP, _U64, _U32, C.POINTER(_VP), C.POINTER(_VP)]),
     "ehb_exchange_merge_dev": (C.c_int, [_VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_search_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP, _VP, _VP]),
+    "ehb_exchange_search_ex_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_timed_out": (C.c_int, [_VP, C.POINTER(_U32)]),
 }
 

@@ -769,10 +769,10 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   uint32_t ef_eff = std::max(ef_in ? ef_in : ef, k);
   if (ef_eff > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
   const bool bf16 = precision == EHB_BF16;
-  if (bf16 && sink) return fail(EHB_ERR_INVALID, "the fused shard exchange walks fp32 rows only");
   if (bf16 && !shadow) return fail(EHB_ERR_STATE, "bf16 shadow missing");
   const ehb::WalkPlan plan = walk_plan(nq, ef_eff, bf16);
-  if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team;  // the team walk writes destination 0 only
+  // the team walk writes destination 0 only (a bf16 search never plans one: its re-rank stores to every destination)
+  if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team;
   if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
   const float* q = dq;
   if (metric == EHB_COSINE) {
@@ -790,15 +790,20 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   }
   CU(cudaEventRecord(sl->ev0, s));
   if (bf16) {
-    // walk the bf16 rows keeping the whole retained set, then re-rank it with the canonical fp32 chain
+    // walk the bf16 rows keeping the whole retained set, then re-rank it with the canonical fp32 chain (with a
+    // sink, the re-rank stores into every destination and raises the slice flags, as the fp32 walk's epilogue does)
     ehb::ResultSink ks;
     std::memset(&ks, 0, sizeof(ks));
     ks.keys = sl->walk_keys.p;
     ehb::GraphView g = view();
     g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
     CU(ehb::launch_search(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, s));
-    CU(ehb::launch_rerank(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
-                          labels.p, nq, k, dl, dd, dc, s));
+    if (sink)
+      CU(ehb::launch_rerank_sink(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
+                                 labels.p, nq, k, *sink, dc, s));
+    else
+      CU(ehb::launch_rerank(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
+                            labels.p, nq, k, dl, dd, dc, s));
   } else if (plan.form == ehb::WalkForm::team) {
     CU(ehb::launch_search_team(plan, view(), q, (uint32_t)nq, k, ef_eff, dl, dd, dc, sl->stats.p, s));
   } else {
@@ -1196,16 +1201,18 @@ int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k
 
 }  // extern "C"
 
-int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef,
+int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed) {
   ENTER_S(ix);
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (!dq || !sink || !sink->n || !sink->labels[0]) return fail(EHB_ERR_INVALID, "null buffer");
   if (k == 0 || nq == 0) return EHB_OK;
-  RET(ix->ensure_built(_g, false, ix->walk_screens(nq)));
+  const bool bf16 = precision == EHB_BF16;
+  RET(ix->ensure_built(_g, bf16, !bf16 && ix->walk_screens(nq)));
   ehb::SearchSlot* sl = nullptr;
   RET(ix->acquire_slot(&sl));
   cudaStream_t s = stream ? stream : sl->stream;
-  int rc = ix->search_dev(sl, nq, dq, k, ef, sink->labels[0], sink->dists[0], dc, s, sink, pushed);
+  int rc = ix->search_dev(sl, nq, dq, k, ef, sink->labels[0], sink->dists[0], dc, s, sink, pushed, precision);
   ix->release_slot(sl, s);
   return rc;
 }

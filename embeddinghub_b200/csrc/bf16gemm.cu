@@ -408,12 +408,16 @@ cudaError_t launch_bf16_dist_tile(const void* q_bf16, uint64_t q_rows, const voi
 // ---- fp32 re-rank of the bf16 candidates (canonical arithmetic, total order (dist, index)) ----------------
 // One warp per query: candidates cand[q][kc] (keys from the select pass: low 32 bits = row index), exact
 // distance per candidate by lane-strided loop over candidates (each lane runs the sequential FMA chain),
-// then the k best by repeated warp arg-min.
-__global__ void rerank_kernel(const uint64_t* __restrict__ cand, uint32_t kc, const float* __restrict__ qpad,
-                              const float* __restrict__ vecs, uint32_t dpad, uint32_t dim, int metric,
-                              const uint64_t* __restrict__ labels, uint64_t nq, uint32_t k,
-                              uint64_t* __restrict__ out_labels, float* __restrict__ out_dists,
-                              uint32_t* __restrict__ out_counts) {
+// then the k best by repeated warp arg-min.  kSink: the results go to every destination of `sink` (sink_store and
+// sink_query_done, walk.cuh) instead of out_labels / out_dists: the k selected keys are collected in shared memory
+// first (the row tile is free by then), then every lane stores its elements of the list to each destination,
+// coalesced.
+template <bool kSink>
+__device__ __forceinline__ void rerank_body(const uint64_t* __restrict__ cand, uint32_t kc, const float* __restrict__ qpad,
+                                            const float* __restrict__ vecs, uint32_t dpad, uint32_t dim, int metric,
+                                            const uint64_t* __restrict__ labels, uint64_t nq, uint32_t k,
+                                            uint64_t* __restrict__ out_labels, float* __restrict__ out_dists,
+                                            const ResultSink& sink, uint32_t* __restrict__ out_counts) {
   extern __shared__ uint64_t skeys[];  // [wpb][kc] keys, then [wpb][32][33] row tile, [wpb][32] query segment
   const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   const uint64_t q = (uint64_t)blockIdx.x * wpb + w;
@@ -421,6 +425,7 @@ __global__ void rerank_kernel(const uint64_t* __restrict__ cand, uint32_t kc, co
   uint64_t* keys = skeys + (size_t)w * kc;
   float* tile = (float*)(skeys + (size_t)wpb * kc) + (size_t)w * (32 * 33 + 32);
   float* qseg = tile + 32 * 33;
+  uint64_t* sel = (uint64_t*)tile;  // kSink: the selected keys (the tile and query segment hold 544 >= kMaxEf)
   const float* qv = qpad + q * dpad;
   // 32 candidates at a time: rows are staged 32 floats per row per step with coalesced loads, then every
   // lane advances the canonical (k ascending, single accumulator) chain of ITS candidate by 32 terms
@@ -465,26 +470,65 @@ __global__ void rerank_kernel(const uint64_t* __restrict__ cand, uint32_t kc, co
     }
     if (best == kMaxKey) break;
     if (lane == 0) {
-      out_labels[q * k + i] = labels[(uint32_t)best];
-      if (out_dists) out_dists[q * k + i] = key_dist(best);
+      if constexpr (kSink) {
+        sel[i] = best;
+      } else {
+        out_labels[q * k + i] = labels[(uint32_t)best];
+        if (out_dists) out_dists[q * k + i] = key_dist(best);
+      }
       keys[bpos] = kMaxKey;
     }
     __syncwarp();
     found++;
   }
-  for (uint32_t i = found + lane; i < k; i += 32) {
-    out_labels[q * k + i] = 0xFFFFFFFFFFFFFFFFull;
-    if (out_dists) out_dists[q * k + i] = INFINITY;
+  if constexpr (kSink) {
+    for (uint32_t i = found + lane; i < k; i += 32) sel[i] = kMaxKey;
+    __syncwarp();
+    for (uint32_t i = lane; i < k; i += 32) {
+      const uint64_t key = sel[i];
+      const bool ok = key != kMaxKey;
+      sink_store(sink, (size_t)q * k + i, ok ? labels[(uint32_t)key] : 0xFFFFFFFFFFFFFFFFull,
+                 ok ? key_dist(key) : INFINITY);
+    }
+    sink_query_done(sink, (uint32_t)q, (uint32_t)nq, lane);
+  } else {
+    for (uint32_t i = found + lane; i < k; i += 32) {
+      out_labels[q * k + i] = 0xFFFFFFFFFFFFFFFFull;
+      if (out_dists) out_dists[q * k + i] = INFINITY;
+    }
   }
   if (lane == 0 && out_counts) out_counts[q] = found;
+}
+
+__global__ void rerank_kernel(const uint64_t* __restrict__ cand, uint32_t kc, const float* __restrict__ qpad,
+                              const float* __restrict__ vecs, uint32_t dpad, uint32_t dim, int metric,
+                              const uint64_t* __restrict__ labels, uint64_t nq, uint32_t k,
+                              uint64_t* __restrict__ out_labels, float* __restrict__ out_dists,
+                              uint32_t* __restrict__ out_counts) {
+  rerank_body<false>(cand, kc, qpad, vecs, dpad, dim, metric, labels, nq, k, out_labels, out_dists, ResultSink{},
+                     out_counts);
+}
+
+// The re-rank of a bf16 graph walk that is the last kernel of a sharded search step: destination 0 is this shard's
+// block, the others are its block in every peer's receive buffer, and the slice flags rise as queries finish.
+__global__ void rerank_sink_kernel(const uint64_t* __restrict__ cand, uint32_t kc, const float* __restrict__ qpad,
+                                   const float* __restrict__ vecs, uint32_t dpad, uint32_t dim, int metric,
+                                   const uint64_t* __restrict__ labels, uint64_t nq, uint32_t k,
+                                   const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts) {
+  rerank_body<true>(cand, kc, qpad, vecs, dpad, dim, metric, labels, nq, k, nullptr, nullptr, sink, out_counts);
+}
+
+constexpr uint32_t kRerankWarps = 4;
+static size_t rerank_smem(uint32_t kc) {
+  return (size_t)kRerankWarps * kc * 8 + (size_t)kRerankWarps * (32 * 33 + 32) * 4;
 }
 
 cudaError_t launch_rerank(const uint64_t* cand, uint32_t kc, const float* qpad, const float* vecs, uint32_t dpad,
                           uint32_t dim, int metric, const uint64_t* labels, uint64_t nq, uint32_t k,
                           uint64_t* out_labels, float* out_dists, uint32_t* out_counts, cudaStream_t s) {
   if (nq == 0) return cudaSuccess;
-  uint32_t wpb = 4;
-  size_t smem = (size_t)wpb * kc * 8 + (size_t)wpb * (32 * 33 + 32) * 4;
+  const uint32_t wpb = kRerankWarps;
+  const size_t smem = rerank_smem(kc);
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(rerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -492,6 +536,22 @@ cudaError_t launch_rerank(const uint64_t* cand, uint32_t kc, const float* qpad, 
   rerank_kernel<<<(unsigned)((nq + wpb - 1) / wpb), 32 * wpb, smem, s>>>(cand, kc, qpad, vecs, dpad, dim, metric,
                                                                          labels, nq, k, out_labels, out_dists,
                                                                          out_counts);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rerank_sink(const uint64_t* cand, uint32_t kc, const float* qpad, const float* vecs, uint32_t dpad,
+                               uint32_t dim, int metric, const uint64_t* labels, uint64_t nq, uint32_t k,
+                               const ResultSink& sink, uint32_t* out_counts, cudaStream_t s) {
+  if (nq == 0) return cudaSuccess;
+  if (k > kMaxEf || nq > 0xFFFFFFFFull || !sink.n) return cudaErrorInvalidValue;
+  const uint32_t wpb = kRerankWarps;
+  const size_t smem = rerank_smem(kc);
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(rerank_sink_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  rerank_sink_kernel<<<(unsigned)((nq + wpb - 1) / wpb), 32 * wpb, smem, s>>>(cand, kc, qpad, vecs, dpad, dim, metric,
+                                                                              labels, nq, k, sink, out_counts);
   return cudaGetLastError();
 }
 

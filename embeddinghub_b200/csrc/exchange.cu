@@ -280,16 +280,24 @@ int ehb_exchange_merge_dev(ehb_exchange* ex, float* out_dists_dev, uint64_t* out
   return launch_exchange_merge(ex, nq, k, out_dists_dev, out_labels_dev, out_counts_dev, (cudaStream_t)stream, false);
 }
 
-// One sharded graph search step, fused: this rank's walk stores every query's top-k straight into every peer's
-// receive buffer from its epilogue (coalesced stores over NVLink while the other queries are still walking) and
-// raises per-slice flags; then one kernel waits for the peers' flags and merges.  Falls back to push-after-walk
-// when the batch is small enough for the team walk.  Call in lock step on every rank.
-int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
-                            uint32_t ef, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
-                            uint32_t* shard_counts_dev, void* stream) {
+// One sharded graph search step, fused: this rank's search stores every query's top-k straight into every peer's
+// receive buffer from its last kernel (the fp32 walk's epilogue, or the re-rank after a bf16 walk: coalesced stores
+// over NVLink while the other queries are still running) and raises per-slice flags; then one kernel waits for the
+// peers' flags and merges.  Falls back to push-after-walk when the batch is small enough for the team walk (fp32
+// only).  Call in lock step on every rank.  Everything that can be rejected is checked before the epoch advances:
+// a rank that failed after it would be one step out of phase with its peers, whose merges would then wait for it
+// until they time out.
+int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                               uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
+                               uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream) {
   if (!ex || !ix || !queries_dev || !out_labels_dev) return fail(EHB_ERR_INVALID, "null argument");
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (nq == 0 || k == 0 || nq * k > ex->max_elems) return fail(EHB_ERR_INVALID, "nq * k exceeds the exchange capacity");
   if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
+  {
+    std::shared_lock<ehb::RwLock> lk(ix->rw);  // ef == 0 reads the index default
+    if (std::max(ef ? ef : ix->ef, k) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
+  }
   CU(cudaSetDevice(ex->device));
   std::lock_guard<std::mutex> g(ex->mu);
   ex->epoch++;
@@ -315,9 +323,17 @@ int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const 
   sink.epoch = ex->epoch;
   sink.slice_count = ex->slice_count;
   bool pushed = false;
-  RET(ehb_index_search_dev_sink(ix, nq, queries_dev, k, ef, &sink, shard_counts_dev, (cudaStream_t)stream, &pushed));
+  RET(ehb_index_search_dev_sink(ix, nq, queries_dev, k, ef, precision, &sink, shard_counts_dev, (cudaStream_t)stream,
+                                &pushed));
   CU(cudaSetDevice(ex->device));
   return launch_exchange_merge(ex, nq, k, out_dists_dev, out_labels_dev, out_counts_dev, (cudaStream_t)stream, pushed);
+}
+
+int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                            uint32_t ef, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
+                            uint32_t* shard_counts_dev, void* stream) {
+  return ehb_exchange_search_ex_dev(ex, ix, nq, queries_dev, k, ef, EHB_FP32, out_dists_dev, out_labels_dev,
+                                    out_counts_dev, shard_counts_dev, stream);
 }
 
 // 1 when some exchange kernel of this rank gave up waiting for a peer (its results are then invalid).

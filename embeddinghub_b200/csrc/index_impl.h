@@ -196,7 +196,7 @@ constexpr uint32_t kScreenMinBatchPerSm = 4;  // default fp32 walk screen: batch
 }  // namespace ehb
 
 // ehb_index_search_dev with a result sink (exchange.cu)
-int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef,
+int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed);
 
 struct ehb_index {

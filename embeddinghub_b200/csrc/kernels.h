@@ -111,6 +111,11 @@ cudaError_t launch_bf16_dist_tile(const void* q_bf16, uint64_t q_rows, const voi
 cudaError_t launch_rerank(const uint64_t* cand, uint32_t kc, const float* qpad, const float* vecs, uint32_t dpad,
                           uint32_t dim, int metric, const uint64_t* labels, uint64_t nq, uint32_t k,
                           uint64_t* out_labels, float* out_dists, uint32_t* out_counts, cudaStream_t s);
+// The same re-rank storing into every destination of a result sink and raising its slice flags (walk.cuh):
+// the bf16 graph walk's last kernel in a sharded search step.  k <= kMaxEf.
+cudaError_t launch_rerank_sink(const uint64_t* cand, uint32_t kc, const float* qpad, const float* vecs, uint32_t dpad,
+                               uint32_t dim, int metric, const uint64_t* labels, uint64_t nq, uint32_t k,
+                               const ResultSink& sink, uint32_t* out_counts, cudaStream_t s);
 cudaError_t launch_bruteforce(const float* vecs, uint32_t dpad, uint32_t dim, uint64_t n, const uint64_t* labels,
                               int metric, const float* qpad, uint64_t nq, uint32_t k, BruteScratch& sc,
                               const Bf16Ctx* bf, uint64_t* out_labels, float* out_dists, uint32_t* out_counts,

@@ -63,26 +63,10 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
         const bool ok = rk[s] != kMaxKey;
         const uint64_t lab = ok ? g.labels[key_id(rk[s])] : 0xFFFFFFFFFFFFFFFFull;
         const float dist = ok ? key_dist(rk[s]) : INFINITY;
-        const size_t at = (size_t)q * k + idx;
-        for (uint32_t t = 0; t < sink.n; ++t) {
-          sink.labels[t][at] = lab;
-          if (sink.dists[t]) sink.dists[t][at] = dist;
-        }
+        sink_store(sink, (size_t)q * k + idx, lab, dist);
       }
     }
-    if (sink.qs) {  // sharded: the warp that completes a slice raises its flag on every peer
-      __threadfence_system();
-      __syncwarp();
-      if (c.lane == 0) {
-        const uint32_t slice = q / sink.qs;
-        const uint32_t size = min(sink.qs, nq - slice * sink.qs);
-        if (atomicAdd(&sink.slice_count[slice], 1u) + 1u == size) {
-          sink.slice_count[slice] = 0;  // ready for the next step (which starts after this kernel)
-          __threadfence_system();       // the other warps fenced before their atomicAdd: fence-fence ordering
-          for (uint32_t t = 1; t < sink.n; ++t) st_release_sys(sink.flags[t] + slice, sink.epoch);
-        }
-      }
-    }
+    sink_query_done(sink, q, nq, c.lane);
   }
   if (c.lane == 0) {
     if (out_counts) out_counts[q] = found;

@@ -80,6 +80,33 @@ struct ResultSink {
   uint64_t* keys;
 };
 
+// The epilogue of every kernel that ends a graph search in a result sink (the fp32 walk, the re-rank after a bf16
+// walk).  sink_store: element `at` of the [nq][k] results to every destination; the lanes of a warp store
+// consecutive elements, so each destination gets coalesced stores.  sink_query_done, after all of query q's stores,
+// with the whole warp: when the sink has slices, the warp fences its stores system-wide and counts its query in, and
+// the warp that completes the slice resets the counter and raises the slice's flag on every peer (t >= 1).
+__device__ __forceinline__ void sink_store(const ResultSink& sink, size_t at, uint64_t lab, float dist) {
+  for (uint32_t t = 0; t < sink.n; ++t) {
+    sink.labels[t][at] = lab;
+    if (sink.dists[t]) sink.dists[t][at] = dist;
+  }
+}
+__device__ __forceinline__ void sink_query_done(const ResultSink& sink, uint32_t q, uint32_t nq, uint32_t lane) {
+  if (sink.qs) {  // sharded: the warp that completes a slice raises its flag on every peer
+    __threadfence_system();
+    __syncwarp();
+    if (lane == 0) {
+      const uint32_t slice = q / sink.qs;
+      const uint32_t size = min(sink.qs, nq - slice * sink.qs);
+      if (atomicAdd(&sink.slice_count[slice], 1u) + 1u == size) {
+        sink.slice_count[slice] = 0;  // ready for the next step (which starts after this kernel)
+        __threadfence_system();       // the other warps fenced before their atomicAdd: fence-fence ordering
+        for (uint32_t t = 1; t < sink.n; ++t) st_release_sys(sink.flags[t] + slice, sink.epoch);
+      }
+    }
+  }
+}
+
 __host__ __device__ inline uint32_t align_up(uint32_t x, uint32_t a) { return (x + a - 1) / a * a; }
 
 // ---- Row shapes ------------------------------------------------------------------------------------------

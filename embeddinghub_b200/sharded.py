@@ -123,11 +123,12 @@ class ShardedSearcher:
         if bruteforce:
             self.ix.search_bruteforce_dev(q.data_ptr(), nq, k, precision, lp, dp, cp, stream_ptr)
         else:
-            self.ix.search_dev(q.data_ptr(), nq, k, ef, lp, dp, cp, stream_ptr)
+            self.ix.search_dev(q.data_ptr(), nq, k, ef, lp, dp, cp, stream_ptr, precision)
 
     def search_dev(self, q, k, ef, stream_ptr, bruteforce=False, precision=0):
         """q: CUDA float32 tensor [nq, dim].  Returns (labels int64-viewed-u64, dists, counts) CUDA tensors
-        holding the global top-k on every rank.  Nothing synchronises the host."""
+        holding the global top-k on every rank.  precision (FP32 or BF16) applies to graph searches and brute force
+        alike, on every exchange.  Nothing synchronises the host."""
         nq = q.shape[0]
         b = self._bufs(nq, k)
         if self.world == 1:
@@ -137,12 +138,13 @@ class ShardedSearcher:
         if self.exchange == "peer":
             self._ensure_exchange(nq, k)
             if not bruteforce:
-                # fused: the walk's epilogue stores each query's top-k into every peer's receive buffer and raises
-                # the slice flags; one kernel waits for the peers' flags and merges
-                check(lib().ehb_exchange_search_dev(self._ex, self.ix._h, nq, C.c_void_p(q.data_ptr()), k, ef,
-                                                    C.c_void_p(b["md"].data_ptr()), C.c_void_p(b["ml"].data_ptr()),
-                                                    C.c_void_p(b["mc"].data_ptr()), C.c_void_p(b["c"].data_ptr()),
-                                                    C.c_void_p(stream_ptr)))
+                # fused: the search's last kernel (the fp32 walk's epilogue, or the re-rank after a bf16 walk)
+                # stores each query's top-k into every peer's receive buffer and raises the slice flags; one kernel
+                # waits for the peers' flags and merges
+                check(lib().ehb_exchange_search_ex_dev(self._ex, self.ix._h, nq, C.c_void_p(q.data_ptr()), k, ef,
+                                                       int(precision), C.c_void_p(b["md"].data_ptr()),
+                                                       C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
+                                                       C.c_void_p(b["c"].data_ptr()), C.c_void_p(stream_ptr)))
                 return b["ml"], b["md"], b["mc"]
             lp, dp = C.c_void_p(), C.c_void_p()
             check(lib().ehb_exchange_begin(self._ex, nq, k, C.byref(lp), C.byref(dp)))

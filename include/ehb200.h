@@ -286,14 +286,22 @@ int ehb_exchange_attach_local(ehb_exchange* ex, uint32_t peer_rank, ehb_exchange
 int ehb_exchange_begin(ehb_exchange* ex, uint64_t nq, uint32_t k, uint64_t** labels_dev, float** dists_dev);
 int ehb_exchange_merge_dev(ehb_exchange* ex, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
                            void* stream);
-/* The fused step for graph searches (replaces begin + ehb_index_search_dev + merge_dev): the walk kernel's
- * epilogue stores each query's top-k into every peer's receive buffer (coalesced stores over NVLink, overlapping
- * the rest of the walk) and raises per-slice flags; one kernel then waits for the peers' flags and merges.
- * shard_counts_dev ([nq], this shard's hit counts) may be NULL.  This step walks fp32 rows only (there is no
- * bf16 form: a bf16 walk hands its retained set to a re-rank kernel rather than to the peers). */
+/* The fused step for graph searches (replaces begin + ehb_index_search_ex_dev + merge_dev): the search's last
+ * kernel stores each query's top-k into every peer's receive buffer (coalesced stores over NVLink, overlapping
+ * the rest of the search) and raises per-slice flags; one kernel then waits for the peers' flags and merges.
+ * With EHB_FP32 that kernel is the walk itself (a batch small enough for the multi-warp team walk is pushed after
+ * it instead); with EHB_BF16 it is the fp32 re-rank that follows the bf16 walk, so every rank's results are those
+ * of ehb_index_search_ex_dev at EHB_BF16, merged.  The first EHB_BF16 step creates the index's bf16 copy of its
+ * rows, as any first bf16 search does.  shard_counts_dev ([nq], this shard's hit counts) may be NULL.  An unknown
+ * precision, a null pointer, nq * k above the capacity and max(ef, k) > 512 fail before the step starts, so the
+ * next step still pairs with the peers' (call it on every rank, so every rank fails the same way).
+ * ehb_exchange_search_dev is exactly the _ex form with EHB_FP32. */
 int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
                             uint32_t ef, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
                             uint32_t* shard_counts_dev, void* stream);
+int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                               uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
+                               uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream);
 int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a peer gave up (~20 s) */);
 
 /* Named integer options (A/B switches and construction knobs that are not part of
