@@ -9,7 +9,7 @@ OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(SRCS))
 LIB       := embeddinghub_b200/libehb200.so
 
 all: $(LIB) oracle tests/cpp/ann_index_cases tests/cpp/concurrent_search tests/cpp/sharded_two_dev tests/cpp/rwlock_stress \
-     tests/cpp/libbf16_probe.so tests/cpp/libi8_probe.so tests/cpp/ann_index_bf16
+     tests/cpp/libbf16_probe.so tests/cpp/libi8_probe.so tests/cpp/ann_index_bf16 tests/cpp/ann_index_by_key
 
 # test-only extern "C" wrappers around the K3 launchers of the shipped library (run by tests/test_gpu_bf16_gemm.py)
 tests/cpp/libbf16_probe.so: tests/cpp/bf16_probe.cu $(CSRC)/kernels.h $(LIB)
@@ -27,6 +27,10 @@ tests/cpp/ann_index_cases: tests/cpp/ann_index_cases.cc include/ehb200_ann_index
 
 # the C++ twin with a bf16 graph search (run by tests/test_gpu_bf16_walk.py)
 tests/cpp/ann_index_bf16: tests/cpp/ann_index_bf16.cc include/ehb200_ann_index.hpp $(LIB)
+	g++ -std=c++17 -O2 -Iinclude $< -Lembeddinghub_b200 -lehb200 -Wl,-rpath,'$$ORIGIN/../../embeddinghub_b200' -o $@
+
+# key mode through the C++ twin (run by tests/test_gpu_search_by_label.py)
+tests/cpp/ann_index_by_key: tests/cpp/ann_index_by_key.cc include/ehb200_ann_index.hpp $(LIB)
 	g++ -std=c++17 -O2 -Iinclude $< -Lembeddinghub_b200 -lehb200 -Wl,-rpath,'$$ORIGIN/../../embeddinghub_b200' -o $@
 
 # 64 pthreads issuing Q=1 searches through the C ABI (the cgo goroutine pattern; run by tests/test_gpu_round2.py)

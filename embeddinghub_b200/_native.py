@@ -85,6 +85,10 @@ SYMBOLS = {
     "ehb_index_search_ex_dev": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce_dev": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP, _VP]),
+    "ehb_index_get_batch": (C.c_int, [_VP, _U64, _VP, _VP]),
+    "ehb_index_search_by_label_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_index_search_bruteforce_by_label": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_index_neighbor_table": (C.c_int, [_VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, C.POINTER(_U64)]),
     "ehb_index_stats": (C.c_int, [_VP, C.POINTER(Stats)]),
     "ehb_index_screen_stats": (C.c_int, [_VP, C.POINTER(_U64), C.POINTER(_U64)]),
     "ehb_index_last_kernel_ms": (C.c_int, [_VP, C.POINTER(C.c_float)]),
@@ -112,6 +116,8 @@ SYMBOLS = {
     "ehb_sharded_search": (C.c_int, [_VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP]),
     "ehb_sharded_search_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_sharded_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_sharded_get_batch": (C.c_int, [_VP, _U64, _VP, _VP]),
+    "ehb_sharded_search_by_label_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_exchange_create": (C.c_int, [_I32, _U32, _U32, _U64, _U32, C.POINTER(_VP)]),
     "ehb_exchange_destroy": (C.c_int, [_VP]),
     "ehb_exchange_ipc_handle": (C.c_int, [_VP, _VP]),
@@ -149,6 +155,12 @@ def check(rc):
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _check_key(rc, labels):
+    if rc == 5:
+        raise KeyError(labels)
+    check(rc)
 
 
 class NativeIndex:
@@ -244,6 +256,14 @@ class NativeIndex:
         check(rc)
         return out
 
+    def get_batch(self, labels):
+        """The stored rows of `labels` ([n][dim]), each exactly as get() returns it; KeyError for an unknown or
+        deleted label (ehb_index_get_batch)."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out = np.empty((lab.shape[0], self.dim), np.float32)
+        _check_key(lib().ehb_index_get_batch(self._h, lab.shape[0], _p(lab), _p(out)), labels)
+        return out
+
     def _alloc(self, nq, k):
         return (np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.empty(nq, np.uint32))
 
@@ -266,6 +286,44 @@ class NativeIndex:
         if k == 0:
             counts[:] = 0
         return labels, dists, counts
+
+    def search_by_label(self, labels, k, ef=0, precision=FP32):
+        """Key mode of the reference's NearestNeighbor (server.cc:190-207): each stored point's k nearest other points.
+        The point's row is searched at k + 1; its own label is removed, or the last hit dropped when it is absent
+        (ehb_index_search_by_label_ex).  KeyError for an unknown or deleted label."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out_l, out_d, out_c = self._alloc(lab.shape[0], k)
+        _check_key(lib().ehb_index_search_by_label_ex(self._h, lab.shape[0], _p(lab), k, ef, int(precision), _p(out_l),
+                                                      _p(out_d), _p(out_c)), labels)
+        if k == 0:
+            out_c[:] = 0
+        return out_l, out_d, out_c
+
+    def search_bruteforce_by_label(self, labels, k, precision=FP32):
+        """search_by_label over the exact (or bf16) brute force at k + 1 (ehb_index_search_bruteforce_by_label)."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out_l, out_d, out_c = self._alloc(lab.shape[0], k)
+        _check_key(lib().ehb_index_search_bruteforce_by_label(self._h, lab.shape[0], _p(lab), k, int(precision),
+                                                              _p(out_l), _p(out_d), _p(out_c)), labels)
+        if k == 0:
+            out_c[:] = 0
+        return out_l, out_d, out_c
+
+    def neighbor_table(self, k, ef=0, precision=FP32):
+        """(query_labels, labels, dists, counts): search_by_label of every live point, rows in internal-id order
+        (ehb_index_neighbor_table; option "table_chunk" sets the batch)."""
+        st = self.stats()
+        rows = st["size"] - st["deleted"]
+        q = np.empty(rows, np.uint64)
+        out_l, out_d, out_c = self._alloc(rows, k)
+        got = C.c_uint64(rows)
+        check(lib().ehb_index_neighbor_table(self._h, k, ef, int(precision), _p(q), _p(out_l), _p(out_d), _p(out_c),
+                                             C.byref(got)))
+        if k == 0:
+            out_c[:] = 0
+            return q[:0], out_l[:0], out_d[:0], out_c[:0]
+        n = got.value
+        return q[:n], out_l[:n], out_d[:n], out_c[:n]
 
     def search_dev(self, q_ptr, nq, k, ef, labels_ptr, dists_ptr, counts_ptr, stream=0, precision=FP32):
         check(lib().ehb_index_search_ex_dev(self._h, nq, C.c_void_p(q_ptr), k, ef, int(precision),
@@ -398,6 +456,21 @@ class ShardedIndex:
             raise KeyError(label)
         check(rc)
         return out
+
+    def get_batch(self, labels):
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out = np.empty((lab.shape[0], self.dim), np.float32)
+        _check_key(lib().ehb_sharded_get_batch(self._h, lab.shape[0], _p(lab), _p(out)), labels)
+        return out
+
+    def search_by_label(self, labels, k, ef=0, precision=FP32):
+        """NativeIndex.search_by_label on the sharded index (ehb_sharded_search_by_label_ex)."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        nq = lab.shape[0]
+        out_l, out_d, out_c = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
+        _check_key(lib().ehb_sharded_search_by_label_ex(self._h, nq, _p(lab), k, ef, int(precision), _p(out_l),
+                                                        _p(out_d), _p(out_c)), labels)
+        return out_l, out_d, out_c
 
     @property
     def size(self):

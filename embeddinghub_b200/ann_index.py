@@ -102,10 +102,51 @@ class ANNIndex:
             labels, _, counts = self._nn.search(values, num, ef, *extra)
         return [[self._label_to_key[int(l)] for l in row[:c]] for row, c in zip(labels, counts)]
 
+    def _labels_of(self, keys):
+        for k in keys:
+            if k not in self:
+                raise KeyError(k)
+        return np.array([self._key_to_label[k] for k in keys], np.uint64)
+
+    def approx_nearest_by_keys(self, keys, num, ef=0, precision=FP32):
+        """Key mode of NearestNeighbor (server.cc:190-207): for each stored key, the `num` nearest other keys.  The
+        key's stored row is searched at num + 1 on the device and the key itself removed there (or, when it is not
+        among the hits, the last hit dropped), so this answers what get + approx_nearest_batch(num + 1) + that rule
+        answers.  KeyError for an unknown or deleted key; beyond the register-resident beam (max(num + 1, ef) > 512)
+        the exact scan answers, like approx_nearest_batch."""
+        keys = list(keys)
+        labels = self._labels_of(keys)
+        if num == 0 or not keys:
+            return [[] for _ in keys]
+        extra = () if precision == FP32 else (precision,)
+        if max(num + 1, ef) > 512:
+            out, _, counts = self._nn.search_bruteforce_by_label(labels, num, *extra)
+        else:
+            out, _, counts = self._nn.search_by_label(labels, num, ef, *extra)
+        return [[self._label_to_key[int(l)] for l in row[:c]] for row, c in zip(out, counts)]
+
+    def neighbor_table(self, num, ef=0, precision=FP32):
+        """{key: its `num` nearest other keys} for every stored key, in insertion order: approx_nearest_by_keys of
+        all keys, computed in batches on the device (ehb_index_neighbor_table; graph walk, so max(num + 1, ef) <= 512).
+        Writers wait until it returns."""
+        if num == 0:
+            return {k: [] for k in self.keys()}
+        q, out, _, counts = self._nn.neighbor_table(num, ef, precision)
+        key = self._label_to_key
+        return {key[int(lq)]: [key[int(l)] for l in row[:c]] for lq, row, c in zip(q, out, counts)}
+
     def get(self, key):
         if key in self._deleted:
             raise KeyError(key)
         return self._nn.get(self._key_to_label[key])
+
+    def multiget(self, keys):
+        """The stored rows of `keys` ([n][dims]) in one device gather (ehb_index_get_batch); KeyError for an unknown
+        or deleted key."""
+        keys = list(keys)
+        if not keys:
+            return np.empty((0, self._dims), np.float32)
+        return self._nn.get_batch(self._labels_of(keys))
 
     def set_ef(self, ef):
         self._nn.set_ef(ef)

@@ -1028,6 +1028,91 @@ int search_host_combined(ehb_index* ix, uint64_t nq, const float* q, uint32_t k,
   return EHB_OK;
 }
 
+// ---- queries that are stored points (bylabel.cu) ---------------------------------------------------------------
+// Caller holds the shared lock.  hnswlib getDataByLabel: a tombstoned label reads as not found.
+int resolve_labels(const ehb_index* ix, uint64_t n, const uint64_t* labels, std::vector<uint32_t>& ids) {
+  ids.resize(n);
+  for (uint64_t i = 0; i < n; ++i)
+    if (!ix->find_id(labels[i], &ids[i]) || ix->h_deleted[ids[i]]) return fail(EHB_ERR_NOT_FOUND, "label not found");
+  return EHB_OK;
+}
+
+// Caller holds the shared lock and `sl`: the rows of ids into out ([n][dim]) on s, exactly as ehb_index_get reads them.
+int gather_ids(ehb_index* ix, ehb::SearchSlot* sl, const std::vector<uint32_t>& ids, float* out, cudaStream_t s) {
+  const uint64_t n = ids.size();
+  CU(sl->q_ids.grow(n, 0, -1, s));
+  CU(cudaMemcpyAsync(sl->q_ids.p, ids.data(), n * 4, cudaMemcpyHostToDevice, s));
+  CU(ehb::launch_gather_rows(ix->vecs.p, ix->dpad, sl->q_ids.p, out, ix->dim, nullptr, n, ix->dim, s));
+  return EHB_OK;
+}
+
+// Search with the stored rows of `labels` as queries at k + 1, then the reference's self-removal
+// (server.cc:190-207) on the device; one slot, one stream, one synchronisation.  brute: the exact / bf16 brute force
+// instead of the graph walk.
+int search_by_label(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, bool brute, uint64_t nq, const uint64_t* labels,
+                    uint32_t k, uint32_t ef, int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
+  if (nq && (!labels || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (k == 0 || nq == 0) return EHB_OK;
+  const uint32_t k1 = k + 1;
+  if (brute) {
+    if (k1 > 2048) return fail(EHB_ERR_INVALID, "k + 1 must be <= 2048 for brute force");
+    if (precision == EHB_BF16) RET(ix->ensure_shadow(lk));
+  } else {
+    if (std::max(ef ? ef : ix->ef, k1) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k + 1) must be <= 512");
+    RET(ix->ensure_built(lk, precision == EHB_BF16, precision == EHB_FP32 && ix->walk_screens(nq)));
+  }
+  std::vector<uint32_t> ids;
+  RET(resolve_labels(ix, nq, labels, ids));
+  std::unique_lock<std::mutex> bg(ix->bf_mu, std::defer_lock);
+  if (brute) bg.lock();  // brute-force scratch and stream
+  ehb::SearchSlot* sl = nullptr;
+  RET(ix->acquire_slot(&sl));
+  cudaStream_t s = brute ? ix->stream : sl->stream;
+  auto run = [&]() -> int {
+    if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
+    CU(sl->q_in.grow(nq * ix->dim, 0, -1, s));
+    CU(sl->q_labels.grow(nq, 0, -1, s));
+    CU(sl->o_labels.grow(nq * k1, 0, -1, s));
+    CU(sl->o_dists.grow(nq * k1, 0, -1, s));
+    CU(sl->o_counts.grow(nq, 0, -1, s));
+    CU(sl->s_labels.grow(nq * k, 0, -1, s));
+    CU(sl->s_dists.grow(nq * k, 0, -1, s));
+    CU(sl->s_counts.grow(nq, 0, -1, s));
+    RET(gather_ids(ix, sl, ids, sl->q_in.p, s));
+    CU(cudaMemcpyAsync(sl->q_labels.p, labels, nq * 8, cudaMemcpyHostToDevice, s));
+    if (brute)
+      RET(ix->bruteforce_dev(nq, sl->q_in.p, k1, precision, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s));
+    else
+      RET(ix->search_dev(sl, nq, sl->q_in.p, k1, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s, nullptr, nullptr,
+                         precision));
+    CU(ehb::launch_drop_self(sl->q_labels.p, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, nq, k, sl->s_labels.p,
+                             sl->s_dists.p, sl->s_counts.p, s));
+    CU(cudaMemcpyAsync(ol, sl->s_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s));
+    if (od) CU(cudaMemcpyAsync(od, sl->s_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s));
+    if (oc) CU(cudaMemcpyAsync(oc, sl->s_counts.p, nq * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return EHB_OK;
+  };
+  int rc = run();
+  ix->release_slot(sl, s);
+  return rc;
+}
+
+// Stream and events of the neighbour table's result copies; released on every return.
+struct TableCopies {
+  cudaStream_t s = nullptr;
+  cudaEvent_t ready[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
+  ~TableCopies() {
+    if (s) cudaStreamSynchronize(s);
+    for (int b = 0; b < 2; ++b) {
+      if (ready[b]) cudaEventDestroy(ready[b]);
+      if (copied[b]) cudaEventDestroy(copied[b]);
+    }
+    if (s) cudaStreamDestroy(s);
+  }
+};
+
 }  // namespace
 
 extern "C" {
@@ -1162,6 +1247,140 @@ int ehb_index_get(ehb_index* ix, uint64_t label, float* out) {
   return EHB_OK;
 }
 
+int ehb_index_get_batch(ehb_index* ix, uint64_t n, const uint64_t* labels, float* out) {
+  ENTER_S(ix);
+  if (n && (!labels || !out)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (n == 0) return EHB_OK;
+  std::vector<uint32_t> ids;
+  RET(resolve_labels(ix, n, labels, ids));
+  ehb::SearchSlot* sl = nullptr;
+  RET(ix->acquire_slot(&sl));
+  cudaStream_t s = sl->stream;
+  auto run = [&]() -> int {
+    if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
+    CU(sl->q_in.grow(n * ix->dim, 0, -1, s));
+    RET(gather_ids(ix, sl, ids, sl->q_in.p, s));
+    CU(cudaMemcpyAsync(out, sl->q_in.p, n * ix->dim * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return EHB_OK;
+  };
+  int rc = run();
+  ix->release_slot(sl, s);
+  return rc;
+}
+
+int ehb_index_search_by_label_ex(ehb_index* ix, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                                 int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  ENTER_S(ix);
+  return search_by_label(ix, _g, false, nq, labels, k, ef, precision, ol, od, oc);
+}
+
+int ehb_index_search_bruteforce_by_label(ehb_index* ix, uint64_t nq, const uint64_t* labels, uint32_t k, int precision,
+                                         uint64_t* ol, float* od, uint32_t* oc) {
+  ENTER_S(ix);
+  return search_by_label(ix, _g, true, nq, labels, k, 0, precision, ol, od, oc);
+}
+
+// Chunks of C live points in internal-id order.  Chunk j + 1 is gathered and walked while the results of chunk j
+// are copied out (two result buffers).  The shared lock is held throughout: the table is one snapshot.
+int ehb_index_neighbor_table(ehb_index* ix, uint32_t k, uint32_t ef, int precision, uint64_t* oq, uint64_t* ol,
+                             float* od, uint32_t* oc, uint64_t* out_rows) {
+  ENTER_S(ix);
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
+  if (!oq || !ol || !out_rows) return fail(EHB_ERR_INVALID, "null buffer");
+  if (k == 0) return EHB_OK;
+  const uint32_t k1 = k + 1;
+  if (std::max(ef ? ef : ix->ef, k1) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k + 1) must be <= 512");
+  const uint64_t C = ix->o_table_chunk;
+  RET(ix->ensure_built(_g, precision == EHB_BF16,
+                       precision == EHB_FP32 && ix->walk_screens(std::min<uint64_t>(C, ix->n - ix->n_deleted))));
+  const uint64_t n = ix->n, live = n - ix->n_deleted;
+  if (live > *out_rows) {
+    const uint64_t room = *out_rows;
+    *out_rows = live;
+    return fail(EHB_ERR_INVALID, "the buffers hold " + std::to_string(room) + " rows, the table has " +
+                                     std::to_string(live));
+  }
+  if (live == 0) {
+    *out_rows = 0;
+    return EHB_OK;
+  }
+  TableCopies tc;
+  CU(cudaStreamCreateWithFlags(&tc.s, cudaStreamNonBlocking));
+  for (int b = 0; b < 2; ++b) {
+    CU(cudaEventCreateWithFlags(&tc.ready[b], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&tc.copied[b], cudaEventDisableTiming));
+  }
+  const uint64_t cmax = std::min(C, live);
+  ehb::DevBuf<uint64_t> rl[2];
+  ehb::DevBuf<float> rd[2];
+  ehb::DevBuf<uint32_t> rc_[2];
+  ehb::SearchSlot* sl = nullptr;
+  RET(ix->acquire_slot(&sl));
+  cudaStream_t s = sl->stream;
+  auto run = [&]() -> int {
+    if (sl->busy_valid) CU(cudaStreamWaitEvent(s, sl->busy, 0));
+    for (int b = 0; b < 2; ++b) {
+      CU(rl[b].grow(cmax * k, 0, -1, s));
+      CU(rd[b].grow(cmax * k, 0, -1, s));
+      CU(rc_[b].grow(cmax, 0, -1, s));
+    }
+    CU(sl->q_in.grow(cmax * ix->dim, 0, -1, s));
+    CU(sl->q_labels.grow(live, 0, -1, s));
+    CU(sl->o_labels.grow(cmax * k1, 0, -1, s));
+    CU(sl->o_dists.grow(cmax * k1, 0, -1, s));
+    CU(sl->o_counts.grow(cmax, 0, -1, s));
+    // the live ids (none to list without tombstones: chunk rows are then consecutive ids)
+    const bool listed = ix->n_deleted != 0;
+    if (listed) {
+      CU(sl->q_ids.grow(n + 1, 0, -1, s));
+      CU(ehb::launch_live_ids(ix->deleted.p, n, sl->q_ids.p, sl->q_ids.p + n, s));
+      std::vector<uint32_t> ids(live);
+      CU(cudaMemcpyAsync(ids.data(), sl->q_ids.p, live * 4, cudaMemcpyDeviceToHost, s));
+      CU(cudaStreamSynchronize(s));
+      for (uint64_t r = 0; r < live; ++r) oq[r] = ix->h_labels[ids[r]];
+    } else {
+      std::copy(ix->h_labels.begin(), ix->h_labels.begin() + n, oq);
+    }
+    CU(cudaMemcpyAsync(sl->q_labels.p, oq, live * 8, cudaMemcpyHostToDevice, s));
+    auto copy_out = [&](uint64_t off, uint64_t m, int b) -> int {
+      CU(cudaStreamWaitEvent(tc.s, tc.ready[b], 0));
+      CU(cudaMemcpyAsync(ol + off * k, rl[b].p, m * k * 8, cudaMemcpyDeviceToHost, tc.s));
+      if (od) CU(cudaMemcpyAsync(od + off * k, rd[b].p, m * k * 4, cudaMemcpyDeviceToHost, tc.s));
+      if (oc) CU(cudaMemcpyAsync(oc + off, rc_[b].p, m * 4, cudaMemcpyDeviceToHost, tc.s));
+      CU(cudaEventRecord(tc.copied[b], tc.s));
+      return EHB_OK;
+    };
+    uint64_t prev_off = 0, prev_m = 0;
+    for (uint64_t off = 0, j = 0; off < live; off += C, ++j) {
+      const uint64_t m = std::min(C, live - off);
+      const int b = (int)(j & 1);
+      if (j >= 2) CU(cudaStreamWaitEvent(s, tc.copied[b], 0));  // chunk j - 2's results have left buffer b
+      if (listed)
+        CU(ehb::launch_gather_rows(ix->vecs.p, ix->dpad, sl->q_ids.p + off, sl->q_in.p, ix->dim, nullptr, m, ix->dim, s));
+      else
+        CU(ehb::launch_gather_rows(ix->vecs.p + off * ix->dpad, ix->dpad, nullptr, sl->q_in.p, ix->dim, nullptr, m,
+                                   ix->dim, s));
+      RET(ix->search_dev(sl, m, sl->q_in.p, k1, ef, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, s, nullptr, nullptr,
+                         precision));
+      CU(ehb::launch_drop_self(sl->q_labels.p + off, sl->o_labels.p, sl->o_dists.p, sl->o_counts.p, m, k, rl[b].p,
+                               rd[b].p, rc_[b].p, s));
+      CU(cudaEventRecord(tc.ready[b], s));
+      // chunk j - 1 is copied out while chunk j runs
+      if (j >= 1) RET(copy_out(prev_off, prev_m, 1 - b));
+      prev_off = off, prev_m = m;
+    }
+    RET(copy_out(prev_off, prev_m, (int)(((live + C - 1) / C - 1) & 1)));
+    CU(cudaStreamSynchronize(tc.s));
+    CU(cudaStreamSynchronize(s));
+    *out_rows = live;
+    return EHB_OK;
+  };
+  int rc = run();
+  ix->release_slot(sl, s);
+  return rc;
+}
+
 int ehb_index_search_ex(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
                         uint64_t* ol, float* od, uint32_t* oc) {
   ENTER_S(ix);
@@ -1214,6 +1433,23 @@ int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint3
   cudaStream_t s = stream ? stream : sl->stream;
   int rc = ix->search_dev(sl, nq, dq, k, ef, sink->labels[0], sink->dists[0], dc, s, sink, pushed, precision);
   ix->release_slot(sl, s);
+  return rc;
+}
+
+int ehb_index_gather_dev(ehb_index* ix, uint64_t n, const uint64_t* labels, float* rows_dev, cudaStream_t stream) {
+  ENTER_S(ix);
+  if (n && (!labels || !rows_dev)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (n == 0) return EHB_OK;
+  std::vector<uint32_t> ids;
+  RET(resolve_labels(ix, n, labels, ids));
+  ehb::SearchSlot* sl = nullptr;
+  RET(ix->acquire_slot(&sl));
+  auto run = [&]() -> int {
+    if (sl->busy_valid) CU(cudaStreamWaitEvent(stream, sl->busy, 0));
+    return gather_ids(ix, sl, ids, rows_dev, stream);
+  };
+  int rc = run();
+  ix->release_slot(sl, stream);
   return rc;
 }
 
@@ -1370,6 +1606,9 @@ int ehb_index_set_option(ehb_index* ix, const char* name, int64_t value) {
     ix->screen_no_room = false;
   } else if (o == "combine") {
     ix->o_combine = value != 0;
+  } else if (o == "table_chunk") {
+    if (value < 1 || value > (1ll << 31)) return fail(EHB_ERR_INVALID, "table_chunk must be in 1..2^31");
+    ix->o_table_chunk = (uint64_t)value;
   } else {
     return fail(EHB_ERR_INVALID, "unknown option: " + o);
   }

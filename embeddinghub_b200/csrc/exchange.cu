@@ -363,6 +363,13 @@ struct ehb_sharded {
   std::vector<ehb::DevBuf<float>*> q_dev;   // per device
   std::vector<ehb::DevBuf<unsigned char>*> local_out;  // per device (no peer access): [labels | dists]
   std::vector<ehb::DevBuf<uint32_t>*> cnt_dev;
+  // by-label searches: per device, the gathered rows in owner order and each row's query position; on device 0 the
+  // query labels and the results after self-removal
+  std::vector<ehb::DevBuf<float>*> q_stage;
+  std::vector<ehb::DevBuf<uint32_t>*> q_pos;
+  ehb::DevBuf<uint64_t> s_self, s_labels;
+  ehb::DevBuf<float> s_dists;
+  ehb::DevBuf<uint32_t> s_counts;
   std::vector<cudaStream_t> st;
   std::vector<cudaEvent_t> done;
   cudaEvent_t q_ready = nullptr;
@@ -387,6 +394,8 @@ int ehb_sharded_destroy(ehb_sharded* sh) {
     if (g < sh->q_dev.size()) delete sh->q_dev[g];
     if (g < sh->local_out.size()) delete sh->local_out[g];
     if (g < sh->cnt_dev.size()) delete sh->cnt_dev[g];
+    if (g < sh->q_stage.size()) delete sh->q_stage[g];
+    if (g < sh->q_pos.size()) delete sh->q_pos[g];
     ehb_index_destroy(sh->shard[g]);
   }
   if (!sh->dev.empty()) {
@@ -396,6 +405,10 @@ int ehb_sharded_destroy(ehb_sharded* sh) {
     sh->m_dists.release();
     sh->m_labels.release();
     sh->m_counts.release();
+    sh->s_self.release();
+    sh->s_labels.release();
+    sh->s_dists.release();
+    sh->s_counts.release();
   }
   delete sh;
   return EHB_OK;
@@ -429,6 +442,8 @@ int ehb_sharded_create(const ehb_params* p, const int32_t* device_ids, uint32_t 
       sh->q_dev.push_back(new ehb::DevBuf<float>());
       sh->local_out.push_back(new ehb::DevBuf<unsigned char>());
       sh->cnt_dev.push_back(new ehb::DevBuf<uint32_t>());
+      sh->q_stage.push_back(new ehb::DevBuf<float>());
+      sh->q_pos.push_back(new ehb::DevBuf<uint32_t>());
       if (g > 0 && device_ids[g] != device_ids[0]) {  // device g must be able to store into device 0
         int can = 0;
         CU(cudaDeviceCanAccessPeer(&can, device_ids[g], device_ids[0]));
@@ -555,15 +570,12 @@ int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
   return EHB_OK;
 }
 
-// Host queries in, merged host results out.  mode: 0 = graph walk, 1 = exact brute force, 2 = bf16 brute force.
+// Every shard searches, device 0 merges into m_labels / m_dists / m_counts (queued on st[0]).  Caller holds mu.
+// q: host queries, or nullptr when every q_dev already holds them (queued on the shards' streams).
+// mode: 0 = graph walk, 1 = exact brute force, 2 = bf16 brute force.
 // precision: of the graph walk (a bf16 walk re-ranks straight into device 0's gather block, like the fp32 walk).
-static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
-                          int precision, uint64_t* ol, float* od, uint32_t* oc) {
-  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
-  if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
-  if (nq == 0 || k == 0) return EHB_OK;
-  std::lock_guard<std::mutex> g(sh->mu);
+static int sharded_merge(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
+                         int precision) {
   const uint32_t G = (uint32_t)sh->shard.size();
   const uint32_t dim = sh->prm.dim;
   const uint64_t blk = (nq * k * 12ull + 255) / 256 * 256;
@@ -579,7 +591,7 @@ static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q
     cudaStream_t s = sh->st[i];
     CU(sh->q_dev[i]->grow(nq * dim, 0, -1, s));
     CU(sh->cnt_dev[i]->grow(nq, 0, -1, s));
-    CU(cudaMemcpyAsync(sh->q_dev[i]->p, q, nq * dim * 4, cudaMemcpyHostToDevice, s));
+    if (q) CU(cudaMemcpyAsync(sh->q_dev[i]->p, q, nq * dim * 4, cudaMemcpyHostToDevice, s));
     unsigned char* dst;
     if (i == 0 || sh->peer_direct || sh->dev[i] == sh->dev[0]) {
       dst = sh->gather.p + blk * i;  // device i's kernels store straight into device 0's gather block
@@ -604,6 +616,19 @@ static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q
   for (uint32_t i = 1; i < G; ++i) CU(cudaStreamWaitEvent(s0, sh->done[i], 0));
   CU(ehb::launch_merge_topk(G, nq, k, (const float*)(sh->gather.p + nq * k * 8ull), (const uint64_t*)sh->gather.p, blk,
                             blk, sh->m_dists.p, sh->m_labels.p, sh->m_counts.p, s0));
+  return EHB_OK;
+}
+
+// Host queries in, merged host results out.
+static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
+                          int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
+  if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (nq == 0 || k == 0) return EHB_OK;
+  std::lock_guard<std::mutex> g(sh->mu);
+  RET(sharded_merge(sh, mode, nq, q, k, ef, precision));
+  cudaStream_t s0 = sh->st[0];
   CU(cudaMemcpyAsync(ol, sh->m_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s0));
   if (od) CU(cudaMemcpyAsync(od, sh->m_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s0));
   if (oc) CU(cudaMemcpyAsync(oc, sh->m_counts.p, nq * 4, cudaMemcpyDeviceToHost, s0));
@@ -622,6 +647,101 @@ int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, int precision, uint64_t* ol,
                                   float* od, uint32_t* oc) {
   return sharded_search(sh, precision == EHB_BF16 ? 2 : 1, nq, q, k, 0, EHB_FP32, ol, od, oc);
+}
+
+int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, float* out) {
+  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
+  if (n && (!labels || !out)) return fail(EHB_ERR_INVALID, "null buffer");
+  const size_t G = sh->shard.size(), dim = sh->prm.dim;
+  std::vector<std::vector<uint64_t>> labs(G), pos(G);
+  for (uint64_t i = 0; i < n; ++i) {
+    const uint32_t o = sh->owner(labels[i]);
+    labs[o].push_back(labels[i]);
+    pos[o].push_back(i);
+  }
+  std::vector<std::vector<float>> rows(G);  // every shard answers before anything is written
+  for (size_t o = 0; o < G; ++o) {
+    if (labs[o].empty()) continue;
+    rows[o].resize(labs[o].size() * dim);
+    RET(ehb_index_get_batch(sh->shard[o], labs[o].size(), labs[o].data(), rows[o].data()));
+  }
+  for (size_t o = 0; o < G; ++o)
+    for (size_t j = 0; j < pos[o].size(); ++j)
+      std::copy(rows[o].begin() + j * dim, rows[o].begin() + (j + 1) * dim, out + pos[o][j] * dim);
+  return EHB_OK;
+}
+
+// The rows are laid out in owner order: shard o gathers its labels' rows into its own staging rows
+// [first[o], first[o] + m_o) and copies them into every other shard's staging buffer; each shard then scatters the
+// staging rows to their query positions in q_dev, and the k + 1 search + merge of ehb_sharded_search_ex runs on them.
+int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                                   int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
+  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
+  if (nq && (!labels || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
+  if (nq == 0 || k == 0) return EHB_OK;
+  const uint32_t k1 = k + 1;
+  if (std::max(ef, k1) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k + 1) must be <= 512");
+  std::lock_guard<std::mutex> g(sh->mu);
+  const uint32_t G = (uint32_t)sh->shard.size();
+  const uint32_t dim = sh->prm.dim;
+  std::vector<std::vector<uint64_t>> labs(G);
+  std::vector<uint32_t> order;  // query position of each staging row
+  std::vector<uint64_t> first(G);
+  order.reserve(nq);
+  {
+    std::vector<std::vector<uint32_t>> pos(G);
+    for (uint64_t i = 0; i < nq; ++i) {
+      const uint32_t o = sh->owner(labels[i]);
+      labs[o].push_back(labels[i]);
+      pos[o].push_back((uint32_t)i);
+    }
+    for (uint32_t o = 0; o < G; ++o) {
+      first[o] = order.size();
+      order.insert(order.end(), pos[o].begin(), pos[o].end());
+    }
+  }
+  for (uint32_t i = 0; i < G; ++i) {
+    CU(cudaSetDevice(sh->dev[i]));
+    CU(sh->q_stage[i]->grow(nq * dim, 0, -1, sh->st[i]));
+    CU(sh->q_pos[i]->grow(nq, 0, -1, sh->st[i]));
+    CU(sh->q_dev[i]->grow(nq * dim, 0, -1, sh->st[i]));
+  }
+  for (uint32_t o = 0; o < G; ++o) {
+    if (labs[o].empty()) continue;
+    const uint64_t m = labs[o].size();
+    float* rows = sh->q_stage[o]->p + first[o] * dim;
+    RET(ehb_index_gather_dev(sh->shard[o], m, labs[o].data(), rows, sh->st[o]));
+    CU(cudaSetDevice(sh->dev[o]));
+    for (uint32_t i = 0; i < G; ++i)
+      if (i != o)
+        CU(cudaMemcpyPeerAsync(sh->q_stage[i]->p + first[o] * dim, sh->dev[i], rows, sh->dev[o], m * dim * 4ull,
+                               sh->st[o]));
+    CU(cudaEventRecord(sh->done[o], sh->st[o]));
+  }
+  for (uint32_t i = 0; i < G; ++i) {
+    CU(cudaSetDevice(sh->dev[i]));
+    cudaStream_t s = sh->st[i];
+    for (uint32_t o = 0; o < G; ++o)
+      if (o != i && !labs[o].empty()) CU(cudaStreamWaitEvent(s, sh->done[o], 0));
+    CU(cudaMemcpyAsync(sh->q_pos[i]->p, order.data(), nq * 4, cudaMemcpyHostToDevice, s));
+    CU(ehb::launch_gather_rows(sh->q_stage[i]->p, dim, nullptr, sh->q_dev[i]->p, dim, sh->q_pos[i]->p, nq, dim, s));
+  }
+  RET(sharded_merge(sh, 0, nq, nullptr, k1, ef, precision));
+  CU(cudaSetDevice(sh->dev[0]));
+  cudaStream_t s0 = sh->st[0];
+  CU(sh->s_self.grow(nq, 0, -1, s0));
+  CU(sh->s_labels.grow(nq * k, 0, -1, s0));
+  CU(sh->s_dists.grow(nq * k, 0, -1, s0));
+  CU(sh->s_counts.grow(nq, 0, -1, s0));
+  CU(cudaMemcpyAsync(sh->s_self.p, labels, nq * 8, cudaMemcpyHostToDevice, s0));
+  CU(ehb::launch_drop_self(sh->s_self.p, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, nq, k, sh->s_labels.p,
+                           sh->s_dists.p, sh->s_counts.p, s0));
+  CU(cudaMemcpyAsync(ol, sh->s_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s0));
+  if (od) CU(cudaMemcpyAsync(od, sh->s_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s0));
+  if (oc) CU(cudaMemcpyAsync(oc, sh->s_counts.p, nq * 4, cudaMemcpyDeviceToHost, s0));
+  CU(cudaStreamSynchronize(s0));
+  return EHB_OK;
 }
 
 }  // extern "C"

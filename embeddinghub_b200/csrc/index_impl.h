@@ -161,6 +161,12 @@ struct SearchSlot {
   DevBuf<uint32_t> walk_counts; // bf16 graph search: [nq] retained count (the keys re-ranked)
   bool last_bf16 = false;       // the most recent search on this slot walked the bf16 shadow
   DevBuf<unsigned long long> stat_sum;
+  // by-label searches (bylabel.cu): the queries' internal ids and labels, and the results after self-removal
+  DevBuf<uint32_t> q_ids;
+  DevBuf<uint64_t> q_labels;
+  DevBuf<uint64_t> s_labels;
+  DevBuf<float> s_dists;
+  DevBuf<uint32_t> s_counts;
   PinBuf h_q, h_l, h_d, h_c;
   uint64_t last_nq = 0;
   char last_kernel[96] = {0};  // name of the graph-walk kernel of the most recent search on this slot
@@ -198,6 +204,9 @@ constexpr uint32_t kScreenMinBatchPerSm = 4;  // default fp32 walk screen: batch
 // ehb_index_search_dev with a result sink (exchange.cu)
 int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed);
+// The stored rows of n live labels into rows_dev ([n][dim] on the index's device), queued on `stream`; an unknown or
+// tombstoned label fails with EHB_ERR_NOT_FOUND before anything is queued (exchange.cu: by-label sharded searches)
+int ehb_index_gather_dev(ehb_index* ix, uint64_t n, const uint64_t* labels_host, float* rows_dev, cudaStream_t stream);
 
 struct ehb_index {
   ehb_params prm;
@@ -296,6 +305,7 @@ struct ehb_index {
   // cleared when the option is set again).
   int o_walk_screen = -1;
   bool screen_no_room = false;
+  uint64_t o_table_chunk = 65536;  // ehb_index_neighbor_table: live points searched per batch
 
   std::default_random_engine level_rng;
 

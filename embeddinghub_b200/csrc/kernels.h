@@ -190,4 +190,18 @@ cudaError_t launch_compact_orphans(const uint32_t* links0, uint64_t n, uint32_t 
 cudaError_t launch_compact_move_rows(float* vecs, uint32_t dpad, const uint32_t* inv, uint64_t lo, uint64_t n,
                                      float* stage, uint64_t stage_rows, cudaStream_t s);
 
+// K7 — queries that are stored points (bylabel.cu).
+// out[dst ? dst[j] : j][0:dim] = in[src ? src[j] : j][0:dim] for j < n (row strides in floats): the stored rows of
+// labels as queries, and the scatter of gathered rows to their query positions on a sharded index.
+cudaError_t launch_gather_rows(const float* in, uint32_t in_stride, const uint32_t* src, float* out,
+                               uint32_t out_stride, const uint32_t* dst, uint64_t n, uint32_t dim, cudaStream_t s);
+// Self-removal of the reference's key mode (server.cc:190-207): from [nq][k + 1] results (nearest-first, counts
+// in_counts) to [nq][k]: query q's own label self[q] is removed when present among its hits, else the last hit is
+// dropped when there are k + 1; rows are padded with EHB_NO_LABEL / +inf.
+cudaError_t launch_drop_self(const uint64_t* self, const uint64_t* in_labels, const float* in_dists,
+                             const uint32_t* in_counts, uint64_t nq, uint32_t k, uint64_t* out_labels,
+                             float* out_dists, uint32_t* out_counts, cudaStream_t s);
+// The ids i < n with deleted[i] == 0, ascending, into ids[0..*count).
+cudaError_t launch_live_ids(const uint8_t* deleted, uint64_t n, uint32_t* ids, uint32_t* count, cudaStream_t s);
+
 }  // namespace ehb

@@ -185,6 +185,44 @@ int ehb_index_search_bruteforce_dev(ehb_index* ix, uint64_t nq, const float* que
                                     uint64_t* out_labels_dev, float* out_dists_dev, uint32_t* out_counts_dev,
                                     void* stream);
 
+/* Batched Version::get: the stored rows of n labels into out_vecs_host ([n][dim]), each exactly as
+ * ehb_index_get returns it (for cosine: the normalised row).  One gather kernel and one copy instead of n
+ * synchronous reads.  An unknown or tombstoned label fails with EHB_ERR_NOT_FOUND and nothing is written. */
+int ehb_index_get_batch(ehb_index* ix, uint64_t n, const uint64_t* labels_host, float* out_vecs_host);
+
+/* Key mode of the reference's NearestNeighbor (embeddinghub/embeddingstore/server.cc:190-207, also
+ * serving/offlinehub.py:110-130): the neighbours of points already stored, named by label.  For each label L the
+ * stored row (as ehb_index_get returns it) is the query, prepared like any host query (cosine normalises it
+ * again), and searched at k + 1 with the given ef and precision, taking the walk an ehb_index_search_ex of the same
+ * nq would take.  From that list R of c hits, nearest-first: if L is in R it is removed; otherwise, if c > k, the
+ * last hit is dropped.  The first k remaining entries are written, padded with EHB_NO_LABEL / +inf, and the count
+ * is min(c', k).  Labels, distance bits and counts equal the host composition ehb_index_get of every label ->
+ * ehb_index_search_ex(rows, k + 1, ef, precision) -> that rule; the queries never leave the device.
+ * Checked before anything is written: a null pointer or max(ef, k + 1) > 512 fails with EHB_ERR_INVALID, an
+ * unknown or tombstoned label with EHB_ERR_NOT_FOUND.  nq == 0 or k == 0 writes nothing.  The call does not go
+ * through the combining queue; ehb_index_last_kernel_ms / _name and ehb_index_stats describe its walk.
+ * out_dists / out_counts may be NULL. */
+int ehb_index_search_by_label_ex(ehb_index* ix, uint64_t nq, const uint64_t* labels_host, uint32_t k, uint32_t ef,
+                                 int precision, uint64_t* out_labels_host, float* out_dists_host,
+                                 uint32_t* out_counts_host);
+/* The same rule over ehb_index_search_bruteforce(rows, k + 1, precision); k + 1 must be <= 2048. */
+int ehb_index_search_bruteforce_by_label(ehb_index* ix, uint64_t nq, const uint64_t* labels_host, uint32_t k,
+                                         int precision, uint64_t* out_labels_host, float* out_dists_host,
+                                         uint32_t* out_counts_host);
+/* Every live point's k nearest other points: ehb_index_search_by_label_ex (same rule, server.cc:190-207) over
+ * all live labels in internal-id order (insertion order, which compaction keeps), in consecutive chunks of
+ * "table_chunk" points (ehb_index_set_option, default 65536); each chunk's rows are by definition
+ * ehb_index_search_by_label_ex of that chunk's labels.  out_query_labels[r] is row r's label.  *out_rows is in / out:
+ * on entry the rows the buffers hold (size them for size - deleted rows, ehb_stats), on return the rows written;
+ * when the table has more rows, the call fails with EHB_ERR_INVALID, writes nothing else and stores the row count
+ * needed in *out_rows.  The call holds the index's reader side
+ * throughout, so the table is one consistent snapshot: searches run alongside it, and mutations (add, remove,
+ * build, compact) wait until it returns.  Errors as ehb_index_search_by_label_ex; k == 0 writes nothing.
+ * out_dists / out_counts may be NULL. */
+int ehb_index_neighbor_table(ehb_index* ix, uint32_t k, uint32_t ef, int precision, uint64_t* out_query_labels_host,
+                             uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host,
+                             uint64_t* out_rows);
+
 int ehb_index_stats(ehb_index* ix, ehb_stats* out);
 /* Counters of the fp32 walk's int8 screen in the most recent graph search (option "walk_screen"):
  * screened_evals = distance evaluations made on the int8 copy first (dim code bytes + 16 bytes of per-row terms each), fp32_row_reads = fp32 rows the walk read
@@ -267,6 +305,16 @@ int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* queries_hos
                           int precision, uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, int precision,
                                   uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
+/* ehb_index_get_batch routed to each label's shard. */
+int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels_host, float* out_vecs_host);
+/* Key mode (server.cc:190-207, offlinehub.py:110-130) on the sharded index: each label's owning shard copies its
+ * row into every shard's query buffer (device-to-device, no round trip through the host), every shard searches at
+ * k + 1, the lists are merged on device_ids[0], and the self-removal rule of ehb_index_search_by_label_ex runs
+ * there.  Equal to ehb_sharded_get of every label -> ehb_sharded_search_ex(rows, k + 1) -> that rule; errors as
+ * ehb_index_search_by_label_ex. */
+int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels_host, uint32_t k, uint32_t ef,
+                                   int precision, uint64_t* out_labels_host, float* out_dists_host,
+                                   uint32_t* out_counts_host);
 
 /* Shard exchange for one-process-per-GPU deployments (torchrun / MPI): replaces "one ncclAllGather of the
  * per-shard top-k + merge kernel" (SURVEY.md §8e) with ONE kernel per rank that pushes this rank's lists
@@ -309,6 +357,7 @@ int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a pe
  *   "build_frac"    a construction wave links at most size/build_frac points (0 = default 64)
  *   "bf16_unfused"  bf16 brute force keeps the distance tiles in HBM (A/B of the fused epilogue)
  *   "combine"       1 (default): concurrent host searches of <= 256 queries share batched launches
+ *   "table_chunk"   live points per batch of ehb_index_neighbor_table (default 65536, 1..2^31)
  *   "walk_prefetch" 1: L2-prefetch the speculated next hop's vectors (default 0: it also fetches rows the walk
  *                   never evaluates, extra DRAM traffic for a DRAM-bound walk)
  *   "walk_screen"   the fp32 walk's int8 screen, for inner product and cosine with 256 < dim <= 1536: once the

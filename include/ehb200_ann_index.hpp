@@ -10,8 +10,11 @@
 //   * approx_nearest returns the keys that exist when fewer than `num` points are
 //     stored (index.cc:42-50 pops `num` entries regardless — undefined behaviour);
 //   * a batched approx_nearest_batch() is added (docs/inference.md:14-22), with an optional ef and precision
-//     (EHB_BF16: the graph walk over bf16 rows, re-ranked in fp32; ehb_index_search_ex).
+//     (EHB_BF16: the graph walk over bf16 rows, re-ranked in fp32; ehb_index_search_ex);
+//   * approx_nearest_by_key() / approx_nearest_by_keys() answer the server's key mode (server.cc:190-207) on the
+//     device.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <memory>
 #include <stdexcept>
@@ -76,6 +79,38 @@ class ANNIndex {
     check(ehb_index_search_ex(ix_, values.size(), q.data(), (uint32_t)num, ef, precision, labels.data(), nullptr,
                               counts.data()));
     for (size_t i = 0; i < values.size(); ++i)
+      for (uint32_t j = 0; j < counts[i]; ++j) out[i].push_back(label_to_key_.at(labels[i * num + j]));
+    return out;
+  }
+
+  // Key mode of NearestNeighbor (server.cc:190-207): the `num` nearest other keys of a stored key.  The key's row
+  // is searched at num + 1 on the device and the key removed there, or the last hit dropped when the key is not
+  // among them (ehb_index_search_by_label_ex), so a server calls this one member instead of get + approx_nearest
+  // with num + 1 + erase.  An unknown or removed key throws.
+  std::vector<std::string> approx_nearest_by_key(const std::string& key, size_t num) const {
+    return approx_nearest_by_keys(std::vector<std::string>{key}, num)[0];
+  }
+
+  std::vector<std::vector<std::string>> approx_nearest_by_keys(const std::vector<std::string>& keys, size_t num,
+                                                               uint32_t ef = 0, int precision = EHB_FP32) const {
+    std::vector<uint64_t> q(keys.size());
+    for (size_t i = 0; i < keys.size(); ++i) {
+      auto it = key_to_label_.find(keys[i]);
+      if (it == key_to_label_.end() || deleted_.count(keys[i]))
+        throw std::runtime_error("ANNIndex::approx_nearest_by_key: unknown key");
+      q[i] = it->second;
+    }
+    std::vector<std::vector<std::string>> out(keys.size());
+    if (num == 0 || keys.empty()) return out;
+    std::vector<uint64_t> labels(keys.size() * num);
+    std::vector<uint32_t> counts(keys.size());
+    if (std::max<size_t>(num + 1, ef) > 512)  // beyond the graph walk's beam: the exact scan
+      check(ehb_index_search_bruteforce_by_label(ix_, keys.size(), q.data(), (uint32_t)num, precision, labels.data(),
+                                                 nullptr, counts.data()));
+    else
+      check(ehb_index_search_by_label_ex(ix_, keys.size(), q.data(), (uint32_t)num, ef, precision, labels.data(),
+                                         nullptr, counts.data()));
+    for (size_t i = 0; i < keys.size(); ++i)
       for (uint32_t j = 0; j < counts[i]; ++j) out[i].push_back(label_to_key_.at(labels[i * num + j]));
     return out;
   }
