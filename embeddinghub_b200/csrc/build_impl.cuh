@@ -81,6 +81,57 @@ __device__ __forceinline__ uint32_t heuristic_select(WarpCtx& c, const GraphView
   return nsel;
 }
 
+// Drops `id` from the sorted key list c.keys[0..cnt) if it is there.  hnswlib's repairConnectionsForUpdate walks
+// and admits the moved point like any other node and removes it from the result list afterwards.
+__device__ __forceinline__ void list_remove_id(WarpCtx& c, uint32_t id) {
+  uint32_t pos = kInvalid;
+  for (uint32_t base = 0; base < c.cnt && pos == kInvalid; base += 32) {
+    const uint32_t i = base + c.lane;
+    const uint32_t m = __ballot_sync(0xffffffffu, i < c.cnt && key_id(c.keys[i]) == id);
+    if (m) pos = base + __ffs(m) - 1;
+  }
+  if (pos == kInvalid) return;
+  for (uint32_t base = pos & ~31u; base < c.cnt; base += 32) {
+    const uint32_t i = base + c.lane;
+    const uint64_t v = i + 1 < c.cnt ? c.keys[i + 1] : kMaxKey;
+    __syncwarp();
+    if (i >= pos && i + 1 < c.cnt) c.keys[i] = v;
+    __syncwarp();
+  }
+  c.cnt--;
+}
+
+// The update path never rewrites a row in place while other warps of the wave may read it: a new row is staged in
+// bb.side_out (one slot of M0 entries per row, bb.side_row names the row) and copied back by apply_staged_kernel
+// once every warp has read the graph.  Returns the slot the calling warp writes (lanes < row width); slot side_cap
+// is a sink that is never copied back (the build then reports an overflow).
+__device__ __forceinline__ uint32_t* stage_row(const BuildBuffers& bb, uint32_t rid, uint32_t M0, uint32_t lane) {
+  uint32_t slot = 0;
+  if (lane == 0) {
+    slot = atomicAdd(bb.side_count, 1u);
+    if (slot < bb.side_cap) bb.side_row[slot] = rid;
+    else atomicExch(bb.error_flag, 1u);
+  }
+  slot = __shfl_sync(0xffffffffu, slot, 0);
+  return bb.side_out + (size_t)min(slot, bb.side_cap) * M0;
+}
+
+// Copies the staged rows back (one thread per entry) and clears the rows' update tags (bb.row_fill).
+static __global__ void apply_staged_kernel(BuildBuffers bb, uint32_t* links0, uint32_t* links_up, uint32_t cap,
+                                           uint32_t M0, uint32_t M) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t slot = (uint32_t)(t / M0), j = (uint32_t)(t % M0);
+  if (slot >= min(*bb.side_count, bb.side_cap)) return;
+  const uint32_t rid = bb.side_row[slot];
+  const uint32_t v = bb.side_out[(size_t)slot * M0 + j];
+  if (rid < cap) {
+    links0[(size_t)rid * M0 + j] = v;
+  } else if (j < M) {
+    links_up[(size_t)(rid - cap) * M + j] = v;
+  }
+  if (j == 0) bb.row_fill[rid] = 0u;
+}
+
 template <int LPV, int NQ, int KPL, bool HASDEL>
 __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ ids,
                                                            uint32_t first, uint32_t b, int is_update, BuildBuffers bb,
@@ -110,12 +161,18 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
   uint32_t* links0 = const_cast<uint32_t*>(g.links0);
   uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
   for (int level = min(level_p, top); level >= 0; --level) {
-    beam_search<LPV, NQ, KPL, false, HASDEL>(c, g, qr, ul, cur, curdist, level, bg.efc, is_update ? p : kInvalid, wc);
+    beam_search<LPV, NQ, KPL, false, HASDEL>(c, g, qr, ul, cur, curdist, level, bg.efc, kInvalid, wc);
     ul_extract_all<KPL>(c, ul);  // the list the selection heuristic walks
+    if (is_update) list_remove_id(c, p);
     if (c.cnt == 0) continue;
     uint32_t nsel = heuristic_select<LPV, NQ>(c, g, g.M, a);
     uint32_t width = level == 0 ? g.M0 : g.M;
     uint32_t* row = level == 0 ? links0 + (size_t)p * g.M0 : links_up + (size_t)(g.up_off[p] + level - 1) * g.M;
+    if (is_update) {
+      // other warps of the wave may still walk this row: stage it, it lands before phase C
+      const uint32_t rid = level == 0 ? p : bg.cap + g.up_off[p] + (uint32_t)(level - 1);
+      row = stage_row(bb, rid, g.M0, c.lane);
+    }
     if (c.lane < width) row[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
     uint32_t base = 0;
     if (c.lane == 0) base = atomicAdd(bb.edge_count, nsel);
@@ -194,8 +251,23 @@ __device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g,
 // re-selected by the heuristic over the closest ef_construction members of
 //   sCand = {p} U one-hop(p) U two-hop(p)   (minus nb itself),
 // distances measured from nb.  One warp per updated point; sCand (<= 1 + 2M + 2M*2M ids) is gathered
-// into `upd_cand`.  Rows are written under a per-row spin lock (bb.row_fill, idle in this phase) because
-// two updated points of one wave may share a neighbour.
+// into `upd_cand`.  Every warp reads the pre-wave graph.  When several moved points of one wave share a
+// neighbour, the latest in arrival order re-selects its row: update_tag_kernel leaves 1 + that wave index in
+// bb.row_fill (idle in this phase), only the winner computes the row, and it is staged (stage_row), so the
+// result does not depend on scheduling.
+static __global__ void update_tag_kernel(GraphView g, const uint8_t* __restrict__ levels, uint32_t cap,
+                                         const uint32_t* __restrict__ ids, uint32_t b, uint32_t* tag) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (pi >= b) return;
+  const uint32_t p = ids[pi];
+  const int level_p = min((int)levels[p], g.max_level);
+  for (int layer = 0; layer <= level_p; ++layer) {
+    const uint32_t nb = load_row(g, p, layer, lane);
+    if (nb != kInvalid) atomicMax(&tag[layer == 0 ? nb : cap + g.up_off[nb] + (uint32_t)(layer - 1)], pi + 1u);
+  }
+}
+
 template <int LPV, int NQ, int KPL>
 __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, WalkCfg cfg,
                                                                const uint32_t* __restrict__ ids, uint32_t b,
@@ -210,8 +282,6 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
   ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
   Aux a = aux_of(c);
   uint32_t* cand = bb.upd_cand + (size_t)pi * kUpdCandCap;
-  uint32_t* links0 = const_cast<uint32_t*>(g.links0);
-  uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
   const int level_p = min((int)bg.levels[p], g.max_level);
   for (int layer = 0; layer <= level_p; ++layer) {
     const uint32_t one = load_row(g, p, layer, c.lane);
@@ -230,19 +300,13 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
     const uint32_t Mmax = layer == 0 ? g.M0 : g.M;
     for (uint32_t j = 0; j < n1; ++j) {
       const uint32_t nbid = __shfl_sync(0xffffffffu, one, j);
+      const uint32_t rid = layer == 0 ? nbid : bg.cap + g.up_off[nbid] + (uint32_t)(layer - 1);
+      if (bb.row_fill[rid] != pi + 1u) continue;  // a later moved point of this wave re-selects this row
       // nb is always a member of sCand
       const uint32_t nsel = reselect_row<LPV, NQ, KPL>(c, g, a, cand, ncand, nbid, min(bg.efc, ncand - 1u), Mmax);
-      const uint32_t rid = layer == 0 ? nbid : bg.cap + g.up_off[nbid] + (uint32_t)(layer - 1);
-      uint32_t* row = layer == 0 ? links0 + (size_t)nbid * g.M0
-                                 : links_up + (size_t)(g.up_off[nbid] + (uint32_t)(layer - 1)) * g.M;
-      if (c.lane == 0)
-        while (atomicCAS(&bb.row_fill[rid], 0u, 1u) != 0u) {
-        }
-      __syncwarp();
+      uint32_t* row = stage_row(bb, rid, g.M0, c.lane);
       if (c.lane < Mmax) row[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
-      __threadfence();
       __syncwarp();
-      if (c.lane == 0) atomicExch(&bb.row_fill[rid], 0u);
     }
   }
 }
@@ -315,7 +379,8 @@ static __global__ void edge_scatter_kernel(BuildBuffers bb) {
 // a time, exactly like hnswlib's mutuallyConnectNewElement: append while the row
 // has room; when it is full re-select the row with the heuristic over
 // (existing + the one new link).  Only after kMaxSeqPrunes such re-selections
-// in one wave (hub rows) is the remainder folded into a single re-selection.
+// in one wave (hub rows) is the remainder -- every record of the row with a higher
+// source id, however many -- folded into a single re-selection.
 constexpr uint32_t kMaxSeqPrunes = 3;
 
 template <int LPV, int NQ>
@@ -395,14 +460,15 @@ __global__ void __launch_bounds__(128) merge_rows_kernel(BuildGraph bg, WalkCfg 
     list_insert(c, make_key(sd, sid), limit);
     bool fold_rest = ++prunes > kMaxSeqPrunes;
     if (fold_rest) {
-      for (uint32_t i2 = i + 1; i2 < ninc; ++i2) {
-        uint32_t sv2 = in_src[0], jv2 = in_j[0];
-#pragma unroll
-        for (int s = 1; s < 4; ++s)
-          if ((i2 >> 5) == (uint32_t)s) sv2 = in_src[s], jv2 = in_j[s];
-        uint32_t sid2 = __shfl_sync(0xffffffffu, sv2, i2 & 31);
-        uint32_t sj2 = __shfl_sync(0xffffffffu, jv2, i2 & 31);
-        list_insert(c, make_key(bb.seg_dist[start + sj2], sid2), limit);  // list_insert drops duplicate ids
+      // every record not applied yet (source id above sid), read from the whole segment: a hub row can receive
+      // more records than the `limit` lowest source ids ordered above.  The list keeps the `limit` closest by
+      // (distance, id) whatever the insertion order; list_insert drops duplicate ids.
+      for (uint32_t j0 = 0; j0 < ninc_all; j0 += 32) {
+        const uint32_t j = j0 + c.lane;
+        const uint32_t s2 = j < ninc_all ? bb.seg_src[start + j] : 0u;
+        const uint64_t key = j < ninc_all && s2 > sid ? make_key(bb.seg_dist[start + j], s2) : kMaxKey;
+        for (uint32_t q = __ballot_sync(0xffffffffu, key != kMaxKey); q; q &= q - 1)
+          list_insert(c, __shfl_sync(0xffffffffu, key, __ffs(q) - 1), limit);
       }
     }
     uint32_t nsel = heuristic_select<LPV, NQ>(c, g, W, a);
@@ -417,6 +483,13 @@ __global__ void __launch_bounds__(128) merge_rows_kernel(BuildGraph bg, WalkCfg 
     bb.row_cnt[r] = 0;
     bb.row_fill[r] = 0;
   }
+}
+
+static cudaError_t apply_staged(const BuildGraph& bg, const BuildBuffers& bb, cudaStream_t s) {
+  const uint64_t threads = (uint64_t)bb.side_cap * bg.g.M0;
+  apply_staged_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(
+      bb, const_cast<uint32_t*>(bg.g.links0), const_cast<uint32_t*>(bg.g.links_up), bg.cap, bg.g.M0, bg.g.M);
+  return cudaGetLastError();
 }
 
 template <uint32_t DPAD>
@@ -437,6 +510,11 @@ cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, c
     if ((e = cudaFuncSetAttribute(ku, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)uwsm * uwpb))) !=
         cudaSuccess)
       return e;
+    if (mode == kBuildUpdate) {
+      if (!bb.side_row || !bb.side_out || !bb.side_count) return cudaErrorInvalidValue;
+      if ((e = cudaMemsetAsync(bb.side_count, 0, 4, s)) != cudaSuccess) return e;
+      update_tag_kernel<<<(b + 3) / 4, 128, 0, s>>>(bg.g, bg.levels, bg.cap, ids, b, bb.row_fill);
+    }
     // one warp per moved point / repaired row; repairs go in launches of <= kRepairWarps rows (upd_cand slots)
     const uint32_t chunk = mode == kBuildUpdate ? b : kRepairWarps;
     for (uint32_t off = 0; off < b; off += chunk) {
@@ -447,6 +525,8 @@ cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, c
     }
     // updatePoint's neighbour re-selection runs before the moved points are re-linked
     if (mode == kBuildRepair) return cudaGetLastError();
+    if ((e = apply_staged(bg, bb, s)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(bb.side_count, 0, 4, s)) != cudaSuccess) return e;
   }
   if ((e = cudaMemsetAsync(bb.edge_count, 0, 4, s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(bb.touched_count, 0, 4, s)) != cudaSuccess) return e;
@@ -471,6 +551,7 @@ cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, c
   edge_count_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);
   edge_alloc_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);
   edge_scatter_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);
+  if (is_update && (e = apply_staged(bg, bb, s)) != cudaSuccess) return e;  // the moved points' own rows
   km<<<(ethreads + mwpb - 1) / mwpb, 32 * mwpb, msmem, s>>>(bg, mcfg, bb, mwsm);
   return cudaGetLastError();
 }

@@ -288,13 +288,14 @@ struct ehb_index {
 
   // build scratch
   ehb::DevBuf<uint32_t> b_edge_row, b_edge_src, b_row_cnt, b_row_fill, b_row_start, b_touched, b_seg_src, b_counters,
-      b_ids, b_upd_cand;
+      b_ids, b_upd_cand, b_side_row, b_side_out;
   ehb::DevBuf<float> b_edge_dist, b_seg_dist, b_stage_in;
 
   // tuning (0 = auto)
   uint32_t t_slots = 0, t_groups = 0, t_hash_bits = 0, t_wpb = 0, t_team = 0;
   // options (ehb_index_set_option)
   uint32_t o_build_frac = 0;     // a wave links at most n_linked / build_frac points (0 = 64)
+  uint64_t o_seq_updates = 4096; // up to this many pending moves are re-linked one point per wave
   bool o_bf16_unfused = false;   // bf16 brute force: keep the distance tiles in HBM (A/B)
   bool o_combine = true;         // coalesce concurrent small host searches
   // L2 prefetch of the speculated next hop's vectors (rows <= 1 KB).  Off: already-visited neighbours and wrong

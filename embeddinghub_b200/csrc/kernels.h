@@ -146,6 +146,11 @@ struct BuildBuffers {
   uint32_t* error_flag; // [1]
   uint32_t* upd_cand;   // [batch][kUpdCandCap] sCand scratch of the update path (nullptr for plain inserts)
   uint32_t* repair_out; // [rows][M0] re-selected rows of the compaction repair (nullptr otherwise)
+  // update path: rows staged until every warp of the phase has read the graph (build_impl.cuh stage_row)
+  uint32_t* side_row;   // [side_cap] row id (edge_row convention)
+  uint32_t* side_out;   // [side_cap + 1][M0] the new rows (+ one sink slot)
+  uint32_t* side_count;
+  uint32_t side_cap;
 };
 struct BuildGraph {
   GraphView g;          // links are written through these pointers (const-cast inside)

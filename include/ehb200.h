@@ -355,6 +355,9 @@ int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a pe
 /* Named integer options (A/B switches and construction knobs that are not part of
  * the reference's surface).  Unknown names fail with EHB_ERR_INVALID.
  *   "build_frac"    a construction wave links at most size/build_frac points (0 = default 64)
+ *   "seq_updates"   up to this many pending moves of existing labels are re-linked one point at a time at a
+ *                   build (default 4096, hnswlib's sequential updatePoint); more go in waves of build_batch
+ *                   (default 1024)
  *   "bf16_unfused"  bf16 brute force keeps the distance tiles in HBM (A/B of the fused epilogue)
  *   "combine"       1 (default): concurrent host searches of <= 256 queries share batched launches
  *   "table_chunk"   live points per batch of ehb_index_neighbor_table (default 65536, 1..2^31)
