@@ -163,6 +163,11 @@ def _check_key(rc, labels):
     check(rc)
 
 
+def _alloc(nq, k):
+    """Result buffers of nq queries at k; the counts start at 0, which is what a call with k == 0 leaves them."""
+    return np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
+
+
 class NativeIndex:
     """Thin owner of an ehb_index handle; numpy in / numpy out (host entry points)."""
 
@@ -219,10 +224,7 @@ class NativeIndex:
     def remove(self, labels):
         """Tombstones (hnswlib markDelete): KeyError for an unknown label."""
         lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
-        rc = lib().ehb_index_remove(self._h, lab.shape[0], _p(lab))
-        if rc == 5:
-            raise KeyError(labels)
-        check(rc)
+        _check_key(lib().ehb_index_remove(self._h, lab.shape[0], _p(lab)), labels)
 
     def compact(self):
         """Drops every tombstone and repairs the graph on the GPU: size() counts the survivors, labels and vectors
@@ -250,10 +252,7 @@ class NativeIndex:
 
     def get(self, label):
         out = np.empty(self.dim, np.float32)
-        rc = lib().ehb_index_get(self._h, int(label), _p(out))
-        if rc == 5:
-            raise KeyError(label)
-        check(rc)
+        _check_key(lib().ehb_index_get(self._h, int(label), _p(out)), label)
         return out
 
     def get_batch(self, labels):
@@ -264,27 +263,20 @@ class NativeIndex:
         _check_key(lib().ehb_index_get_batch(self._h, lab.shape[0], _p(lab), _p(out)), labels)
         return out
 
-    def _alloc(self, nq, k):
-        return (np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.empty(nq, np.uint32))
-
     def search(self, q, k, ef=0, precision=FP32):
         """Graph search.  precision=BF16 walks the bf16 copy of the rows and re-ranks the walk's whole result set
         in fp32: every distance is the exact fp32 one (ehb_index_search_ex)."""
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
-        labels, dists, counts = self._alloc(q.shape[0], k)
+        labels, dists, counts = _alloc(q.shape[0], k)
         check(lib().ehb_index_search_ex(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
                                         _p(counts)))
-        if k == 0:
-            counts[:] = 0
         return labels, dists, counts
 
     def search_bruteforce(self, q, k, precision=FP32):
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
-        labels, dists, counts = self._alloc(q.shape[0], k)
+        labels, dists, counts = _alloc(q.shape[0], k)
         check(lib().ehb_index_search_bruteforce(self._h, q.shape[0], _p(q), k, precision, _p(labels), _p(dists),
                                                 _p(counts)))
-        if k == 0:
-            counts[:] = 0
         return labels, dists, counts
 
     def search_by_label(self, labels, k, ef=0, precision=FP32):
@@ -292,21 +284,17 @@ class NativeIndex:
         The point's row is searched at k + 1; its own label is removed, or the last hit dropped when it is absent
         (ehb_index_search_by_label_ex).  KeyError for an unknown or deleted label."""
         lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
-        out_l, out_d, out_c = self._alloc(lab.shape[0], k)
+        out_l, out_d, out_c = _alloc(lab.shape[0], k)
         _check_key(lib().ehb_index_search_by_label_ex(self._h, lab.shape[0], _p(lab), k, ef, int(precision), _p(out_l),
                                                       _p(out_d), _p(out_c)), labels)
-        if k == 0:
-            out_c[:] = 0
         return out_l, out_d, out_c
 
     def search_bruteforce_by_label(self, labels, k, precision=FP32):
         """search_by_label over the exact (or bf16) brute force at k + 1 (ehb_index_search_bruteforce_by_label)."""
         lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
-        out_l, out_d, out_c = self._alloc(lab.shape[0], k)
+        out_l, out_d, out_c = _alloc(lab.shape[0], k)
         _check_key(lib().ehb_index_search_bruteforce_by_label(self._h, lab.shape[0], _p(lab), k, int(precision),
                                                               _p(out_l), _p(out_d), _p(out_c)), labels)
-        if k == 0:
-            out_c[:] = 0
         return out_l, out_d, out_c
 
     def neighbor_table(self, k, ef=0, precision=FP32):
@@ -315,14 +303,11 @@ class NativeIndex:
         st = self.stats()
         rows = st["size"] - st["deleted"]
         q = np.empty(rows, np.uint64)
-        out_l, out_d, out_c = self._alloc(rows, k)
+        out_l, out_d, out_c = _alloc(rows, k)
         got = C.c_uint64(rows)
         check(lib().ehb_index_neighbor_table(self._h, k, ef, int(precision), _p(q), _p(out_l), _p(out_d), _p(out_c),
                                              C.byref(got)))
-        if k == 0:
-            out_c[:] = 0
-            return q[:0], out_l[:0], out_d[:0], out_c[:0]
-        n = got.value
+        n = got.value if k else 0
         return q[:n], out_l[:n], out_d[:n], out_c[:n]
 
     def search_dev(self, q_ptr, nq, k, ef, labels_ptr, dists_ptr, counts_ptr, stream=0, precision=FP32):
@@ -438,10 +423,7 @@ class ShardedIndex:
 
     def remove(self, labels):
         lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
-        rc = lib().ehb_sharded_remove(self._h, lab.shape[0], _p(lab))
-        if rc == 5:
-            raise KeyError(labels)
-        check(rc)
+        _check_key(lib().ehb_sharded_remove(self._h, lab.shape[0], _p(lab)), labels)
 
     def build(self):
         check(lib().ehb_sharded_build(self._h))
@@ -451,10 +433,7 @@ class ShardedIndex:
 
     def get(self, label):
         out = np.empty(self.dim, np.float32)
-        rc = lib().ehb_sharded_get(self._h, int(label), _p(out))
-        if rc == 5:
-            raise KeyError(label)
-        check(rc)
+        _check_key(lib().ehb_sharded_get(self._h, int(label), _p(out)), label)
         return out
 
     def get_batch(self, labels):
@@ -466,10 +445,9 @@ class ShardedIndex:
     def search_by_label(self, labels, k, ef=0, precision=FP32):
         """NativeIndex.search_by_label on the sharded index (ehb_sharded_search_by_label_ex)."""
         lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
-        nq = lab.shape[0]
-        out_l, out_d, out_c = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
-        _check_key(lib().ehb_sharded_search_by_label_ex(self._h, nq, _p(lab), k, ef, int(precision), _p(out_l),
-                                                        _p(out_d), _p(out_c)), labels)
+        out_l, out_d, out_c = _alloc(lab.shape[0], k)
+        _check_key(lib().ehb_sharded_search_by_label_ex(self._h, lab.shape[0], _p(lab), k, ef, int(precision),
+                                                        _p(out_l), _p(out_d), _p(out_c)), labels)
         return out_l, out_d, out_c
 
     @property
@@ -488,15 +466,14 @@ class ShardedIndex:
 
     def search(self, q, k, ef=0, precision=FP32):
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
-        nq = q.shape[0]
-        labels, dists, counts = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
-        check(lib().ehb_sharded_search_ex(self._h, nq, _p(q), k, ef, int(precision), _p(labels), _p(dists),
+        labels, dists, counts = _alloc(q.shape[0], k)
+        check(lib().ehb_sharded_search_ex(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
                                           _p(counts)))
         return labels, dists, counts
 
     def search_bruteforce(self, q, k, precision=FP32):
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
-        nq = q.shape[0]
-        labels, dists, counts = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.zeros(nq, np.uint32)
-        check(lib().ehb_sharded_search_bruteforce(self._h, nq, _p(q), k, precision, _p(labels), _p(dists), _p(counts)))
+        labels, dists, counts = _alloc(q.shape[0], k)
+        check(lib().ehb_sharded_search_bruteforce(self._h, q.shape[0], _p(q), k, precision, _p(labels), _p(dists),
+                                                  _p(counts)))
         return labels, dists, counts

@@ -291,13 +291,13 @@ int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, con
                                uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
                                uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream) {
   if (!ex || !ix || !queries_dev || !out_labels_dev) return fail(EHB_ERR_INVALID, "null argument");
-  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
-  if (nq == 0 || k == 0 || nq * k > ex->max_elems) return fail(EHB_ERR_INVALID, "nq * k exceeds the exchange capacity");
-  if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
+  bool none;
   {
-    std::shared_lock<ehb::RwLock> lk(ix->rw);  // ef == 0 reads the index default
-    if (std::max(ef ? ef : ix->ef, k) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k) must be <= 512");
+    std::shared_lock<ehb::RwLock> lk(ix->rw);  // ef == 0 reads the index default; the search below gets the checked ef
+    RET(ehb::check_request(ix, false, precision, false, nq, k, k, &ef, &none));
   }
+  if (none || nq * k > ex->max_elems) return fail(EHB_ERR_INVALID, "nq * k exceeds the exchange capacity");
+  if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
   CU(cudaSetDevice(ex->device));
   std::lock_guard<std::mutex> g(ex->mu);
   ex->epoch++;
@@ -526,8 +526,8 @@ int ehb_sharded_size(ehb_sharded* sh, uint64_t* out) {
   return EHB_OK;
 }
 
-// Links every shard; the shards build concurrently (one host thread per device).
-int ehb_sharded_build(ehb_sharded* sh) {
+// Runs fn on every shard concurrently (one host thread per device) and reports the first shard's error.
+static int on_every_shard(ehb_sharded* sh, int (*fn)(ehb_index*)) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   std::lock_guard<std::mutex> g(sh->mu);
   const size_t G = sh->shard.size();
@@ -536,7 +536,7 @@ int ehb_sharded_build(ehb_sharded* sh) {
   std::vector<std::thread> th;
   for (size_t i = 0; i < G; ++i)
     th.emplace_back([&, i]() {
-      rc[i] = ehb_index_build(sh->shard[i]);
+      rc[i] = fn(sh->shard[i]);
       if (rc[i] != EHB_OK) msg[i] = ehb::last_error_text();
     });
   for (auto& t : th) t.join();
@@ -545,24 +545,11 @@ int ehb_sharded_build(ehb_sharded* sh) {
   return EHB_OK;
 }
 
-// Compacts every shard; the shards compact concurrently (one host thread per device).
-int ehb_sharded_compact(ehb_sharded* sh) {
-  if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  std::lock_guard<std::mutex> g(sh->mu);
-  const size_t G = sh->shard.size();
-  std::vector<int> rc(G, EHB_OK);
-  std::vector<std::string> msg(G);
-  std::vector<std::thread> th;
-  for (size_t i = 0; i < G; ++i)
-    th.emplace_back([&, i]() {
-      rc[i] = ehb_index_compact(sh->shard[i]);
-      if (rc[i] != EHB_OK) msg[i] = ehb::last_error_text();
-    });
-  for (auto& t : th) t.join();
-  for (size_t i = 0; i < G; ++i)
-    if (rc[i] != EHB_OK) return fail(rc[i], msg[i]);
-  return EHB_OK;
-}
+// Links every shard; the shards build concurrently.
+int ehb_sharded_build(ehb_sharded* sh) { return on_every_shard(sh, ehb_index_build); }
+
+// Compacts every shard; the shards compact concurrently.
+int ehb_sharded_compact(ehb_sharded* sh) { return on_every_shard(sh, ehb_index_compact); }
 
 int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
@@ -572,9 +559,9 @@ int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
 
 // Every shard searches, device 0 merges into m_labels / m_dists / m_counts (queued on st[0]).  Caller holds mu.
 // q: host queries, or nullptr when every q_dev already holds them (queued on the shards' streams).
-// mode: 0 = graph walk, 1 = exact brute force, 2 = bf16 brute force.
-// precision: of the graph walk (a bf16 walk re-ranks straight into device 0's gather block, like the fp32 walk).
-static int sharded_merge(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
+// brute: the exact / bf16 brute force instead of the graph walk (a bf16 walk re-ranks straight into device 0's gather
+// block, like the fp32 walk).
+static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
                          int precision) {
   const uint32_t G = (uint32_t)sh->shard.size();
   const uint32_t dim = sh->prm.dim;
@@ -602,11 +589,10 @@ static int sharded_merge(ehb_sharded* sh, int mode, uint64_t nq, const float* q,
     }
     uint64_t* dl = (uint64_t*)dst;
     float* dd = (float*)(dst + nq * k * 8ull);
-    if (mode == 0)
-      RET(ehb_index_search_ex_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, ef, precision, dl, dd, sh->cnt_dev[i]->p, s));
+    if (brute)
+      RET(ehb_index_search_bruteforce_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, precision, dl, dd, sh->cnt_dev[i]->p, s));
     else
-      RET(ehb_index_search_bruteforce_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, mode == 2 ? EHB_BF16 : EHB_FP32, dl, dd,
-                                          sh->cnt_dev[i]->p, s));
+      RET(ehb_index_search_ex_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, ef, precision, dl, dd, sh->cnt_dev[i]->p, s));
     CU(cudaSetDevice(sh->dev[i]));
     if (i && !sh->peer_direct && sh->dev[i] != sh->dev[0])
       CU(cudaMemcpyPeerAsync(sh->gather.p + blk * i, sh->dev[0], dst, sh->dev[i], nq * k * 12ull, s));
@@ -619,34 +605,43 @@ static int sharded_merge(ehb_sharded* sh, int mode, uint64_t nq, const float* q,
   return EHB_OK;
 }
 
+// ehb::check_request on every shard, each under its reader lock (ef == 0 reads the shard's default; each shard's search
+// resolves and checks it again under its own lock).
+static int check_shards(ehb_sharded* sh, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
+                        uint64_t k_walk, uint32_t ef, bool* none) {
+  for (ehb_index* ix : sh->shard) {
+    std::shared_lock<ehb::RwLock> lk(ix->rw);
+    uint32_t ef_shard = ef;
+    RET(ehb::check_request(ix, brute, precision, null_buf, nq, k, k_walk, brute ? nullptr : &ef_shard, none));
+  }
+  return EHB_OK;
+}
+
 // Host queries in, merged host results out.
-static int sharded_search(ehb_sharded* sh, int mode, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
+static int sharded_search(ehb_sharded* sh, bool brute, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
                           int precision, uint64_t* ol, float* od, uint32_t* oc) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
-  if (nq && (!q || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
-  if (nq == 0 || k == 0) return EHB_OK;
+  bool none;
+  RET(check_shards(sh, brute, precision, nq && (!q || !ol), nq, k, k, ef, &none));
+  if (none) return EHB_OK;
   std::lock_guard<std::mutex> g(sh->mu);
-  RET(sharded_merge(sh, mode, nq, q, k, ef, precision));
-  cudaStream_t s0 = sh->st[0];
-  CU(cudaMemcpyAsync(ol, sh->m_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s0));
-  if (od) CU(cudaMemcpyAsync(od, sh->m_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s0));
-  if (oc) CU(cudaMemcpyAsync(oc, sh->m_counts.p, nq * 4, cudaMemcpyDeviceToHost, s0));
-  CU(cudaStreamSynchronize(s0));
+  RET(sharded_merge(sh, brute, nq, q, k, ef, precision));
+  RET(ehb::copy_results(nq, k, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, ol, od, oc, sh->st[0]));
+  CU(cudaStreamSynchronize(sh->st[0]));
   return EHB_OK;
 }
 
 int ehb_sharded_search(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, uint32_t ef, uint64_t* ol, float* od,
                        uint32_t* oc) {
-  return sharded_search(sh, 0, nq, q, k, ef, EHB_FP32, ol, od, oc);
+  return sharded_search(sh, false, nq, q, k, ef, EHB_FP32, ol, od, oc);
 }
 int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
                           uint64_t* ol, float* od, uint32_t* oc) {
-  return sharded_search(sh, 0, nq, q, k, ef, precision, ol, od, oc);
+  return sharded_search(sh, false, nq, q, k, ef, precision, ol, od, oc);
 }
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, int precision, uint64_t* ol,
                                   float* od, uint32_t* oc) {
-  return sharded_search(sh, precision == EHB_BF16 ? 2 : 1, nq, q, k, 0, EHB_FP32, ol, od, oc);
+  return sharded_search(sh, true, nq, q, k, 0, precision, ol, od, oc);
 }
 
 int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, float* out) {
@@ -677,11 +672,10 @@ int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, f
 int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
                                    int precision, uint64_t* ol, float* od, uint32_t* oc) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
-  if (nq && (!labels || !ol)) return fail(EHB_ERR_INVALID, "null buffer");
-  if (nq == 0 || k == 0) return EHB_OK;
+  bool none;
+  RET(check_shards(sh, false, precision, nq && (!labels || !ol), nq, k, k + 1ull, ef, &none));
+  if (none) return EHB_OK;
   const uint32_t k1 = k + 1;
-  if (std::max(ef, k1) > ehb::kMaxEf) return fail(EHB_ERR_INVALID, "max(ef, k + 1) must be <= 512");
   std::lock_guard<std::mutex> g(sh->mu);
   const uint32_t G = (uint32_t)sh->shard.size();
   const uint32_t dim = sh->prm.dim;
@@ -727,7 +721,7 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
     CU(cudaMemcpyAsync(sh->q_pos[i]->p, order.data(), nq * 4, cudaMemcpyHostToDevice, s));
     CU(ehb::launch_gather_rows(sh->q_stage[i]->p, dim, nullptr, sh->q_dev[i]->p, dim, sh->q_pos[i]->p, nq, dim, s));
   }
-  RET(sharded_merge(sh, 0, nq, nullptr, k1, ef, precision));
+  RET(sharded_merge(sh, false, nq, nullptr, k1, ef, precision));
   CU(cudaSetDevice(sh->dev[0]));
   cudaStream_t s0 = sh->st[0];
   CU(sh->s_self.grow(nq, 0, -1, s0));
@@ -737,9 +731,7 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
   CU(cudaMemcpyAsync(sh->s_self.p, labels, nq * 8, cudaMemcpyHostToDevice, s0));
   CU(ehb::launch_drop_self(sh->s_self.p, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, nq, k, sh->s_labels.p,
                            sh->s_dists.p, sh->s_counts.p, s0));
-  CU(cudaMemcpyAsync(ol, sh->s_labels.p, nq * k * 8, cudaMemcpyDeviceToHost, s0));
-  if (od) CU(cudaMemcpyAsync(od, sh->s_dists.p, nq * k * 4, cudaMemcpyDeviceToHost, s0));
-  if (oc) CU(cudaMemcpyAsync(oc, sh->s_counts.p, nq * 4, cudaMemcpyDeviceToHost, s0));
+  RET(ehb::copy_results(nq, k, sh->s_labels.p, sh->s_dists.p, sh->s_counts.p, ol, od, oc, s0));
   CU(cudaStreamSynchronize(s0));
   return EHB_OK;
 }

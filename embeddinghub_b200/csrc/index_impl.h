@@ -199,6 +199,21 @@ constexpr uint32_t kCombineLeaders = 2;    // batches in flight (copies of one o
 constexpr uint32_t kDeletedQueue = 64;     // side queue of tombstoned candidates per walking warp
 constexpr uint32_t kScreenMinBatchPerSm = 4;  // default fp32 walk screen: batches of >= 4 queries per SM
 
+class SlotLease;
+
+// The checks every search entry point makes before it touches the index, in this order: the precision, the buffers
+// (null_buf: the entry point found a pointer it needs null), then k == 0 or nq == 0, which sets *none (the call does
+// nothing and returns EHB_OK), then the width: max(*ef, k_walk) <= 512 for the graph walk; k_walk <= 2048 and, at bf16,
+// a dim padded to whole 64-wide blocks for the brute force.  k_walk is k + 1 for the by-label searches, k otherwise.
+// ef (graph walk; nullptr for the brute force): in, the requested beam, 0 for the index default; out, the beam that was
+// checked, which the search must use: the default can change while ensure_built drops the lock.  Caller holds the
+// reader side of ix->rw.
+int check_request(const ehb_index* ix, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
+                  uint64_t k_walk, uint32_t* ef, bool* none);
+// Queues the copies of nq result rows of k to the host on s: labels, and dists / counts where the host asked for them.
+int copy_results(uint64_t nq, uint32_t k, const uint64_t* dl, const float* dd, const uint32_t* dc, uint64_t* ol,
+                 float* od, uint32_t* oc, cudaStream_t s);
+
 }  // namespace ehb
 
 // ehb_index_search_dev with a result sink (exchange.cu)
@@ -261,11 +276,10 @@ struct ehb_index {
   uint32_t cq_leaders = 0;
   std::atomic<uint64_t> combined_batches{0}, combined_queries{0};
 
-  // brute-force scratch (one brute-force search at a time: bf_mu)
+  // brute-force scratch (one brute-force search at a time: bf_mu; a host call stages in a search slot)
   std::mutex bf_mu;
-  ehb::DevBuf<float> bf_q_in, bf_o_dists, bf_dist, bf_qpad;
-  ehb::DevBuf<uint64_t> bf_o_labels, bf_part, bf_run;
-  ehb::DevBuf<uint32_t> bf_o_counts;
+  ehb::DevBuf<float> bf_dist, bf_qpad;
+  ehb::DevBuf<uint64_t> bf_part, bf_run;
   ehb::DevBuf<uint16_t> q_bf16;
   ehb::DevBuf<float> q_norm2, bf_thr;
   ehb::DevBuf<uint64_t> bf_cbuf;
@@ -341,8 +355,11 @@ struct ehb_index {
   int create_shadow();
   int derive_rows(uint64_t first, uint64_t cnt);  // re-derive rows [first, first + cnt) of every copy that exists
   void drop_derived();
-  int acquire_slot(ehb::SearchSlot** out);
-  void release_slot(ehb::SearchSlot* sl, cudaStream_t used);
+  // what a search of nq queries needs before it runs: the graph built (walk) and the copies it reads (ensure_built,
+  // ensure_shadow)
+  int prepare(std::shared_lock<ehb::RwLock>& lk, bool brute, int precision, uint64_t nq);
+  // Caller holds the reader lock and has checked the request (ehb::check_request); `sl` is leased on s.  ef is the
+  // beam the check resolved and passed (never 0).
   // sink (optional): extra destinations + slice flags for the sharded exchange; *pushed tells whether the
   // launched kernel honoured it (the one-warp walk does, the team walk does not)
   // precision EHB_BF16 walks the bf16 shadow (caller made sure it exists) and re-ranks the retained set in fp32
@@ -353,3 +370,22 @@ struct ehb_index {
                      cudaStream_t s);
   void reset_content();
 };
+
+namespace ehb {
+// The only way to use a search slot: one for the length of a call.  take() acquires a slot from ix's pool and orders
+// `s` (nullptr: the slot's own stream) after the slot's previous user; the destructor records the slot's `busy` event
+// on `s` and returns the slot, so the next user waits for this call's work without a host synchronisation.
+class SlotLease {
+ public:
+  explicit SlotLease(ehb_index* ix) : ix_(ix) {}
+  SlotLease(const SlotLease&) = delete;
+  SlotLease& operator=(const SlotLease&) = delete;
+  ~SlotLease();
+  int take(cudaStream_t stream = nullptr);
+  SearchSlot* sl = nullptr;
+  cudaStream_t s = nullptr;
+
+ private:
+  ehb_index* ix_;
+};
+}  // namespace ehb

@@ -178,7 +178,9 @@ int ehb_index_search_ex_dev(ehb_index* ix, uint64_t nq, const float* queries_dev
  * the north star).  EHB_FP32 is exact with a defined total order (distance asc,
  * insertion index asc) and canonical arithmetic (one fp32 FMA chain, k
  * ascending) so ids are reproducible bit-for-bit.  EHB_BF16 is the tensor-core
- * path (bf16 GEMM + fp32 re-rank of an oversampled candidate set). */
+ * path (bf16 GEMM + fp32 re-rank of an oversampled candidate set).  An unknown
+ * precision fails with EHB_ERR_INVALID whatever k and nq are, as in the graph
+ * search, and so does ehb_sharded_search_bruteforce. */
 int ehb_index_search_bruteforce(ehb_index* ix, uint64_t nq, const float* queries_host, uint32_t k, int precision,
                                 uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
 int ehb_index_search_bruteforce_dev(ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k, int precision,
@@ -342,7 +344,9 @@ int ehb_exchange_merge_dev(ehb_exchange* ex, float* out_dists_dev, uint64_t* out
  * of ehb_index_search_ex_dev at EHB_BF16, merged.  The first EHB_BF16 step creates the index's bf16 copy of its
  * rows, as any first bf16 search does.  shard_counts_dev ([nq], this shard's hit counts) may be NULL.  An unknown
  * precision, a null pointer, nq * k above the capacity and max(ef, k) > 512 fail before the step starts, so the
- * next step still pairs with the peers' (call it on every rank, so every rank fails the same way).
+ * next step still pairs with the peers' (call it on every rank, so every rank fails the same way).  These are
+ * checked as in any search (precision, then max(ef, k)) before the exchange's own state, so a call that is both too
+ * wide and made before the peers are attached fails with EHB_ERR_INVALID, not EHB_ERR_STATE.
  * ehb_exchange_search_dev is exactly the _ex form with EHB_FP32. */
 int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
                             uint32_t ef, float* out_dists_dev, uint64_t* out_labels_dev, uint32_t* out_counts_dev,
