@@ -119,6 +119,7 @@ SYMBOLS = {
     "ehb_sharded_get_batch": (C.c_int, [_VP, _U64, _VP, _VP]),
     "ehb_sharded_search_by_label_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_exchange_create": (C.c_int, [_I32, _U32, _U32, _U64, _U32, C.POINTER(_VP)]),
+    "ehb_exchange_create_ex": (C.c_int, [_I32, _U32, _U32, _U64, _U32, _U32, C.POINTER(_VP)]),
     "ehb_exchange_destroy": (C.c_int, [_VP]),
     "ehb_exchange_ipc_handle": (C.c_int, [_VP, _VP]),
     "ehb_exchange_open": (C.c_int, [_VP, _VP]),
@@ -127,6 +128,7 @@ SYMBOLS = {
     "ehb_exchange_merge_dev": (C.c_int, [_VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_search_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_search_ex_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "ehb_exchange_search_by_label_ex_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP]),
     "ehb_exchange_timed_out": (C.c_int, [_VP, C.POINTER(_U32)]),
 }
 

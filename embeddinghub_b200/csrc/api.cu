@@ -1407,10 +1407,16 @@ int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k
 int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed) {
   ENTER_S(ix);
+  return ehb_index_search_dev_sink_held(ix, _g, nq, dq, k, ef, precision, sink, dc, stream, pushed);
+}
+
+int ehb_index_search_dev_sink_held(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, uint64_t nq, const float* dq,
+                                   uint32_t k, uint32_t ef, int precision, const ehb::ResultSink* sink, uint32_t* dc,
+                                   cudaStream_t stream, bool* pushed) {
   bool none;
   RET(ehb::check_request(ix, false, precision, !dq || !sink || !sink->n || !sink->labels[0], nq, k, k, &ef, &none));
   if (none) return EHB_OK;
-  RET(ix->prepare(_g, false, precision, nq));
+  RET(ix->prepare(lk, false, precision, nq));
   ehb::SlotLease ls(ix);
   RET(ls.take(stream));
   return ix->search_dev(ls.sl, nq, dq, k, ef, sink->labels[0], sink->dists[0], dc, ls.s, sink, pushed, precision);

@@ -77,6 +77,11 @@ cudaError_t launch_drop_self(const uint64_t* self, const uint64_t* in_labels, co
   return cudaGetLastError();
 }
 
+cudaError_t load_drop_self() {
+  cudaFuncAttributes a;
+  return cudaFuncGetAttributes(&a, drop_self_kernel);
+}
+
 // One block walks deleted[0..n) in tiles of 16 flags per thread; a block-wide exclusive scan of the live counts
 // places each live id, so ids come out ascending in a single pass.
 constexpr uint32_t kLiveThreads = 1024;

@@ -94,6 +94,104 @@ __global__ void __launch_bounds__(kExchangeThreads) exchange_merge_kernel(Exchan
   }
 }
 
+// The query rows of a by-label step (ehb_exchange_search_by_label_ex_dev) in every rank's exported block, as mapped
+// HERE.  All parity-indexed like the receive buffer.
+struct RowView {
+  float* rows[kMaxWorld];           // [2][row_stride]: a step of dimension dim uses [nq][dim] of its parity
+  unsigned char* marks[kMaxWorld];  // [2][world][max_nq]: marks[p][g][q] = 1 when rank g holds query q's label
+  uint64_t* digests[kMaxWorld];     // [2][world]: each rank's digest of its label list
+  uint32_t* flags[kMaxWorld];       // the flag array of the receive buffer
+  uint32_t world, rank;
+  uint64_t row_stride;              // floats per parity (a multiple of 64)
+  uint64_t max_nq;
+};
+
+// Bits of the verdict word of a row step.  Every rank reads the same digests, so kRowsDigest is set on every rank or on
+// none; when it is clear every rank was given the same list and reads the same marks, so the whole word is equal.
+constexpr uint32_t kRowsMissing = 1;   // a query that no rank holds
+constexpr uint32_t kRowsShared = 2;    // a query that more than one rank holds
+constexpr uint32_t kRowsDigest = 4;    // a peer's label list differs from this rank's
+constexpr uint32_t kRowsTimeout = 8;   // a peer never raised its flags (the timeout word is set too)
+
+// One persistent launch per rank (grid sized like exchange_merge_kernel).  Phase 1: every query this rank holds
+// (ids[q] != kInvalid) has its stored row copied from vecs (dpad stride) into row q of every rank's row region, this
+// rank's own included: one warp per row, each 16-byte chunk read once and stored to every destination.  The whole
+// mark vector and (with slice 0) the digest go to every rank too; then the slice flags, released at system scope.
+// Phase 2: wait for every peer's slice flags, count each query's holders over the ranks, compare the digests, and OR
+// the outcome into the local verdict word (zeroed before the launch).
+__global__ void __launch_bounds__(kExchangeThreads) exchange_rows_kernel(RowView v, uint32_t parity, uint32_t epoch,
+                                                             uint64_t nq, uint32_t qs, uint32_t nslices,
+                                                             const uint32_t* __restrict__ ids,
+                                                             const float* __restrict__ vecs, uint32_t dpad,
+                                                             uint32_t dim, uint64_t digest,
+                                                             uint32_t* __restrict__ verdict,
+                                                             uint32_t* __restrict__ timeout_flag) {
+  const uint32_t W = v.world, me = v.rank;
+  const uint32_t warps = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // the row region is 256-byte aligned and each parity's part starts a whole number of 64 floats in
+  // (ehb_exchange::row_stride), so a row q * dim floats in is 16-byte aligned when dim is; dpad is a multiple of 4
+  const bool vec4 = (dim & 3) == 0;
+  const uint64_t row0 = (uint64_t)parity * v.row_stride;
+  // ---- phase 1: rows, marks and digest to every rank, then the flags ------------------------------------------
+  for (uint32_t s = blockIdx.x; s < nslices; s += gridDim.x) {
+    const uint64_t q0 = min(nq, (uint64_t)s * qs), q1 = min(nq, q0 + qs);
+    for (uint64_t q = q0 + w; q < q1; q += warps) {
+      const uint32_t id = ids[q];
+      if (id == kInvalid) continue;
+      const float* src = vecs + (uint64_t)id * dpad;
+      const uint64_t at = row0 + q * dim;
+      if (vec4) {
+        for (uint32_t c = lane; c < dim / 4; c += 32) {
+          const float4 x = reinterpret_cast<const float4*>(src)[c];
+          for (uint32_t g = 0; g < W; ++g) reinterpret_cast<float4*>(v.rows[g] + at)[c] = x;
+        }
+      } else {
+        for (uint32_t c = lane; c < dim; c += 32) {
+          const float x = src[c];
+          for (uint32_t g = 0; g < W; ++g) v.rows[g][at + c] = x;
+        }
+      }
+    }
+    const uint64_t mine = ((uint64_t)parity * W + me) * v.max_nq;
+    for (uint64_t q = q0 + threadIdx.x; q < q1; q += blockDim.x) {
+      const unsigned char held = ids[q] != kInvalid;
+      for (uint32_t g = 0; g < W; ++g) v.marks[g][mine + q] = held;
+    }
+    if (s == 0 && threadIdx.x < W) v.digests[threadIdx.x][(uint64_t)parity * W + me] = digest;
+    __threadfence_system();  // every thread's stores are ordered before the flags below
+    __syncthreads();
+    if (threadIdx.x < W && threadIdx.x != me)
+      st_release_sys(v.flags[threadIdx.x] + ((uint64_t)parity * W + me) * kMaxSlices + s, epoch);
+    __syncthreads();
+  }
+  // ---- phase 2: wait for each slice from every peer, count the holders ---------------------------------------
+  for (uint32_t s = blockIdx.x; s < nslices; s += gridDim.x) {
+    if (threadIdx.x < W && threadIdx.x != me) {
+      const uint32_t* f = v.flags[me] + ((uint64_t)parity * W + threadIdx.x) * kMaxSlices + s;
+      uint32_t spins = 0;  // bounded (~20 s), as in exchange_merge_kernel
+      while (ld_acquire_sys(f) != epoch) {
+        __nanosleep(64);
+        if (++spins > (1u << 28)) {
+          atomicExch(timeout_flag, 1u);
+          atomicOr(verdict, kRowsTimeout);
+          break;
+        }
+      }
+    }
+    __syncthreads();
+    uint32_t bits = 0;
+    const uint64_t q0 = min(nq, (uint64_t)s * qs), q1 = min(nq, q0 + qs);
+    const unsigned char* marks = v.marks[me] + (uint64_t)parity * W * v.max_nq;
+    for (uint64_t q = q0 + threadIdx.x; q < q1; q += blockDim.x) {
+      uint32_t holders = 0;
+      for (uint32_t g = 0; g < W; ++g) holders += marks[(uint64_t)g * v.max_nq + q];
+      bits |= holders == 0 ? kRowsMissing : holders > 1 ? kRowsShared : 0u;
+    }
+    if (s == 0 && threadIdx.x < W && v.digests[me][(uint64_t)parity * W + threadIdx.x] != digest) bits |= kRowsDigest;
+    if (bits) atomicOr(verdict, bits);
+  }
+}
+
 }  // namespace ehb
 
 // =====================================================================================================
@@ -115,15 +213,36 @@ struct ehb_exchange {
   uint32_t slot_k = 0;
   int sms = 132;
   std::mutex mu;
+  // by-label steps (max_dim > 0).  In the exported block, after the receive buffer: the row region, the marks and the
+  // digests (ehb::RowView).  Local scratch: the resolved ids, the query labels, the merged k + 1 lists, the verdict word;
+  // pinned staging of the ids, labels and verdict; `bl_done` ends the last by-label step's use of the scratch.
+  uint64_t max_nq = 0;
+  uint32_t max_dim = 0;
+  size_t rows_off = 0, marks_off = 0, digests_off = 0;
+  uint64_t row_stride = 0;  // floats per parity of the row region: max_nq * max_dim rounded up to a multiple of 64
+  unsigned char* bl = nullptr;
+  uint32_t* bl_ids = nullptr;
+  uint64_t* bl_self = nullptr;
+  uint64_t* bl_labels = nullptr;
+  float* bl_dists = nullptr;
+  uint32_t* bl_counts = nullptr;
+  uint32_t* bl_verdict = nullptr;
+  unsigned char* bl_host = nullptr;  // [max_nq] u64 labels | [max_nq] u32 ids | u32 verdict
+  cudaEvent_t bl_done = nullptr;
 };
+
+namespace {
+size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+}  // namespace
 
 extern "C" {
 
-int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
-                        ehb_exchange** out) {
+int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
+                           uint32_t max_dim, ehb_exchange** out) {
   if (!out) return fail(EHB_ERR_INVALID, "null argument");
   if (world == 0 || world > ehb::kMaxWorld || rank >= world) return fail(EHB_ERR_INVALID, "bad world / rank");
   if (max_nq == 0 || max_k == 0) return fail(EHB_ERR_INVALID, "max_nq and max_k must be positive");
+  if (max_dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "max_dim must be <= 2048");
   CU(cudaSetDevice(device));
   ehb_exchange* ex = new (std::nothrow) ehb_exchange();
   if (!ex) return fail(EHB_ERR_OOM, "host allocation failed");
@@ -134,12 +253,46 @@ int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t 
   ex->stride = (ex->max_elems * 12ull + 255) / 256 * 256;
   ex->flag_bytes = (2ull * world * ehb::kMaxSlices * 4 + 4 + 4095) / 4096 * 4096;
   ex->total_bytes = ex->flag_bytes + 2ull * world * ex->stride;
+  ex->max_nq = max_nq;
+  ex->max_dim = max_dim;
+  if (max_dim) {
+    ex->row_stride = (max_nq * max_dim + 63) / 64 * 64;
+    ex->rows_off = ex->total_bytes;
+    ex->marks_off = ex->rows_off + round256(2ull * ex->row_stride * 4);
+    ex->digests_off = ex->marks_off + round256(2ull * world * max_nq);
+    ex->total_bytes = ex->digests_off + round256(2ull * world * 8);
+  }
   cudaDeviceGetAttribute(&ex->sms, cudaDevAttrMultiProcessorCount, device);
   cudaError_t e = cudaMalloc((void**)&ex->local, ex->total_bytes);
   if (e == cudaSuccess) e = cudaMemset(ex->local, 0, ex->flag_bytes);
   if (e == cudaSuccess) e = cudaMalloc((void**)&ex->slice_count, ehb::kMaxSlices * 4);
   if (e == cudaSuccess) e = cudaMemset(ex->slice_count, 0, ehb::kMaxSlices * 4);
+  if (e == cudaSuccess && max_dim) {
+    const size_t ids = round256(max_nq * 4), self = round256(max_nq * 8), labs = round256(ex->max_elems * 8),
+                 dists = round256(ex->max_elems * 4), counts = round256(max_nq * 4);
+    e = cudaMalloc((void**)&ex->bl, ids + self + labs + dists + counts + 256);
+    if (e == cudaSuccess) {
+      unsigned char* p = ex->bl;
+      ex->bl_ids = (uint32_t*)p;
+      ex->bl_self = (uint64_t*)(p += ids);
+      ex->bl_labels = (uint64_t*)(p += self);
+      ex->bl_dists = (float*)(p += labs);
+      ex->bl_counts = (uint32_t*)(p += dists);
+      ex->bl_verdict = (uint32_t*)(p += counts);
+      e = cudaMallocHost((void**)&ex->bl_host, max_nq * 12 + 4);
+    }
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ex->bl_done, cudaEventDisableTiming);
+    // load the step's own kernels now: under lazy module loading a first launch may wait for every kernel running in
+    // the context, and with two ranks in one process one of those is a peer's exchange kernel waiting for this rank
+    cudaFuncAttributes a;
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, ehb::exchange_rows_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, ehb::exchange_merge_kernel);
+    if (e == cudaSuccess) e = ehb::load_drop_self();
+  }
   if (e != cudaSuccess) {
+    if (ex->bl_done) cudaEventDestroy(ex->bl_done);
+    if (ex->bl_host) cudaFreeHost(ex->bl_host);
+    if (ex->bl) cudaFree(ex->bl);
     if (ex->slice_count) cudaFree(ex->slice_count);
     if (ex->local) cudaFree(ex->local);
     delete ex;
@@ -151,12 +304,20 @@ int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t 
   return EHB_OK;
 }
 
+int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
+                        ehb_exchange** out) {
+  return ehb_exchange_create_ex(device, world, rank, max_nq, max_k, 0, out);
+}
+
 int ehb_exchange_destroy(ehb_exchange* ex) {
   if (!ex) return EHB_OK;
   cudaSetDevice(ex->device);
   cudaDeviceSynchronize();
   for (uint32_t g = 0; g < ex->world; ++g)
     if (ex->opened[g]) cudaIpcCloseMemHandle(ex->mapped[g]);
+  if (ex->bl_done) cudaEventDestroy(ex->bl_done);
+  if (ex->bl_host) cudaFreeHost(ex->bl_host);
+  if (ex->bl) cudaFree(ex->bl);
   if (ex->slice_count) cudaFree(ex->slice_count);
   if (ex->local) cudaFree(ex->local);
   delete ex;
@@ -194,6 +355,7 @@ int ehb_exchange_open(ehb_exchange* ex, const void* handles) {
 // Same process, different device: attach a peer exchange directly (peer access must be possible).
 int ehb_exchange_attach_local(ehb_exchange* ex, uint32_t peer_rank, ehb_exchange* peer) {
   if (!ex || !peer || peer_rank >= ex->world || peer_rank == ex->rank) return fail(EHB_ERR_INVALID, "bad argument");
+  if (peer->max_dim != ex->max_dim) return fail(EHB_ERR_INVALID, "the peers' max_dim differ (their row regions would)");
   CU(cudaSetDevice(ex->device));
   if (peer->device != ex->device) {
     int can = 0;
@@ -263,6 +425,70 @@ int launch_exchange_merge(ehb_exchange* ex, uint64_t nq, uint32_t k, float* out_
   return EHB_OK;
 }
 
+// The destinations of this rank's [nq][k] results at the current epoch: its own block of its own buffer first, then
+// its block of every peer's buffer, with the slice flags the search's last kernel raises.
+ehb::ResultSink step_sink(ehb_exchange* ex, uint64_t nq, uint32_t k) {
+  const uint32_t parity = ex->epoch & 1u, W = ex->world, me = ex->rank;
+  const uint64_t blk = ((uint64_t)parity * W + me) * ex->stride;
+  uint32_t qs, nslices;
+  slice_plan(ex, nq, &qs, &nslices);
+  ehb::ResultSink sink;
+  std::memset(&sink, 0, sizeof(sink));
+  uint32_t t = 0;
+  auto add = [&](uint32_t r) {
+    unsigned char* base = ex->mapped[r] + ex->flag_bytes + blk;
+    sink.labels[t] = (uint64_t*)base;
+    sink.dists[t] = (float*)(base + nq * k * 8ull);
+    sink.flags[t] = (uint32_t*)ex->mapped[r] + ((uint64_t)parity * W + me) * ehb::kMaxSlices;
+    ++t;
+  };
+  add(me);  // destination 0 = my own block of my own buffer
+  for (uint32_t r = 0; r < W; ++r)
+    if (r != me) add(r);
+  sink.n = t;
+  sink.qs = qs;
+  sink.epoch = ex->epoch;
+  sink.slice_count = ex->slice_count;
+  return sink;
+}
+
+// The row step of a by-label search at the current epoch.  Its slice count does not depend on nq (every rank raises
+// the same flags whatever list it was given); the verdict word must be zero on `stream`.
+int launch_exchange_rows(ehb_exchange* ex, const ehb_index* ix, uint64_t nq, uint64_t digest, cudaStream_t stream) {
+  ehb::RowView v;
+  std::memset(&v, 0, sizeof(v));
+  for (uint32_t r = 0; r < ex->world; ++r) {
+    v.rows[r] = (float*)(ex->mapped[r] + ex->rows_off);
+    v.marks[r] = ex->mapped[r] + ex->marks_off;
+    v.digests[r] = (uint64_t*)(ex->mapped[r] + ex->digests_off);
+    v.flags[r] = (uint32_t*)ex->mapped[r];
+  }
+  v.world = ex->world;
+  v.rank = ex->rank;
+  v.row_stride = ex->row_stride;
+  v.max_nq = ex->max_nq;
+  const uint32_t nslices = std::min<uint32_t>(ehb::kMaxSlices, (uint32_t)ex->sms);
+  const uint32_t qs = (uint32_t)((nq + nslices - 1) / nslices);
+  const uint32_t grid = std::min<uint32_t>(nslices, std::max<uint32_t>(1, (uint32_t)ex->sms / ex->same_device_ranks));
+  ehb::exchange_rows_kernel<<<grid, ehb::kExchangeThreads, 0, stream>>>(
+      v, ex->epoch & 1u, ex->epoch, nq, qs, nslices, ex->bl_ids, ix->vecs.p, ix->dpad, ix->dim, digest, ex->bl_verdict,
+      (uint32_t*)(ex->local + ex->flag_bytes - 4));
+  CU(cudaGetLastError());
+  return EHB_OK;
+}
+
+// 64-bit digest of a label list (its length included): splitmix64's finaliser over a running sum
+uint64_t label_digest(uint64_t nq, const uint64_t* labels) {
+  auto mix = [](uint64_t z) {
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    return z ^ (z >> 31);
+  };
+  uint64_t h = mix(nq + 0x9e3779b97f4a7c15ull);
+  for (uint64_t i = 0; i < nq; ++i) h = mix(h + 0x9e3779b97f4a7c15ull + labels[i]);
+  return h;
+}
+
 }  // namespace
 
 extern "C" {
@@ -301,32 +527,73 @@ int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, con
   CU(cudaSetDevice(ex->device));
   std::lock_guard<std::mutex> g(ex->mu);
   ex->epoch++;
-  const uint32_t parity = ex->epoch & 1u, W = ex->world, me = ex->rank;
-  const uint64_t blk = ((uint64_t)parity * W + me) * ex->stride;
-  uint32_t qs, nslices;
-  slice_plan(ex, nq, &qs, &nslices);
-  ehb::ResultSink sink;
-  std::memset(&sink, 0, sizeof(sink));
-  uint32_t t = 0;
-  auto add = [&](uint32_t r) {
-    unsigned char* base = ex->mapped[r] + ex->flag_bytes + blk;
-    sink.labels[t] = (uint64_t*)base;
-    sink.dists[t] = (float*)(base + nq * k * 8ull);
-    sink.flags[t] = (uint32_t*)ex->mapped[r] + ((uint64_t)parity * W + me) * ehb::kMaxSlices;
-    ++t;
-  };
-  add(me);  // destination 0 = my own block of my own buffer
-  for (uint32_t r = 0; r < W; ++r)
-    if (r != me) add(r);
-  sink.n = t;
-  sink.qs = qs;
-  sink.epoch = ex->epoch;
-  sink.slice_count = ex->slice_count;
+  const ehb::ResultSink sink = step_sink(ex, nq, k);
   bool pushed = false;
   RET(ehb_index_search_dev_sink(ix, nq, queries_dev, k, ef, precision, &sink, shard_counts_dev, (cudaStream_t)stream,
                                 &pushed));
   CU(cudaSetDevice(ex->device));
   return launch_exchange_merge(ex, nq, k, out_dists_dev, out_labels_dev, out_counts_dev, (cudaStream_t)stream, pushed);
+}
+
+// Key mode over the exchange: a row step at epoch e (every holder pushes its stored rows to every rank, and every
+// rank agrees that each label has exactly one holder and that all ranks were given the same list), then the fused
+// k + 1 step at e + 1 over the pushed rows, the merge, and the self-removal.  The reader side of ix->rw is held from
+// prepare through the search launch, so the resolved ids cannot move under a compaction.  Locks in the order of
+// ehb_exchange_search_ex_dev: ex->mu first, then ix->rw (a writer-preferring lock taken in the other order by a
+// second thread on the same exchange could deadlock).
+int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                        uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                        uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream) {
+  if (!ex || !ix) return fail(EHB_ERR_INVALID, "null argument");
+  std::lock_guard<std::mutex> g(ex->mu);
+  std::shared_lock<ehb::RwLock> lk(ix->rw);
+  bool none;
+  RET(ehb::check_request(ix, false, precision, !labels_host || !out_labels_dev || !out_dists_dev || !out_counts_dev,
+                         nq, k, k + 1ull, &ef, &none));
+  if (none) return EHB_OK;
+  const uint32_t k1 = k + 1;
+  if (nq > ex->max_nq || nq * k1 > ex->max_elems)
+    return fail(EHB_ERR_INVALID, "nq or nq * (k + 1) exceeds the exchange capacity");
+  if (ix->dim > ex->max_dim) return fail(EHB_ERR_INVALID, "the exchange has no room for rows of this dim (max_dim)");
+  if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
+  CU(cudaSetDevice(ex->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  RET(ix->prepare(lk, false, precision, nq));
+  uint64_t* h_self = (uint64_t*)ex->bl_host;
+  uint32_t* h_ids = (uint32_t*)(h_self + ex->max_nq);
+  uint32_t* h_verdict = h_ids + ex->max_nq;
+  // hnswlib getDataByLabel, as ehb_index_get_batch: a tombstoned label is not held
+  for (uint64_t q = 0; q < nq; ++q)
+    if (!ix->find_id(labels_host[q], &h_ids[q]) || ix->h_deleted[h_ids[q]]) h_ids[q] = ehb::kInvalid;
+  std::memcpy(h_self, labels_host, nq * 8);
+  CU(cudaStreamWaitEvent(s, ex->bl_done, 0));  // the previous by-label step is done with the scratch
+  ex->epoch++;
+  const uint32_t parity = ex->epoch & 1u;
+  CU(cudaMemsetAsync(ex->bl_verdict, 0, 4, s));
+  CU(cudaMemcpyAsync(ex->bl_ids, h_ids, nq * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(ex->bl_self, h_self, nq * 8, cudaMemcpyHostToDevice, s));
+  RET(launch_exchange_rows(ex, ix, nq, label_digest(nq, labels_host), s));
+  CU(cudaMemcpyAsync(h_verdict, ex->bl_verdict, 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));  // the step's only host synchronisation
+  // every rank reads the same verdict and returns the same status; each has consumed epoch e, so they stay in phase.
+  // The digests decide first: they are fresh whatever lists the ranks were given, and a digest mismatch is seen by
+  // every rank.  Only when the lists agree (so nq agrees) are the marks all of this step, and the holder counts used.
+  const uint32_t v = *h_verdict;
+  if (v & ehb::kRowsTimeout) return fail(EHB_ERR_CUDA, "a peer did not arrive within ~20 s (ehb_exchange_timed_out)");
+  if (v & ehb::kRowsDigest) return fail(EHB_ERR_INVALID, "the ranks were given different label lists");
+  if (v & ehb::kRowsMissing) return fail(EHB_ERR_NOT_FOUND, "label not found on any rank");
+  if (v & ehb::kRowsShared) return fail(EHB_ERR_STATE, "a label is stored on more than one rank");
+  ex->epoch++;
+  const float* rows = (const float*)(ex->local + ex->rows_off) + parity * ex->row_stride;
+  const ehb::ResultSink sink = step_sink(ex, nq, k1);
+  bool pushed = false;
+  RET(ehb_index_search_dev_sink_held(ix, lk, nq, rows, k1, ef, precision, &sink, nullptr, s, &pushed));
+  CU(cudaSetDevice(ex->device));
+  RET(launch_exchange_merge(ex, nq, k1, ex->bl_dists, ex->bl_labels, ex->bl_counts, s, pushed));
+  CU(ehb::launch_drop_self(ex->bl_self, ex->bl_labels, ex->bl_dists, ex->bl_counts, nq, k, out_labels_dev,
+                           out_dists_dev, out_counts_dev, s));
+  CU(cudaEventRecord(ex->bl_done, s));
+  return EHB_OK;
 }
 
 int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,

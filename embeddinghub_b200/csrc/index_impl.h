@@ -219,6 +219,11 @@ int copy_results(uint64_t nq, uint32_t k, const uint64_t* dl, const float* dd, c
 // ehb_index_search_dev with a result sink (exchange.cu)
 int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed);
+// The same for a caller that already holds the reader side of ix->rw as `lk` (a second shared acquire would deadlock
+// behind a queued writer) and has made the device current
+int ehb_index_search_dev_sink_held(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, uint64_t nq, const float* dq,
+                                   uint32_t k, uint32_t ef, int precision, const ehb::ResultSink* sink, uint32_t* dc,
+                                   cudaStream_t stream, bool* pushed);
 // The stored rows of n live labels into rows_dev ([n][dim] on the index's device), queued on `stream`; an unknown or
 // tombstoned label fails with EHB_ERR_NOT_FOUND before anything is queued (exchange.cu: by-label sharded searches)
 int ehb_index_gather_dev(ehb_index* ix, uint64_t n, const uint64_t* labels_host, float* rows_dev, cudaStream_t stream);

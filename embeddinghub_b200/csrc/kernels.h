@@ -206,6 +206,10 @@ cudaError_t launch_gather_rows(const float* in, uint32_t in_stride, const uint32
 cudaError_t launch_drop_self(const uint64_t* self, const uint64_t* in_labels, const float* in_dists,
                              const uint32_t* in_counts, uint64_t nq, uint32_t k, uint64_t* out_labels,
                              float* out_dists, uint32_t* out_counts, cudaStream_t s);
+// Loads drop_self_kernel now rather than at its first launch: with lazy module loading a first launch can wait for
+// the kernels already running in the context, and in a key-mode exchange step one of those may be a peer's merge
+// that waits for this rank (ehb_exchange_create_ex).
+cudaError_t load_drop_self();
 // The ids i < n with deleted[i] == 0, ascending, into ids[0..*count).
 cudaError_t launch_live_ids(const uint8_t* deleted, uint64_t n, uint32_t* ids, uint32_t* count, cudaStream_t s);
 

@@ -65,7 +65,7 @@ class ShardedSearcher:
         self._torch = torch
         self._buf = {}
         self.exchange = exchange if world > 1 else "none"
-        self._ex, self._ex_cap = None, (0, 0)
+        self._ex, self._ex_cap = None, (0, 0, 0)
 
     def close(self):
         if self._ex is not None:
@@ -78,22 +78,23 @@ class ShardedSearcher:
         except Exception:
             pass
 
-    def _ensure_exchange(self, nq, k):
-        """(Re)creates the exchange when (nq, k) outgrow it.  Collective: every rank takes the same decision
-        because every rank searches the same batch.  The 64-byte IPC handles travel in one all_gather."""
+    def _ensure_exchange(self, nq, k, dim=0):
+        """(Re)creates the exchange when (nq, k) outgrow it, or when a key-mode step needs room for rows of `dim`
+        floats that it lacks.  Collective: every rank takes the same decision because every rank searches the same
+        batch.  The 64-byte IPC handles travel in one all_gather."""
         import torch.distributed as dist
 
         t = self._torch
-        if self._ex is not None and nq <= self._ex_cap[0] and k <= self._ex_cap[1]:
+        if self._ex is not None and nq <= self._ex_cap[0] and k <= self._ex_cap[1] and dim <= self._ex_cap[2]:
             return
         t.cuda.synchronize()
         if self._ex is not None:
             dist.barrier(group=self.group)   # no peer may still be storing into the buffer that is about to go
         self.close()
-        cap = (max(nq, self._ex_cap[0]), max(k, self._ex_cap[1]))
+        cap = (max(nq, self._ex_cap[0]), max(k, self._ex_cap[1]), max(dim, self._ex_cap[2]))
         rank = dist.get_rank(self.group)
         h = C.c_void_p()
-        check(lib().ehb_exchange_create(self.device, self.world, rank, cap[0], cap[1], C.byref(h)))
+        check(lib().ehb_exchange_create_ex(self.device, self.world, rank, cap[0], cap[1], cap[2], C.byref(h)))
         mine = np.zeros(64, np.uint8)
         check(lib().ehb_exchange_ipc_handle(h, mine.ctypes.data_as(C.c_void_p)))
         dev = t.device("cuda", self.device)
@@ -163,4 +164,38 @@ class ShardedSearcher:
                                               b["recv"].shape[1], C.c_void_p(b["md"].data_ptr()),
                                               C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
                                               self.device, C.c_void_p(stream_ptr)))
+        return b["ml"], b["md"], b["mc"]
+
+    def search_by_label_dev(self, labels, k, ef, stream_ptr, precision=0):
+        """Key mode (server.cc:190-207): the k nearest other points of stored points named by label.  `labels` (u64,
+        the same on every rank) may live on any rank; each is searched with its stored row at k + 1 and its own label
+        is removed, or the last hit dropped when it is absent.  Returns (labels int64-viewed-u64, dists, counts) CUDA
+        tensors [nq][k] holding the global result on every rank.  On the peer exchange this is one
+        ehb_exchange_search_by_label_ex_dev step: the owners push their rows to every rank, every rank agrees that
+        each label has exactly one owner (one 4-byte copy to the host), then the fused k + 1 step runs.  Raises
+        EhbError with the library's status, the same on every rank: 1 (different label lists), else 5 (not found),
+        else 4 (a label on two ranks).  At world 1 it is NativeIndex.search_by_label (KeyError for an unknown label),
+        which synchronises the host, with the results copied into CUDA tensors on stream_ptr.  exchange="nccl" raises
+        ValueError: it has no row exchange."""
+        if self.exchange == "nccl":
+            raise ValueError("search_by_label_dev needs the peer exchange (exchange='peer'); the NCCL path only "
+                             "exchanges result lists")
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        nq = lab.shape[0]
+        if self.world == 1:
+            # a host search (it synchronises); the results are allocated and copied on stream_ptr, so work queued
+            # there afterwards reads them in order
+            ol, od, oc = self.ix.search_by_label(lab, k, ef=ef, precision=precision)
+            t = self._torch
+            dev = t.device("cuda", self.device)
+            s = t.cuda.ExternalStream(stream_ptr, device=dev) if stream_ptr else t.cuda.current_stream(dev)
+            with t.cuda.stream(s):
+                return tuple(t.from_numpy(a).to(dev, non_blocking=False)
+                             for a in (ol.view(np.int64), od, oc.view(np.int32)))
+        b = self._bufs(nq, k)
+        self._ensure_exchange(nq, k + 1, self.ix.dim)
+        check(lib().ehb_exchange_search_by_label_ex_dev(self._ex, self.ix._h, nq, lab.ctypes.data_as(C.c_void_p), k,
+                                                        ef, int(precision), C.c_void_p(b["md"].data_ptr()),
+                                                        C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
+                                                        C.c_void_p(stream_ptr)))
         return b["ml"], b["md"], b["mc"]

@@ -329,6 +329,15 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
 typedef struct ehb_exchange ehb_exchange; /* opaque */
 int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
                         ehb_exchange** out);
+/* ehb_exchange_create is exactly this with max_dim = 0.  max_dim > 0 (at most 2048) also makes room for key-mode
+ * steps (ehb_exchange_search_by_label_ex_dev) over indexes of dim <= max_dim: in the exported block, after the
+ * receive buffer, a row region of two parts of max_nq * max_dim fp32 each (rounded up to 64 floats), a mark array [2][world][max_nq] bytes and [2][world] 64-bit
+ * digests; on this rank only, scratch for one step (the ids and labels of max_nq queries, max_nq * max_k merged
+ * entries, a verdict word) and pinned host staging.  Everything is allocated here; no step allocates or frees.
+ * Every rank creates its exchange with the same world, max_nq, max_k and max_dim (ehb_exchange_attach_local fails
+ * with EHB_ERR_INVALID when the max_dim differ). */
+int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
+                           uint32_t max_dim, ehb_exchange** out);
 int ehb_exchange_destroy(ehb_exchange* ex);
 int ehb_exchange_ipc_handle(ehb_exchange* ex, void* out_handle /* EHB_IPC_HANDLE_BYTES */);
 int ehb_exchange_open(ehb_exchange* ex, const void* handles /* [world][EHB_IPC_HANDLE_BYTES], rank order */);
@@ -354,6 +363,31 @@ int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const 
 int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
                                uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
                                uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream);
+/* Key mode (server.cc:190-207, offlinehub.py:110-130) over the exchange: every rank passes the same nq labels, each
+ * stored on exactly one rank, and every rank receives [nq][k] results.  They equal ehb_exchange_search_ex_dev(rows,
+ * k + 1, ef, precision) followed by the self-removal rule of ehb_index_search_by_label_ex, where rows[q] is label q's
+ * stored row as ehb_index_get returns it on the rank that holds it (cosine rows are normalised again, like any query).
+ * A step takes two epochs.  At the first, one kernel per rank copies the rows of the labels this rank holds (a
+ * tombstoned label is not held) from its index straight into row q of every rank's row region, writes which queries
+ * it holds and a digest of its label list into every rank, raises per-slice flags, waits for the peers' flags and
+ * counts each query's holders.  Then ONE 4-byte copy to the host and a synchronisation of `stream`: the call's only
+ * host synchronisation.  Every rank has read the same digests and, when those agree, the same marks, so every rank
+ * then returns the same status:
+ *   EHB_ERR_INVALID    the ranks were given different label lists (of any lengths);
+ *   EHB_ERR_NOT_FOUND  otherwise, some label is held by no rank (unknown or tombstoned everywhere);
+ *   EHB_ERR_STATE      otherwise, some label is held by more than one rank;
+ * and nothing is written; each rank has consumed the first epoch, so the next step still pairs with the peers'.
+ * Otherwise the fused k + 1 step runs at the second epoch with this rank's row region as its queries (the walk
+ * ehb_exchange_search_ex_dev would take for nq queries), the merge writes into the exchange's scratch, and the
+ * self-removal writes the caller's buffers, all queued on `stream` without further synchronisation.
+ * Checked before the first epoch, as in the fused step (call it on every rank, so every rank fails the same way):
+ * an unknown precision, a null pointer (all three outputs are required), max(ef, k + 1) > 512, nq > max_nq,
+ * nq * (k + 1) > max_nq * max_k and an index dim above max_dim (so an exchange created with max_dim = 0) fail with
+ * EHB_ERR_INVALID, and a call before the peers are attached with EHB_ERR_STATE.  nq == 0 or k == 0 writes nothing
+ * and does not advance the epoch.  A wait that gives up (ehb_exchange_timed_out) fails with EHB_ERR_CUDA. */
+int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                        uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                        uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream);
 int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a peer gave up (~20 s) */);
 
 /* Named integer options (A/B switches and construction knobs that are not part of
