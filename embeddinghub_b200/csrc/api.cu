@@ -88,13 +88,16 @@ int ehb_index::try_screen_copy() {
 ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16,
                                  bool dense, bool screen) const {
   ehb::WalkCfg c;
-  const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);  // bytes of a row as the walk reads it
+  const uint32_t esize = bf16 ? 2u : 4u, vbytes = dpad * esize;  // bytes of a row as the walk reads it
+  // the wide shapes keep the query in shared memory and have no ring (walk.cuh eval_wide)
+  const bool wide = ehb::wide_shape(ehb::row_lpv(vbytes), ehb::row_nq(dpad, vbytes));
   c.lcap = smem_list;
-  c.staged = ehb::row_lpv(vbytes) == 32 ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
+  c.staged = ehb::row_lpv(vbytes) == 32 && !wide ? 1 : 0;  // rows above 1 KB go through the TMA staging ring
   c.dcap = n_deleted ? ehb::kDeletedQueue : 0;
   c.prefetch = o_walk_prefetch ? 1 : 0;
   c.dense = dense ? 1 : 0;
-  const uint32_t warp_target = c.dense ? 20u : 16u;  // resident warps per SM the visited-table sizing aims at
+  // resident warps per SM the visited-table sizing aims at; the wide walk's ~220 registers allow eight
+  const uint32_t warp_target = c.dense ? 20u : (wide ? 8u : 16u);
   uint32_t nslots = std::max(4u, std::min(32u, 24576u / vbytes));
   uint32_t ng = 2;                      // two groups: math on one overlaps the copies of the other
   uint32_t g = std::max(4u, nslots / ng / 4 * 4);  // vectors per group, multiple of the 4-vector math step
@@ -117,7 +120,7 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
     uint32_t want = (uint32_t)std::min<uint64_t>((ctas + sms - 1) / sms, c.staged ? 5u : warp_target / team);
     want = std::max(want, 4u);
     c.hash_size = 0;
-    uint32_t fixed = ehb::warp_smem_bytes(c, vbytes) * team + 1024u + (smem_list ? 256u : 0u);
+    uint32_t fixed = ehb::warp_smem_bytes(c, dpad, esize) * team + 1024u + (smem_list ? 256u : 0u);
     uint32_t per_cta = (227u * 1024u) / want;
     uint32_t avail = per_cta > fixed + 1024u ? (per_cta - fixed) / 4u : 256u;
     hs = std::min(roomy, std::max(tight, avail));
@@ -125,7 +128,7 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
   }
   c.hash_size = ehb::align_up(std::max(hs, 256u), 32);
   // stay inside the 227 KB per-block limit
-  while (ehb::warp_smem_bytes(c, vbytes) + 256 > 200 * 1024 && c.hash_size > 512)
+  while (ehb::warp_smem_bytes(c, dpad, esize) + 256 > 200 * 1024 && c.hash_size > 512)
     c.hash_size = ehb::align_up(c.hash_size / 2, 32);
   // A screened walk keeps the visited table sized as above, for five staged warps per SM, so that it revisits and
   // counts exactly what the unscreened walk does; without the ring that table still leaves room for the ten warps its
@@ -136,8 +139,7 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
 
 uint32_t ehb_index::wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16) const {
   uint32_t w = t_wpb ? t_wpb : 1;
-  const uint32_t vbytes = dpad * (bf16 ? 2u : 4u);
-  while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, vbytes) + extra) * w > 220 * 1024) w >>= 1;
+  while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, dpad, bf16 ? 2u : 4u) + extra) * w > 220 * 1024) w >>= 1;
   return w;
 }
 
@@ -170,6 +172,8 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
   // dense walk (search_impl.cuh): batches big enough to fill 20 warps per SM, on the shapes that have one
   if (team > 1)
     p.form = ehb::WalkForm::team;
+  else if (ehb::wide_shape(p.lpv, p.nq))
+    p.form = ehb::WalkForm::wide;
   else if (nq >= 20ull * (uint64_t)sms && ehb::dense_form(bf16, p.lpv, p.nq, p.kpl, p.hasdel))
     p.form = ehb::WalkForm::dense;
   else
@@ -1156,7 +1160,7 @@ void ehb_params_default(ehb_params* p, uint32_t dim) {
 
 int ehb_index_create(const ehb_params* p, ehb_index** out) {
   if (!p || !out) return fail(EHB_ERR_INVALID, "null argument");
-  if (p->dim == 0 || p->dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "dim must be in 1..2048");
+  if (p->dim == 0 || p->dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "dim must be in 1..4096");
   if (p->M < 2 || p->M > 16) return fail(EHB_ERR_INVALID, "M must be in 2..16");
   if (p->ef_construction > 256) return fail(EHB_ERR_INVALID, "ef_construction must be <= 256");
   if (p->metric < 0 || p->metric > 2) return fail(EHB_ERR_INVALID, "unknown metric");

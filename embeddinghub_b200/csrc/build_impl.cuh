@@ -38,7 +38,17 @@ __device__ __forceinline__ Aux aux_of(const WarpCtx& c) {
   return a;
 }
 __host__ __device__ inline uint32_t build_warp_smem(const WalkCfg& cfg, uint32_t dpad) {
-  return 256u + warp_smem_bytes(cfg, dpad * 4u);
+  return 256u + warp_smem_bytes(cfg, dpad, 4u);
+}
+
+// The query of a build walk is a stored row: into registers, or into the warp's query slice for the wide shapes
+// (walk.cuh load_query_smem; qr is then unused).
+template <int LPV, int NQ>
+__device__ __forceinline__ void load_row_query(WarpCtx& c, float4 (&qr)[NQ], const GraphView& g, uint32_t id) {
+  if constexpr (wide_shape(LPV, NQ))
+    load_query_smem<NQ, float>(c, g.vecs + (size_t)id * g.dpad, g.dpad);
+  else
+    load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)id * g.dpad, c.lane);
 }
 
 // hnswlib getNeighborsByHeuristic2 over keys[0..cnt) (ascending distance to
@@ -62,7 +72,7 @@ __device__ __forceinline__ uint32_t heuristic_select(WarpCtx& c, const GraphView
     bool good = true;
     if (nsel > 0) {
       float4 cr[NQ];
-      load_vec_regs<LPV, NQ>(cr, g.vecs + (size_t)cid * g.dpad, c.lane);
+      load_row_query<LPV, NQ>(c, cr, g, cid);  // (the wide shapes: this replaces the caller's query)
       if (c.lane < nsel) c.cand_id[c.lane] = a.sel_id[c.lane];
       __syncwarp();
       eval_candidates<LPV, NQ>(c, g.vecs, cr, nsel, g.metric);
@@ -146,7 +156,7 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
   ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
   Aux a = aux_of(c);
   float4 qr[NQ];
-  load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)p * g.dpad, c.lane);
+  load_row_query<LPV, NQ>(c, qr, g, p);
   UList<KPL> ul;
   WalkCounters wc = {0, 0, 0, 0};
   const int level_p = bg.levels[p];
@@ -166,6 +176,8 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
     if (is_update) list_remove_id(c, p);
     if (c.cnt == 0) continue;
     uint32_t nsel = heuristic_select<LPV, NQ>(c, g, g.M, a);
+    if constexpr (wide_shape(LPV, NQ))
+      if (level > 0) load_row_query<LPV, NQ>(c, qr, g, p);  // the selection replaced the shared-memory query
     uint32_t width = level == 0 ? g.M0 : g.M;
     uint32_t* row = level == 0 ? links0 + (size_t)p * g.M0 : links_up + (size_t)(g.up_off[p] + level - 1) * g.M;
     if (is_update) {
@@ -216,7 +228,7 @@ template <int LPV, int NQ, int KPL>
 __device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g, const Aux& a, const uint32_t* cand,
                                                  uint32_t ncand, uint32_t owner, uint32_t keep, uint32_t Mmax) {
   float4 qr[NQ];
-  load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)owner * g.dpad, c.lane);
+  load_row_query<LPV, NQ>(c, qr, g, owner);
   UList<KPL> u;
   ul_clear<KPL>(u, keep, c.lane);
   uint32_t cnt = 0, worst_hi = 0xFFFFFFFFu;
@@ -446,7 +458,7 @@ __global__ void __launch_bounds__(128) merge_rows_kernel(BuildGraph bg, WalkCfg 
     }
     // row full: distances of the existing entries to the row's owner are needed once
     if (!have_dists) {
-      load_vec_regs<LPV, NQ>(qr, g.vecs + (size_t)node * g.dpad, c.lane);
+      load_row_query<LPV, NQ>(c, qr, g, node);
       if (c.lane < ne) c.cand_id[c.lane] = e;
       __syncwarp();
       eval_candidates<LPV, NQ>(c, g.vecs, qr, ne, g.metric);

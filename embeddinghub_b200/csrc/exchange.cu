@@ -242,7 +242,7 @@ int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64
   if (!out) return fail(EHB_ERR_INVALID, "null argument");
   if (world == 0 || world > ehb::kMaxWorld || rank >= world) return fail(EHB_ERR_INVALID, "bad world / rank");
   if (max_nq == 0 || max_k == 0) return fail(EHB_ERR_INVALID, "max_nq and max_k must be positive");
-  if (max_dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "max_dim must be <= 2048");
+  if (max_dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "max_dim must be <= 4096");
   CU(cudaSetDevice(device));
   ehb_exchange* ex = new (std::nothrow) ehb_exchange();
   if (!ex) return fail(EHB_ERR_OOM, "host allocation failed");

@@ -7,7 +7,7 @@
 
 namespace ehb {
 
-constexpr uint32_t kMaxDim = 2048;  // pad_dim() supports rows up to 2048 floats
+constexpr uint32_t kMaxDim = 4096;  // pad_dim() supports rows up to 4096 floats
 constexpr uint32_t kMaxEf = 512;    // register-resident list: 16 keys per lane
 constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved point, >= 1 + 32 + 32*32
 constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
@@ -20,7 +20,8 @@ constexpr bool dense_form(bool bf16, int LPV, int NQ, int KPL, bool HASDEL) {
 
 // Which graph-walk kernel a search runs and how it is launched (ehb_index::walk_plan).  The launchers and the
 // reported kernel name read it and decide nothing themselves.
-enum class WalkForm { plain, dense, team };
+// wide: the form of the wide shapes (walk.cuh wide_shape, dpad 3072 and 4096), and their only one.
+enum class WalkForm { plain, dense, team, wide };
 struct WalkPlan {
   bool bf16;           // the walk reads the bf16 shadow g.vecs16 (else the fp32 rows)
   int lpv, nq, kpl;    // row shape (walk.cuh row_lpv / row_nq) and result-set entries per lane (kpl_for)
@@ -35,7 +36,7 @@ struct WalkPlan {
 // the name of the kernel the plan launches, e.g. hnsw_search_kernel<LPV=32,NQ=6,KPL=4>
 void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes);
 
-// K2 — batched k-NN graph walk (hnswlib searchKnn), one warp per query, plain or dense form.  ef >= k.
+// K2 — batched k-NN graph walk (hnswlib searchKnn), one warp per query, plain, dense or wide form.  ef >= k.
 // stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.codes8
 // set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the int8 screen copy (walk.cuh beam_search).
 // With p.bf16 the walk reads the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation) and writes the retained

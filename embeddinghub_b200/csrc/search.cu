@@ -26,8 +26,10 @@ void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes) {
     std::snprintf(out, out_bytes, "hnsw_search_team_kernel<NQ=%d,KPL=%d,T=%u,U=%u>", p.nq, p.kpl, p.T, p.U);
   else
     std::snprintf(out, out_bytes, "%s<LPV=%d,NQ=%d,KPL=%d%s%s>",
-                  p.form == WalkForm::dense ? "hnsw_search_dense_kernel" : "hnsw_search_kernel", p.lpv, p.nq, p.kpl,
-                  p.hasdel ? ",HASDEL=1" : "", p.bf16 ? ",ROW=bf16" : "");
+                  p.form == WalkForm::dense  ? "hnsw_search_dense_kernel"
+                  : p.form == WalkForm::wide ? "hnsw_search_wide_kernel"
+                                             : "hnsw_search_kernel",
+                  p.lpv, p.nq, p.kpl, p.hasdel ? ",HASDEL=1" : "", p.bf16 ? ",ROW=bf16" : "");
 }
 
 // ---------------------------------------------------------------------------

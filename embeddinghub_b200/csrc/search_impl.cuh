@@ -19,8 +19,11 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   constexpr bool kScreen = !kKeys && screen_shape(LPV, NQ);  // can run a screened plan (no ring)
   WarpCtx c;
   ctx_init(c, smem + (size_t)w * warp_smem, cfg, g.dpad, (uint32_t)sizeof(RowT));
-  float4 qr[NQ];
-  load_query_regs<LPV, NQ, RowT>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
+  float4 qr[NQ];  // (unused by the wide shapes: their query is in shared memory)
+  if constexpr (wide_shape(LPV, NQ))
+    load_query_smem<NQ, RowT>(c, queries + (size_t)q * g.dim, g.dim);
+  else
+    load_query_regs<LPV, NQ, RowT>(qr, queries + (size_t)q * g.dim, g.dim, c.lane);
   WalkCounters wc = {0, 0, 0, 0};
   UList<KPL> ul;
   ul_clear<KPL>(ul, ef, c.lane);
@@ -121,21 +124,39 @@ __global__ void __launch_bounds__(128, 5) hnsw_search_dense_kernel(GraphView g, 
   search_body<LPV, NQ, KPL, false, 2, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
 }
 
+// The one-warp walk over wide rows (dpad 3072, 4096; walk.cuh eval_wide), fp32 rows or the bf16 shadow.  Shared
+// memory, not registers, sets its occupancy (the query slice and the visited table: api.cu walk_cfg aims at eight
+// warps per SM, which leave ptxas the full 255 registers; over bf16 rows minBlocksPerSM = 1 again keeps it from
+// spilling).
+template <int NQ, int KPL, bool HASDEL, class RowT>
+__global__ void __launch_bounds__(128, (kWalkMinBlocks<RowT>))
+    hnsw_search_wide_kernel(GraphView g, WalkCfg cfg, const float* __restrict__ queries, uint32_t nq, uint32_t k,
+                            uint32_t ef, const __grid_constant__ ResultSink sink, uint32_t* __restrict__ out_counts,
+                            uint32_t* __restrict__ stats, uint32_t warp_smem) {
+  search_body<32, NQ, KPL, HASDEL, 1, RowT>(g, cfg, queries, nq, k, ef, sink, out_counts, stats, warp_smem);
+}
+
 using WalkKernel = void (*)(GraphView, WalkCfg, const float*, uint32_t, uint32_t, uint32_t, const ResultSink,
                            uint32_t*, uint32_t*, uint32_t);
-// the kernel the plan launches (nullptr: the plan asks for a dense form the shape does not have)
+// the kernel the plan launches (nullptr: the plan asks for a form the shape does not have)
 template <int LPV, int NQ, int KPL, class RowT>
 WalkKernel walk_kernel(const WalkPlan& p) {
   constexpr bool kBf16 = !std::is_same<RowT, float>::value;
-  if (p.form == WalkForm::dense) {
-    if constexpr (dense_form(kBf16, LPV, NQ, KPL, false))
-      if (!p.hasdel) return hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
-    return nullptr;
+  if constexpr (wide_shape(LPV, NQ)) {
+    if (p.form != WalkForm::wide) return nullptr;
+    return p.hasdel ? hnsw_search_wide_kernel<NQ, KPL, true, RowT> : hnsw_search_wide_kernel<NQ, KPL, false, RowT>;
+  } else {
+    if (p.form == WalkForm::wide) return nullptr;
+    if (p.form == WalkForm::dense) {
+      if constexpr (dense_form(kBf16, LPV, NQ, KPL, false))
+        if (!p.hasdel) return hnsw_search_dense_kernel<LPV, NQ, KPL, RowT>;
+      return nullptr;
+    }
+    if constexpr (std::is_same<RowT, float>::value && screen_shape(LPV, NQ))
+      return p.hasdel ? hnsw_search_screen_kernel<LPV, NQ, KPL, true> : hnsw_search_screen_kernel<LPV, NQ, KPL, false>;
+    else
+      return p.hasdel ? hnsw_search_kernel<LPV, NQ, KPL, true, RowT> : hnsw_search_kernel<LPV, NQ, KPL, false, RowT>;
   }
-  if constexpr (std::is_same<RowT, float>::value && screen_shape(LPV, NQ))
-    return p.hasdel ? hnsw_search_screen_kernel<LPV, NQ, KPL, true> : hnsw_search_screen_kernel<LPV, NQ, KPL, false>;
-  else
-    return p.hasdel ? hnsw_search_kernel<LPV, NQ, KPL, true, RowT> : hnsw_search_kernel<LPV, NQ, KPL, false, RowT>;
 }
 
 template <int LPV, int NQ, int KPL, class RowT>
@@ -143,7 +164,7 @@ cudaError_t launch_search_t(const WalkPlan& p, const GraphView& g, const float* 
                             uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                             cudaStream_t s) {
   const uint32_t wpb = p.wpb;
-  uint32_t wsm = warp_smem_bytes(p.cfg, g.dpad * (uint32_t)sizeof(RowT));
+  uint32_t wsm = warp_smem_bytes(p.cfg, g.dpad, (uint32_t)sizeof(RowT));
   size_t smem = (size_t)wsm * wpb;
   dim3 grid((nq + wpb - 1) / wpb), block(32 * wpb);
   const WalkKernel kern = walk_kernel<LPV, NQ, KPL, RowT>(p);

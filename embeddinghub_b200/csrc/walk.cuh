@@ -23,7 +23,9 @@
 //     loops carry no bounds checks;
 //   * the walk reads either the fp32 rows or their bf16 shadow (RowT = __nv_bfloat16: the bf16 graph
 //     search, re-ranked in fp32 afterwards).  The query stays fp32 in registers either way and the same
-//     "rows <= 1 KB direct, larger rows TMA" rule applies to the row's bytes.
+//     "rows <= 1 KB direct, larger rows TMA" rule applies to the row's bytes;
+//   * rows wider than 2048 floats (dpad 3072, 4096: the wide form, eval_wide) keep the fp32 query in the
+//     warp's shared-memory slice instead and read the rows straight into registers in d-slices.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -113,13 +115,15 @@ __host__ __device__ inline uint32_t align_up(uint32_t x, uint32_t a) { return (x
 // The padded row lengths (floats) the walk supports, ascending.  A row of `row_bytes` as the walk reads it
 // (dpad * 4 for fp32 rows, dpad * 2 for the bf16 shadow) is loaded directly by LPV = 8 lanes per vector up to
 // 1 KB, and staged through the TMA ring and read by LPV = 32 lanes above; a lane holds NQ float4 chunks of the
-// fp32 query (dpad == 4 * LPV * NQ).
-constexpr uint32_t kPadDims[] = {32, 64, 128, 256, 384, 512, 768, 1024, 1536, 2048};
+// fp32 query (dpad == 4 * LPV * NQ).  The wide shapes (wide_shape: dpad 3072 and 4096, NQ 24 and 32) hold those
+// chunks in shared memory instead, and have no ring (eval_wide).
+constexpr uint32_t kPadDims[] = {32, 64, 128, 256, 384, 512, 768, 1024, 1536, 2048, 3072, 4096};
 constexpr uint32_t kNumPadDims = sizeof(kPadDims) / sizeof(kPadDims[0]);
 __host__ __device__ constexpr int row_lpv(uint32_t row_bytes) { return row_bytes > 1024 ? 32 : 8; }
 __host__ __device__ constexpr int row_nq(uint32_t dpad, uint32_t row_bytes) {
   return (int)(dpad / (4u * (uint32_t)row_lpv(row_bytes)));
 }
+__host__ __device__ constexpr bool wide_shape(int LPV, int NQ) { return LPV == 32 && NQ > 16; }
 // register-resident result set entries per lane for a beam of ef (<= 512)
 constexpr int kpl_for(uint32_t ef) { return ef <= 64 ? 2 : (ef <= 128 ? 4 : (ef <= 256 ? 8 : 16)); }
 
@@ -131,7 +135,7 @@ inline uint32_t pad_dim(uint32_t dim) {
 
 // Calls f(std::integral_constant<uint32_t, DPAD>{}) for the padded row length DPAD == dpad; any other dpad, or one
 // above MaxDpad, is cudaErrorInvalidValue.
-template <uint32_t MaxDpad = 2048, uint32_t I = 0, class F>
+template <uint32_t MaxDpad = 4096, uint32_t I = 0, class F>
 cudaError_t with_dpad(uint32_t dpad, F&& f) {
   if constexpr (I == kNumPadDims || kPadDims[I] > MaxDpad)
     return cudaErrorInvalidValue;
@@ -143,10 +147,13 @@ cudaError_t with_dpad(uint32_t dpad, F&& f) {
 // The fp32 walk's screen applies to staged fp32 rows of dpad 384 .. 1536 (dpad 2048: DESIGN.md §9).
 __host__ __device__ constexpr bool screen_shape(int LPV, int NQ) { return LPV == 32 && NQ <= 12; }
 
-// Per-warp shared-memory slice; every region offset is a multiple of 128 B.  vbytes: bytes of one row as the
-// walk reads it (dpad * 4 for fp32 rows, dpad * 2 for the bf16 shadow); it sizes the TMA staging ring.
-__host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t vbytes) {
+// Per-warp shared-memory slice; every region offset is a multiple of 128 B.  esize: bytes per row element as the
+// walk reads it (4 for fp32 rows, 2 for the bf16 shadow); dpad * esize sizes the TMA staging ring.  The wide shapes
+// have the fp32 query (dpad * 4 bytes) where the ring would be.
+__host__ __device__ inline uint32_t warp_smem_bytes(const WalkCfg& c, uint32_t dpad, uint32_t esize) {
+  const uint32_t vbytes = dpad * esize;
   uint32_t b = 0;
+  if (wide_shape(row_lpv(vbytes), row_nq(dpad, vbytes))) b += dpad * 4u;
   b += align_up(c.lcap * 8u, 128);
   b += align_up(c.hash_size * 4u, 128);
   b += 128;  // cand_id[32]
@@ -477,12 +484,116 @@ __device__ __forceinline__ void eval_regs(WarpCtx& c, const float* __restrict__ 
   __syncwarp();
 }
 
-// cand_id[0..m) -> cand_dist[0..m): distances from the register-held query.  UDIV > 1 halves (…) the
+// ---- Wide rows (dpad 3072, 4096): the query in shared memory ---------------------------------------------
+// 24 or 32 float4 of query per lane beside a row's chunks leave no registers (a register query spills kilobytes at
+// dpad 4096), and a TMA ring of 12 or 16 KB rows would leave one warp per SM.  The wide form keeps the fp32 query in
+// the warp's shared-memory slice where the ring would be (c.stage, dpad * 4 bytes), in the register layout of
+// load_query_regs: float4 t of lane l at stage[32 t + l], so that the warp's 128-bit reads are free of bank
+// conflicts.  The query of a walk, or a stored row that the build uses as one (first element past dim: dpad).
+template <int NQ, class RowT>
+__device__ __forceinline__ void load_query_smem(WarpCtx& c, const float* __restrict__ src, uint32_t dim) {
+  constexpr int V = LaneChunks<RowT, NQ>::V;
+  float4* qs = (float4*)c.stage + c.lane;
+  __syncwarp();  // the previous query's readers are done
+#pragma unroll 4
+  for (int t = 0; t < NQ; ++t) {
+    const uint32_t e = (c.lane + 32u * (t / V)) * 4u * V + 4u * (t % V);  // load_query_regs' element of (lane, t)
+    float4 v;
+    v.x = e + 0 < dim ? src[e + 0] : 0.f;
+    v.y = e + 1 < dim ? src[e + 1] : 0.f;
+    v.z = e + 2 < dim ? src[e + 2] : 0.f;
+    v.w = e + 3 < dim ? src[e + 3] : 0.f;
+    qs[32 * t] = v;
+  }
+  __syncwarp();
+}
+// cand_id[0..m) -> cand_dist[0..m) from the shared-memory query.  Per batch of kWideRows candidates a lane reads its
+// chunks (lane l: chunks l, l + 32, ..., as eval_staged) straight into registers one d-slice of 1024 elements at a
+// time (32 values per lane: 8 fp32 chunks or 4 bf16 ones, 64 load registers per lane for the batch), and folds each
+// d-slice into the four accumulators of partial_dist in ascending chunk order, with the query slice read once from
+// shared memory for all the batch's rows.  (a0 + a1) + (a2 + a3) and the shuffle tree of eval_staged follow, so the
+// distances have the bits of the register-query walk's chain.  Loading the next d-slice during this one's math would
+// double the load registers (ptxas then spills); the other resident warps overlap the round trips instead.
+constexpr int kWideRows = 4;
+template <int NQ, class RowT>
+__device__ __forceinline__ void eval_wide(WarpCtx& c, const RowT* __restrict__ vecs, uint32_t m, int metric) {
+  using C = LaneChunks<RowT, NQ>;
+  constexpr int V = C::V, SB = kWideRows, NS = 8 / V;
+  static_assert(C::N % NS == 0, "the d-slices tile the row");
+  const float4* qs = (const float4*)c.stage + c.lane;
+#pragma unroll 1
+  for (uint32_t v0 = 0; v0 < m; v0 += SB) {
+    const typename C::T* p[SB];
+#pragma unroll
+    for (int i = 0; i < SB; ++i)  // clamped repeats are discarded below
+      p[i] = (const typename C::T*)(vecs + (size_t)c.cand_id[min(v0 + (uint32_t)i, m - 1u)] * c.dpad) + c.lane;
+    float a[SB][4];
+#pragma unroll
+    for (int i = 0; i < SB; ++i) a[i][0] = a[i][1] = a[i][2] = a[i][3] = 0.f;
+#pragma unroll 1
+    for (int j0 = 0; j0 < C::N; j0 += NS) {
+      typename C::T x[SB][NS];
+#pragma unroll
+      for (int i = 0; i < SB; ++i)
+#pragma unroll
+        for (int j = 0; j < NS; ++j) x[i][j] = ld_chunk(p[i] + 32 * (j0 + j));
+#pragma unroll
+      for (int j = 0; j < NS; ++j) {
+        float4 q[V];
+#pragma unroll
+        for (int v = 0; v < V; ++v) q[v] = qs[32 * ((j0 + j) * V + v)];
+#pragma unroll
+        for (int i = 0; i < SB; ++i) {
+          float4 r[V];
+          widen(x[i][j], r);
+#pragma unroll
+          for (int v = 0; v < V; ++v) {
+            if (metric == 0) {
+              const float dx = q[v].x - r[v].x, dy = q[v].y - r[v].y, dz = q[v].z - r[v].z, dw = q[v].w - r[v].w;
+              a[i][0] = fmaf(dx, dx, a[i][0]);
+              a[i][1] = fmaf(dy, dy, a[i][1]);
+              a[i][2] = fmaf(dz, dz, a[i][2]);
+              a[i][3] = fmaf(dw, dw, a[i][3]);
+            } else {
+              a[i][0] = fmaf(q[v].x, r[v].x, a[i][0]);
+              a[i][1] = fmaf(q[v].y, r[v].y, a[i][1]);
+              a[i][2] = fmaf(q[v].z, r[v].z, a[i][2]);
+              a[i][3] = fmaf(q[v].w, r[v].w, a[i][3]);
+            }
+          }
+        }
+      }
+    }
+    float acc[SB];
+#pragma unroll
+    for (int i = 0; i < SB; ++i) acc[i] = (a[i][0] + a[i][1]) + (a[i][2] + a[i][3]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+      for (int i = 0; i < SB; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+    }
+    if (c.lane < (uint32_t)SB && v0 + c.lane < m) {
+      float d = acc[0];
+#pragma unroll
+      for (int i = 1; i < SB; ++i)
+        if (c.lane == (uint32_t)i) d = acc[i];
+      c.cand_dist[v0 + c.lane] = metric == 0 ? d : 1.0f - d;
+    }
+  }
+  __syncwarp();
+}
+
+// cand_id[0..m) -> cand_dist[0..m): distances from the register-held query (the wide shapes: from the shared-memory
+// query, eval_wide; qr is then unused).  UDIV > 1 halves (…) the
 // load batches kept in flight per warp: fewer registers, more resident warps (the "dense" walk).  SCREEN: the
 // instantiation can run a screened plan, which has no ring (c.staged == 0) and reads its rows into registers.
 template <int LPV, int NQ, int UDIV = 1, class RowT = float, bool SCREEN = false>
 __device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restrict__ vecs, const float4 (&qr)[NQ],
                                                 uint32_t m, int metric) {
+  if constexpr (wide_shape(LPV, NQ)) {
+    eval_wide<NQ, RowT>(c, vecs, m, metric);
+    return;
+  }
   if (LPV == 8) {
     eval_direct<NQ, eval_u(LaneChunks<RowT, NQ>::N, UDIV)>(c, vecs, qr, m, metric);
   } else {

@@ -62,7 +62,7 @@ typedef struct ehb_index ehb_index; /* opaque */
  * (index.cc:14-15: M=16, ef_construction=200, random_seed=100; ef=10 because the
  * reference never calls setEf; init capacity 128, index.h:21). */
 typedef struct ehb_params {
-  uint32_t dim;
+  uint32_t dim;             /* 1..4096 (ehb_index_create: EHB_ERR_INVALID above)  */
   int32_t metric;           /* ehb_metric                                      */
   uint64_t capacity;        /* initial capacity in vectors; grows by doubling  */
   uint32_t M;               /* 2..16 (level-0 rows hold 2*M ids)               */
@@ -108,7 +108,8 @@ void ehb_params_default(ehb_params* p, uint32_t dim);
 int ehb_device_count(int32_t* out);
 
 /* ANNIndex::ANNIndex(dims, init_cap) — index.cc:10-18 (allocates the hnswlib
- * arena); here: device arrays for vectors, labels, levels and adjacency. */
+ * arena); here: device arrays for vectors, labels, levels and adjacency.  dim 1..4096: rows are padded to
+ * 32 ... 2048, 3072 or 4096 floats; above 2048 the graph walk and build run their wide form (DESIGN.md §4). */
 int ehb_index_create(const ehb_params* p, ehb_index** out);
 int ehb_index_destroy(ehb_index* ix);
 
@@ -329,7 +330,7 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
 typedef struct ehb_exchange ehb_exchange; /* opaque */
 int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
                         ehb_exchange** out);
-/* ehb_exchange_create is exactly this with max_dim = 0.  max_dim > 0 (at most 2048) also makes room for key-mode
+/* ehb_exchange_create is exactly this with max_dim = 0.  max_dim > 0 (at most 4096) also makes room for key-mode
  * steps (ehb_exchange_search_by_label_ex_dev) over indexes of dim <= max_dim: in the exported block, after the
  * receive buffer, a row region of two parts of max_nq * max_dim fp32 each (rounded up to 64 floats), a mark array [2][world][max_nq] bytes and [2][world] 64-bit
  * digests; on this rank only, scratch for one step (the ids and labels of max_nq queries, max_nq * max_k merged
