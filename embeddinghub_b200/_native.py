@@ -88,6 +88,9 @@ SYMBOLS = {
     "ehb_index_get_batch": (C.c_int, [_VP, _U64, _VP, _VP]),
     "ehb_index_search_by_label_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_index_search_bruteforce_by_label": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_index_search_beam": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_index_search_beam_dev": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP]),
+    "ehb_index_search_by_label_beam": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_index_neighbor_table": (C.c_int, [_VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, C.POINTER(_U64)]),
     "ehb_index_stats": (C.c_int, [_VP, C.POINTER(Stats)]),
     "ehb_index_screen_stats": (C.c_int, [_VP, C.POINTER(_U64), C.POINTER(_U64)]),
@@ -273,6 +276,31 @@ class NativeIndex:
         check(lib().ehb_index_search_ex(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
                                         _p(counts)))
         return labels, dists, counts
+
+    def search_beam(self, q, k, ef=0, precision=FP32):
+        """search() with max(ef, k) up to EHB_MAX_BEAM = 4096: above 512 the wide-beam walk, which keeps hnswlib's
+        order and stop rule (ehb_index_search_beam); up to 512 exactly search()."""
+        q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
+        labels, dists, counts = _alloc(q.shape[0], k)
+        check(lib().ehb_index_search_beam(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
+                                          _p(counts)))
+        return labels, dists, counts
+
+    def search_beam_dev(self, q_ptr, nq, k, ef, labels_ptr, dists_ptr, counts_ptr, stream=0, precision=FP32):
+        """search_dev() with max(ef, k) up to 4096 (ehb_index_search_beam_dev)."""
+        check(lib().ehb_index_search_beam_dev(self._h, nq, C.c_void_p(q_ptr), k, ef, int(precision),
+                                              C.c_void_p(labels_ptr),
+                                              C.c_void_p(dists_ptr) if dists_ptr else None,
+                                              C.c_void_p(counts_ptr) if counts_ptr else None,
+                                              C.c_void_p(stream) if stream else None))
+
+    def search_by_label_beam(self, labels, k, ef=0, precision=FP32):
+        """search_by_label() with max(ef, k + 1) up to 4096 (ehb_index_search_by_label_beam)."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out_l, out_d, out_c = _alloc(lab.shape[0], k)
+        _check_key(lib().ehb_index_search_by_label_beam(self._h, lab.shape[0], _p(lab), k, ef, int(precision),
+                                                        _p(out_l), _p(out_d), _p(out_c)), labels)
+        return out_l, out_d, out_c
 
     def search_bruteforce(self, q, k, precision=FP32):
         q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)

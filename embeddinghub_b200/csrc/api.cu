@@ -21,6 +21,7 @@ ehb_index::~ehb_index() {
   slots.clear();
   if (bf_ev0) cudaEventDestroy(bf_ev0);
   if (bf_ev1) cudaEventDestroy(bf_ev1);
+  if (beam_done) cudaEventDestroy(beam_done);
   if (stream) cudaStreamDestroy(stream);
 }
 
@@ -159,6 +160,22 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
   // online batches, where one warp's serial chain of memory round trips is the bound), two while 7 CTAs of 64
   // threads do (C2, Q=1000), else one warp per query: once the batch alone fills the SMs, the team walk's
   // speculative expansions only add work (C5 shape, Q=10k).
+  if (ef_eff > ehb::kMaxEf) {  // the wide-beam walk: result set in shared memory, visited table in HBM
+    p.kpl = 0;
+    p.hasdel = n_deleted != 0;
+    p.T = 1;
+    p.U = 0;
+    p.form = ehb::WalkForm::beam;
+    p.screen = false;
+    p.cfg = walk_cfg(ef_eff, ehb::align_up(ef_eff, 32), nq, 1, bf16);
+    p.cfg.hash_size = 0;
+    // tombstoned candidates wait in the side queue; a wider beam keeps proportionally more of them pending
+    if (n_deleted) p.cfg.dcap = std::max(ehb::kDeletedQueue, ehb::align_up(ef_eff / 4, 32));
+    p.vtab = ehb::align_up(2u * M0 * ef_eff + 64u, 32);  // walk_cfg's "roomy" table
+    p.wpb = 1;
+    return p;
+  }
+  p.vtab = 0;
   uint32_t team = t_team;
   if (team == 0) team = nq <= (uint64_t)sms * 3 ? 4 : (nq <= (uint64_t)sms * 7 ? 2 : 1);
   if (dpad > 256 || ef_eff > 256 || n_deleted) team = 1;  // tombstones: the one-warp walk carries the side queue
@@ -785,7 +802,7 @@ ehb::SlotLease::~SlotLease() {
 
 // ---- search --------------------------------------------------------------------------------------------
 int ehb::check_request(const ehb_index* ix, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
-                       uint64_t k_walk, uint32_t* ef, bool* none) {
+                       uint64_t k_walk, uint32_t* ef, bool* none, uint32_t max_beam) {
   *none = false;
   if (precision != EHB_FP32 && precision != EHB_BF16) return fail(EHB_ERR_INVALID, "unknown precision");
   if (null_buf) return fail(EHB_ERR_INVALID, "null buffer");
@@ -797,8 +814,8 @@ int ehb::check_request(const ehb_index* ix, bool brute, int precision, bool null
       return fail(EHB_ERR_INVALID, "bf16 brute force needs dim > 32 (64-wide k-blocks)");
   } else {
     if (*ef == 0) *ef = ix->ef;
-    if (std::max<uint64_t>(*ef, k_walk) > ehb::kMaxEf)
-      return fail(EHB_ERR_INVALID, "max(ef, k) (k + 1 by label) must be <= 512");
+    if (std::max<uint64_t>(*ef, k_walk) > max_beam)
+      return fail(EHB_ERR_INVALID, "max(ef, k) (k + 1 by label) must be <= " + std::to_string(max_beam));
   }
   return EHB_OK;
 }
@@ -819,6 +836,18 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   const bool bf16 = precision == EHB_BF16;
   if (bf16 && !shadow) return fail(EHB_ERR_STATE, "bf16 shadow missing");
   const ehb::WalkPlan plan = walk_plan(nq, ef_eff, bf16);
+  const bool beam = plan.form == ehb::WalkForm::beam;
+  // the wide-beam walk's scratch: after the previous wide-beam search on the device, allocated before anything runs
+  std::unique_lock<std::mutex> bl(beam_mu, std::defer_lock);
+  uint32_t warps = 0;
+  if (beam) {
+    bl.lock();
+    if (!beam_done) CU(cudaEventCreateWithFlags(&beam_done, cudaEventDisableTiming));
+    CU(cudaStreamWaitEvent(s, beam_done, 0));
+    CU(ehb::beam_warps(plan, view(), sms, nq, &warps));
+    CU(beam_vtab.grow((size_t)warps * plan.vtab, 0, -1, s));
+    if (bf16) CU(beam_keys.grow(nq * ef_eff, 0, -1, s));
+  }
   // the team walk writes destination 0 only (a bf16 search never plans one: its re-rank stores to every destination)
   if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team;
   const float* q = dq;
@@ -831,7 +860,7 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   CU(sl->stat_sum.grow(ehb::kStatWords, 0, 0, s));
   if (bf16) {
     CU(sl->q_pad.grow(nq * dpad, 0, -1, s));
-    CU(sl->walk_keys.grow(nq * ef_eff, 0, -1, s));
+    if (!beam) CU(sl->walk_keys.grow(nq * ef_eff, 0, -1, s));
     CU(sl->walk_counts.grow(nq, 0, -1, s));
     CU(ehb::launch_pad_rows(dq, sl->q_pad.p, nq, dim, dpad, metric == EHB_COSINE, s));
   }
@@ -841,15 +870,19 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
     // sink, the re-rank stores into every destination and raises the slice flags, as the fp32 walk's epilogue does)
     ehb::ResultSink ks;
     std::memset(&ks, 0, sizeof(ks));
-    ks.keys = sl->walk_keys.p;
+    ks.keys = beam ? beam_keys.p : sl->walk_keys.p;
     ehb::GraphView g = view();
     g.vecs16 = (const __nv_bfloat16*)x_bf16.p;
-    CU(ehb::launch_search(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, s));
+    if (beam)
+      CU(ehb::launch_search_beam(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p,
+                                 beam_vtab.p, warps, s));
+    else
+      CU(ehb::launch_search(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, s));
     if (sink)
-      CU(ehb::launch_rerank_sink(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
+      CU(ehb::launch_rerank_sink(ks.keys, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
                                  labels.p, nq, k, *sink, dc, s));
     else
-      CU(ehb::launch_rerank(sl->walk_keys.p, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
+      CU(ehb::launch_rerank(ks.keys, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
                             labels.p, nq, k, dl, dd, dc, s));
   } else if (plan.form == ehb::WalkForm::team) {
     CU(ehb::launch_search_team(plan, view(), q, (uint32_t)nq, k, ef_eff, dl, dd, dc, sl->stats.p, s));
@@ -867,8 +900,12 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
       g.codes8 = x_i8.p;
       g.terms8 = x_i8t.p;
     }
-    CU(ehb::launch_search(plan, g, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, s));
+    if (beam)
+      CU(ehb::launch_search_beam(plan, g, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, beam_vtab.p, warps, s));
+    else
+      CU(ehb::launch_search(plan, g, q, (uint32_t)nq, k, ef_eff, *sink, dc, sl->stats.p, s));
   }
+  if (beam) CU(cudaEventRecord(beam_done, s));
   CU(cudaEventRecord(sl->ev1, s));
   sl->last_nq = nq;
   sl->last_bf16 = bf16;
@@ -1063,17 +1100,18 @@ int gather_ids(ehb_index* ix, ehb::SearchSlot* sl, const std::vector<uint32_t>& 
 // every other call stages, searches and copies out on one leased slot with one synchronisation.
 int search_host(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, bool brute, bool by_label, uint64_t nq,
                 const float* q, const uint64_t* labels, uint32_t k, uint32_t ef, int precision, uint64_t* ol, float* od,
-                uint32_t* oc) {
+                uint32_t* oc, uint32_t max_beam = ehb::kMaxEf) {
   const uint64_t k_walk = k + (uint64_t)by_label;
   const bool null_q = by_label ? !labels : !q;
   bool none;
-  RET(ehb::check_request(ix, brute, precision, nq && (null_q || !ol), nq, k, k_walk, brute ? nullptr : &ef, &none));
+  RET(ehb::check_request(ix, brute, precision, nq && (null_q || !ol), nq, k, k_walk, brute ? nullptr : &ef, &none,
+                         max_beam));
   if (none) return EHB_OK;
-  const uint32_t kw = (uint32_t)k_walk;  // checked: <= 2048
+  const uint32_t kw = (uint32_t)k_walk;  // checked: <= 4096
   // before queueing or bf_mu: a waiting follower must never block a writer the leader needs, and the upgrade waits
   // for the other readers
   RET(ix->prepare(lk, brute, precision, nq));
-  if (!brute && !by_label && ix->o_combine && nq <= ehb::kCombineMaxCall)
+  if (!brute && !by_label && ix->o_combine && nq <= ehb::kCombineMaxCall && std::max(ef, kw) <= ehb::kMaxEf)
     return search_host_combined(ix, nq, q, k, ef, precision, ol, od, oc);
   std::vector<uint32_t> ids;
   if (by_label) RET(resolve_labels(ix, nq, labels, ids));
@@ -1404,6 +1442,30 @@ int ehb_index_search_ex_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_
 int ehb_index_search_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, uint64_t* dl, float* dd,
                          uint32_t* dc, void* stream) {
   return ehb_index_search_ex_dev(ix, nq, dq, k, ef, EHB_FP32, dl, dd, dc, stream);
+}
+
+// The wide-beam entry points: the _ex calls with the width limit raised to EHB_MAX_BEAM.  Up to 512 they run exactly
+// what the _ex calls run; above, walk_plan picks the wide-beam walk, which never goes through the combining queue.
+int ehb_index_search_beam(ehb_index* ix, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                          uint64_t* ol, float* od, uint32_t* oc) {
+  ENTER_S(ix);
+  return search_host(ix, _g, false, false, nq, q, nullptr, k, ef, precision, ol, od, oc, ehb::kMaxBeam);
+}
+int ehb_index_search_by_label_beam(ehb_index* ix, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                                   int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  ENTER_S(ix);
+  return search_host(ix, _g, false, true, nq, nullptr, labels, k, ef, precision, ol, od, oc, ehb::kMaxBeam);
+}
+int ehb_index_search_beam_dev(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
+                              uint64_t* dl, float* dd, uint32_t* dc, void* stream) {
+  ENTER_S(ix);
+  bool none;
+  RET(ehb::check_request(ix, false, precision, nq && (!dq || !dl), nq, k, k, &ef, &none, ehb::kMaxBeam));
+  if (none) return EHB_OK;
+  RET(ix->prepare(_g, false, precision, nq));
+  ehb::SlotLease ls(ix);
+  RET(ls.take((cudaStream_t)stream));
+  return ix->search_dev(ls.sl, nq, dq, k, ef, dl, dd, dc, ls.s, nullptr, nullptr, precision);
 }
 
 }  // extern "C"

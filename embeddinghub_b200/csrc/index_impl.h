@@ -198,18 +198,19 @@ constexpr uint32_t kCombineMaxBatch = 8192;
 constexpr uint32_t kCombineLeaders = 2;    // batches in flight (copies of one overlap the walk of the other)
 constexpr uint32_t kDeletedQueue = 64;     // side queue of tombstoned candidates per walking warp
 constexpr uint32_t kScreenMinBatchPerSm = 4;  // default fp32 walk screen: batches of >= 4 queries per SM
+static_assert(EHB_MAX_BEAM == kMaxBeam, "the header's beam limit is the wide-beam walk's");
 
 class SlotLease;
 
 // The checks every search entry point makes before it touches the index, in this order: the precision, the buffers
 // (null_buf: the entry point found a pointer it needs null), then k == 0 or nq == 0, which sets *none (the call does
-// nothing and returns EHB_OK), then the width: max(*ef, k_walk) <= 512 for the graph walk; k_walk <= 2048 and, at bf16,
-// a dim padded to whole 64-wide blocks for the brute force.  k_walk is k + 1 for the by-label searches, k otherwise.
+// nothing and returns EHB_OK), then the width: max(*ef, k_walk) <= max_beam for the graph walk (512, or kMaxBeam on the
+// wide-beam entry points); k_walk <= 2048 and, at bf16, a dim padded to whole 64-wide blocks for the brute force.  k_walk is k + 1 for the by-label searches, k otherwise.
 // ef (graph walk; nullptr for the brute force): in, the requested beam, 0 for the index default; out, the beam that was
 // checked, which the search must use: the default can change while ensure_built drops the lock.  Caller holds the
 // reader side of ix->rw.
 int check_request(const ehb_index* ix, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
-                  uint64_t k_walk, uint32_t* ef, bool* none);
+                  uint64_t k_walk, uint32_t* ef, bool* none, uint32_t max_beam = kMaxEf);
 // Queues the copies of nq result rows of k to the host on s: labels, and dists / counts where the host asked for them.
 int copy_results(uint64_t nq, uint32_t k, const uint64_t* dl, const float* dd, const uint32_t* dc, uint64_t* ol,
                  float* od, uint32_t* oc, cudaStream_t s);
@@ -289,6 +290,13 @@ struct ehb_index {
   ehb::DevBuf<float> q_norm2, bf_thr;
   ehb::DevBuf<uint64_t> bf_cbuf;
   ehb::DevBuf<uint32_t> bf_ccount;
+  // wide-beam walk scratch (WalkForm::beam): the persistent grid's visited tables and, at bf16, the [nq][ef] key sink.
+  // One wide-beam search at a time owns them (beam_mu); beam_done, recorded after its last kernel, orders the next
+  // one's use after it on the device.
+  std::mutex beam_mu;
+  ehb::DevBuf<uint32_t> beam_vtab;
+  ehb::DevBuf<uint64_t> beam_keys;
+  cudaEvent_t beam_done = nullptr;
   // Copies derived from the base rows, sized like vecs (capacity rows).  Each is created on the writer side of `rw`
   // by the first search that needs it, and from then on every mutation keeps rows [0, n) equal to a function of
   // vecs under the writer lock: add_rows and compact call derive_rows for the rows they wrote or moved,

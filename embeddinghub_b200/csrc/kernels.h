@@ -9,6 +9,7 @@ namespace ehb {
 
 constexpr uint32_t kMaxDim = 4096;  // pad_dim() supports rows up to 4096 floats
 constexpr uint32_t kMaxEf = 512;    // register-resident list: 16 keys per lane
+constexpr uint32_t kMaxBeam = 4096; // wide-beam walk (WalkForm::beam): shared-memory list, visited table in HBM
 constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved point, >= 1 + 32 + 32*32
 constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
 
@@ -21,7 +22,8 @@ constexpr bool dense_form(bool bf16, int LPV, int NQ, int KPL, bool HASDEL) {
 // Which graph-walk kernel a search runs and how it is launched (ehb_index::walk_plan).  The launchers and the
 // reported kernel name read it and decide nothing themselves.
 // wide: the form of the wide shapes (walk.cuh wide_shape, dpad 3072 and 4096), and their only one.
-enum class WalkForm { plain, dense, team, wide };
+// beam: every beam above kMaxEf, any row shape (beam_impl.cuh).
+enum class WalkForm { plain, dense, team, wide, beam };
 struct WalkPlan {
   bool bf16;           // the walk reads the bf16 shadow g.vecs16 (else the fp32 rows)
   int lpv, nq, kpl;    // row shape (walk.cuh row_lpv / row_nq) and result-set entries per lane (kpl_for)
@@ -32,6 +34,7 @@ struct WalkPlan {
                        // its cfg then has no TMA ring (staged = 0): rows go straight into registers
   WalkCfg cfg;
   uint32_t wpb;        // warps per block of the one-warp forms
+  uint32_t vtab;       // beam form: entries of each warp's visited table in HBM (cfg.hash_size is 0)
 };
 // the name of the kernel the plan launches, e.g. hnsw_search_kernel<LPV=32,NQ=6,KPL=4>
 void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes);
@@ -51,6 +54,21 @@ struct SearchShape {
   static cudaError_t launch(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
                             uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                             cudaStream_t s);
+};
+
+// K2b — the wide-beam walk (p.form == WalkForm::beam, ef <= kMaxBeam): a persistent grid of one-warp blocks, each
+// with a visited table of p.vtab entries in vtab.  beam_warps: the warps of the launch for nq queries (resident
+// warps, at most nq); vtab must hold warps * p.vtab entries.  Results, key sink and stats as launch_search.
+cudaError_t beam_warps(const WalkPlan& p, const GraphView& g, int sms, uint64_t nq, uint32_t* warps);
+cudaError_t launch_search_beam(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
+                               uint32_t* vtab, uint32_t warps, cudaStream_t s);
+template <uint32_t DPAD, class RowT>
+struct BeamShape {
+  static cudaError_t warps(const WalkPlan& p, int sms, uint64_t nq, uint32_t* out);
+  static cudaError_t launch(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                            uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats, uint32_t* vtab,
+                            uint32_t warps, cudaStream_t s);
 };
 
 // K2t — team walk (p.T warps per query); fp32 rows <= 1 KB and ef <= 256 only.

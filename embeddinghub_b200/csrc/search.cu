@@ -20,10 +20,32 @@ cudaError_t launch_search(const WalkPlan& p, const GraphView& g, const float* qu
   });
 }
 
+cudaError_t beam_warps(const WalkPlan& p, const GraphView& g, int sms, uint64_t nq, uint32_t* warps) {
+  return with_dpad(g.dpad, [&](auto d) {
+    constexpr uint32_t D = decltype(d)::value;
+    return p.bf16 ? BeamShape<D, __nv_bfloat16>::warps(p, sms, nq, warps) : BeamShape<D, float>::warps(p, sms, nq, warps);
+  });
+}
+
+cudaError_t launch_search_beam(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
+                               uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
+                               uint32_t* vtab, uint32_t warps, cudaStream_t s) {
+  if (nq == 0) return cudaSuccess;
+  if (p.bf16 && (!g.vecs16 || !sink.keys)) return cudaErrorInvalidValue;
+  return with_dpad(g.dpad, [&](auto d) {
+    constexpr uint32_t D = decltype(d)::value;
+    return p.bf16 ? BeamShape<D, __nv_bfloat16>::launch(p, g, queries, nq, k, ef, sink, out_counts, stats, vtab, warps, s)
+                  : BeamShape<D, float>::launch(p, g, queries, nq, k, ef, sink, out_counts, stats, vtab, warps, s);
+  });
+}
+
 // (HASDEL and ROW are named only when set, so the common instantiations keep their short names)
 void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes) {
   if (p.form == WalkForm::team)
     std::snprintf(out, out_bytes, "hnsw_search_team_kernel<NQ=%d,KPL=%d,T=%u,U=%u>", p.nq, p.kpl, p.T, p.U);
+  else if (p.form == WalkForm::beam)
+    std::snprintf(out, out_bytes, "hnsw_search_beam_kernel<LPV=%d,NQ=%d%s%s>", p.lpv, p.nq,
+                  p.hasdel ? ",HASDEL=1" : "", p.bf16 ? ",ROW=bf16" : "");
   else
     std::snprintf(out, out_bytes, "%s<LPV=%d,NQ=%d,KPL=%d%s%s>",
                   p.form == WalkForm::dense  ? "hnsw_search_dense_kernel"

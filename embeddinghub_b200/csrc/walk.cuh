@@ -830,6 +830,116 @@ __device__ __forceinline__ void ul_extract_all(WarpCtx& c, UList<KPL>& u) {
 }
 
 // ---------------------------------------------------------------------------
+// Shared-memory result set of the wide-beam walk (ef 513 .. 4096; hnsw_search_beam_kernel): the same unordered set
+// as UList, with the same entry encoding (hi: ordered distance; id: node id | expanded flag; an unused entry is hi 0,
+// id kInvalid), in the warp's key list c.keys, which holds lcap = align_up(ef, 32) 8-byte keys: the hi words
+// hi[0..lcap) and then the id words.  The set is 32 columns of C = lcap / 32 entries, column l at [l C, l C + C);
+// the set's n-th entry goes to row n / 32 of column n % 32, so a column's entries are its first rows.  Lane l keeps
+// its column's summary in registers: the worst (largest) entry and the closest unexpanded one, with their rows.
+// The set's worst entry and its closest unexpanded entry are then one warp reduction each; an insert into a set that
+// is not full tightens one column's summary; replacing the worst entry, or marking an entry expanded, rescans that
+// one column cooperatively (C / 32 shared loads per lane and two reductions: sl_scan).
+// ---------------------------------------------------------------------------
+struct SList {
+  uint32_t* hi;  // [lcap] column-major
+  uint32_t* id;  // [lcap]
+  uint32_t C;    // entries per column
+  uint32_t whi, wrow;  // this lane's column: worst entry (wrow kInvalid: the column is empty)
+  uint32_t uhi, urow;  // this lane's column: closest unexpanded entry (urow kInvalid: none)
+};
+__device__ __forceinline__ void sl_init(SList& u, const WarpCtx& c) {
+  u.hi = (uint32_t*)c.keys;
+  u.id = u.hi + c.lcap;
+  u.C = c.lcap / 32u;
+}
+// Recomputes column col's summary (worst too, when `worst`), held by lane col.  Ties go to the lower row.
+__device__ __forceinline__ void sl_scan(SList& u, uint32_t col, bool worst, uint32_t lane) {
+  __syncwarp();  // the writer of the column is done
+  const uint32_t* hc = u.hi + col * u.C;
+  const uint32_t* ic = u.id + col * u.C;
+  uint32_t wh = 0, wr = kInvalid, uh = 0xFFFFFFFFu, ur = kInvalid;
+  for (uint32_t r = lane; r < u.C; r += 32) {
+    const uint32_t h = hc[r], d = ic[r];
+    if (d != kInvalid && (wr == kInvalid || h > wh)) wh = h, wr = r;
+    if (!(d & kExpandedFlag) && (ur == kInvalid || h < uh)) uh = h, ur = r;
+  }
+  const uint32_t um = __reduce_min_sync(0xffffffffu, ur != kInvalid ? uh : 0xFFFFFFFFu);
+  const uint32_t ub = __ballot_sync(0xffffffffu, ur != kInvalid && uh == um);
+  const uint32_t urow = ub ? __shfl_sync(0xffffffffu, ur, __ffs(ub) - 1) : kInvalid;
+  if (lane == col) u.uhi = um, u.urow = urow;
+  if (worst) {
+    const uint32_t wm = __reduce_max_sync(0xffffffffu, wr != kInvalid ? wh : 0u);
+    const uint32_t wb = __ballot_sync(0xffffffffu, wr != kInvalid && wh == wm);
+    const uint32_t wrow = wb ? __shfl_sync(0xffffffffu, wr, __ffs(wb) - 1) : kInvalid;
+    if (lane == col) u.whi = wm, u.wrow = wrow;
+  }
+}
+__device__ __forceinline__ void ul_clear(SList& u, uint32_t ef, uint32_t lane) {
+  (void)ef;
+  __syncwarp();  // the previous query's readers are done
+  for (uint32_t i = lane; i < 32u * u.C; i += 32) u.hi[i] = 0, u.id[i] = kInvalid;
+  u.whi = 0, u.wrow = kInvalid, u.uhi = 0xFFFFFFFFu, u.urow = kInvalid;
+  __syncwarp();
+}
+// UList's ul_insert contract: warp-uniform; precondition when cnt == ef: hi < worst_hi.
+__device__ __forceinline__ void ul_insert(SList& u, uint32_t hi, uint32_t id, uint32_t ef, uint32_t& cnt,
+                                          uint32_t& worst_hi, uint32_t lane) {
+  if (cnt < ef) {
+    const uint32_t col = cnt & 31u, row = cnt >> 5;
+    if (lane == col) {
+      u.hi[col * u.C + row] = hi, u.id[col * u.C + row] = id;
+      if (u.wrow == kInvalid || hi > u.whi) u.whi = hi, u.wrow = row;
+      if (u.urow == kInvalid || hi < u.uhi) u.uhi = hi, u.urow = row;
+    }
+    __syncwarp();
+    cnt++;
+    if (cnt == ef) worst_hi = __reduce_max_sync(0xffffffffu, u.wrow != kInvalid ? u.whi : 0u);
+  } else {
+    const uint32_t b = __ballot_sync(0xffffffffu, u.wrow != kInvalid && u.whi == worst_hi);
+    const uint32_t col = __ffs(b) - 1;
+    const uint32_t row = __shfl_sync(0xffffffffu, u.wrow, col);
+    if (lane == col) u.hi[col * u.C + row] = hi, u.id[col * u.C + row] = id;
+    sl_scan(u, col, true, lane);
+    worst_hi = __reduce_max_sync(0xffffffffu, u.wrow != kInvalid ? u.whi : 0u);
+  }
+}
+// closest unexpanded entry: its key (flag clear) or kMaxKey; mark sets its expanded flag
+__device__ __forceinline__ uint64_t sl_take_min(SList& u, bool mark, uint32_t lane) {
+  const uint32_t m = __reduce_min_sync(0xffffffffu, u.urow != kInvalid ? u.uhi : 0xFFFFFFFFu);
+  const uint32_t b = __ballot_sync(0xffffffffu, u.urow != kInvalid && u.uhi == m);
+  if (!b) return kMaxKey;
+  const uint32_t col = __ffs(b) - 1;
+  const uint32_t at = col * u.C + __shfl_sync(0xffffffffu, u.urow, col);
+  const uint32_t node = u.id[at];
+  if (mark) {
+    __syncwarp();
+    if (lane == col) u.id[at] = node | kExpandedFlag;
+    sl_scan(u, col, false, lane);
+  }
+  return ((uint64_t)m << 32) | node;
+}
+__device__ __forceinline__ uint32_t ul_min_unexpanded(SList& u, bool mark, uint32_t lane) {
+  const uint64_t key = sl_take_min(u, mark, lane);
+  return key == kMaxKey ? kInvalid : (uint32_t)key;
+}
+__device__ __forceinline__ uint32_t ul_min_unexpanded_hi(const SList& u) {
+  return __reduce_min_sync(0xffffffffu, u.urow != kInvalid ? u.uhi : 0xFFFFFFFFu);
+}
+__device__ __forceinline__ bool ul_contains(const SList& u, uint32_t id) {
+  bool hit = false;
+  for (uint32_t i = (uint32_t)threadIdx.x & 31u; i < 32u * u.C; i += 32) hit |= u.id[i] != kInvalid && (u.id[i] & kIdMask) == id;
+  return __any_sync(0xffffffffu, hit);
+}
+// After the walk: clears every expanded flag, so that sl_take_min(u, true, lane) then takes the entries in ascending
+// order (UList's ul_extract_min).
+__device__ __forceinline__ void sl_begin_extract(SList& u, uint32_t lane) {
+  __syncwarp();
+  for (uint32_t i = lane; i < 32u * u.C; i += 32)
+    if (u.id[i] != kInvalid) u.id[i] &= kIdMask;
+  for (uint32_t col = 0; col < 32; ++col) sl_scan(u, col, false, lane);
+}
+
+// ---------------------------------------------------------------------------
 // Shared-memory sorted key list (cold paths: brute-force select, row merge).
 // Returns the insert position, or kInvalid when rejected (duplicate id or
 // beyond the limit).
@@ -978,8 +1088,9 @@ __device__ __forceinline__ uint32_t dq_min(const WarpCtx& c, uint32_t dn, uint32
 // the survivors are evaluated in fp32 and offered for admission.  A dropped candidate's fp32 distance is >= the
 // hop-start worst result, so it would not have been admitted (nor queued, if tombstoned): the walk, its results and
 // its counters stay the same.
-template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float, bool SCREEN = false>
-__device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], UList<KPL>& u,
+template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, class RowT = float, bool SCREEN = false,
+          class Set = UList<KPL>>
+__device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], Set& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
                                             WalkCounters& wc) {
   static_assert(!SCREEN || (screen_shape(LPV, NQ) && std::is_same<RowT, float>::value), "no screen for this shape");
@@ -1034,7 +1145,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
     __syncwarp();
   }
   hash_clear(c);
-  ul_clear<KPL>(u, ef, c.lane);
+  ul_clear(u, ef, c.lane);
   const uint8_t* __restrict__ del = (HASDEL && c.dcap) ? g.deleted : nullptr;  // warp-uniform
   uint32_t dn = 0;                                                  // entries in the deleted-candidate queue
   uint32_t ovf = 0;
@@ -1048,9 +1159,9 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
   bool ovf_any = false;
   // a tombstoned (or excluded) entry point is expanded once but never becomes a result
   const bool ep_result = ep != exclude && !(del && del[ep]);
-  if (ep_result) ul_insert<KPL>(u, f2ord(epdist), ep, ef, cnt, worst_hi, c.lane);
+  if (ep_result) ul_insert(u, f2ord(epdist), ep, ef, cnt, worst_hi, c.lane);
   uint32_t node = ep;
-  if (ep_result) node = ul_min_unexpanded<KPL>(u, true, c.lane);
+  if (ep_result) node = ul_min_unexpanded(u, true, c.lane);
   uint32_t nb = load_row(g, node, level, c.lane);
   for (;;) {
     if (level == 0) wc.hops_base++; else wc.hops_upper++;
@@ -1058,7 +1169,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
     if (HASDEL && wc.hops_base + wc.hops_upper > 64u * ef + 65536u) break;
     __syncwarp();
     // speculative: the row of the closest entry still unexpanded
-    const uint32_t spec = ul_min_unexpanded<KPL>(u, false, c.lane);
+    const uint32_t spec = ul_min_unexpanded(u, false, c.lane);
     uint32_t spec_row = kInvalid;
     if (spec != kInvalid) spec_row = load_row(g, spec & kIdMask, level, c.lane);
     bool is_new = false;
@@ -1109,8 +1220,8 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
           if (!((unsure >> j) & 1u)) dq_push(c, dn, hj, ij, cnt >= ef ? worst_hi : 0xFFFFFFFFu, ovf);
           continue;
         }
-        if (ovf_any && ul_contains<KPL>(u, ij)) continue;
-        ul_insert<KPL>(u, hj, ij, ef, cnt, worst_hi, c.lane);
+        if (ovf_any && ul_contains(u, ij)) continue;
+        ul_insert(u, hj, ij, ef, cnt, worst_hi, c.lane);
         if (PREFETCH && c.lane == 0) prefetch_l2(g.links0 + (size_t)ij * g.M0);
       }
     }
@@ -1118,7 +1229,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       // candidate_set.top(): the closer of (closest unexpanded result, closest queued tombstone)
       uint32_t dhi;
       const uint32_t dpos = dq_min(c, dn, dhi);
-      if (dhi < ul_min_unexpanded_hi<KPL>(u)) {
+      if (dhi < ul_min_unexpanded_hi(u)) {
         if (cnt >= ef && dhi > worst_hi) break;  // hnswlib: dist > lowerBound && top_candidates.size() == ef
         node = c.dq_id[dpos];
         __syncwarp();
@@ -1129,7 +1240,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
         continue;
       }
     }
-    node = ul_min_unexpanded<KPL>(u, true, c.lane);
+    node = ul_min_unexpanded(u, true, c.lane);
     if (node == kInvalid) break;
     nb = (node == spec) ? spec_row : load_row(g, node, level, c.lane);
   }

@@ -208,6 +208,38 @@ int ehb_index_get_batch(ehb_index* ix, uint64_t n, const uint64_t* labels_host, 
 int ehb_index_search_by_label_ex(ehb_index* ix, uint64_t nq, const uint64_t* labels_host, uint32_t k, uint32_t ef,
                                  int precision, uint64_t* out_labels_host, float* out_dists_host,
                                  uint32_t* out_counts_host);
+/* Graph search with a beam above 512 (hnswlib searchKnn with num in the hundreds or thousands).
+ * - Checks, in the order of every other search: an unknown precision, then a null query / label or out_labels
+ *   pointer fail with EHB_ERR_INVALID; then k == 0 or nq == 0 writes nothing and returns EHB_OK; then
+ *   max(ef, k_walk) > EHB_MAX_BEAM fails with EHB_ERR_INVALID (k_walk: k, or k + 1 by label; ef == 0: the index
+ *   default, which ehb_index_set_ef may set above 512).  By label, an unknown or tombstoned label then fails with
+ *   EHB_ERR_NOT_FOUND.  A rejected call leaves every output buffer untouched.
+ * - Up to max(ef, k_walk) == 512 each call is exactly ehb_index_search_ex(_dev) / ehb_index_search_by_label_ex:
+ *   the same kernel, results and counters.
+ * - Above 512 the wide-beam walk runs (hnsw_search_beam_kernel): hnswlib's searchKnn order and stop rule with beam
+ *   max(ef, k), one warp per query, its result set in shared memory and its visited table (2 * M0 * beam + 64
+ *   entries per walking warp) in device memory.  Labels, distance bits, counts and the hop / evaluation counters
+ *   equal hnswlib's on the same graph as long as the visited table does not overflow, as for the other walks.
+ *   Tombstones, padding with EHB_NO_LABEL / +inf, cosine normalisation and EHB_BF16 (walk the bf16 copy, re-rank
+ *   the whole retained set in fp32) behave as in ehb_index_search_ex; by label is the same k + 1 search followed
+ *   by the rule of ehb_index_search_by_label_ex.  The scratch (visited tables of the resident warps; at EHB_BF16
+ *   also nq * beam 8-byte keys) belongs to the index: it grows on demand, is freed with the index, and one
+ *   wide-beam search at a time uses it (the next waits for it on the device).  An allocation that fails returns
+ *   EHB_ERR_OOM before anything is written.
+ * - These calls do not go through the combining queue.  ehb_index_stats, ehb_index_last_kernel_ms and
+ *   ehb_index_last_kernel_name describe the walk; the kernel name is
+ *   hnsw_search_beam_kernel<LPV=..,NQ=..[,HASDEL=1][,ROW=bf16]>.
+ * out_dists / out_counts may be NULL. */
+#define EHB_MAX_BEAM 4096
+int ehb_index_search_beam(ehb_index* ix, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef,
+                          int precision, uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
+int ehb_index_search_beam_dev(ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k, uint32_t ef,
+                              int precision, uint64_t* out_labels_dev, float* out_dists_dev, uint32_t* out_counts_dev,
+                              void* stream);
+int ehb_index_search_by_label_beam(ehb_index* ix, uint64_t nq, const uint64_t* labels_host, uint32_t k, uint32_t ef,
+                                   int precision, uint64_t* out_labels_host, float* out_dists_host,
+                                   uint32_t* out_counts_host);
+
 /* The same rule over ehb_index_search_bruteforce(rows, k + 1, precision); k + 1 must be <= 2048. */
 int ehb_index_search_bruteforce_by_label(ehb_index* ix, uint64_t nq, const uint64_t* labels_host, uint32_t k,
                                          int precision, uint64_t* out_labels_host, float* out_dists_host,
