@@ -121,6 +121,8 @@ SYMBOLS = {
     "ehb_sharded_search_bruteforce": (C.c_int, [_VP, _U64, _VP, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_sharded_get_batch": (C.c_int, [_VP, _U64, _VP, _VP]),
     "ehb_sharded_search_by_label_ex": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_sharded_search_beam": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
+    "ehb_sharded_search_by_label_beam": (C.c_int, [_VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP]),
     "ehb_exchange_create": (C.c_int, [_I32, _U32, _U32, _U64, _U32, C.POINTER(_VP)]),
     "ehb_exchange_create_ex": (C.c_int, [_I32, _U32, _U32, _U64, _U32, _U32, C.POINTER(_VP)]),
     "ehb_exchange_destroy": (C.c_int, [_VP]),
@@ -132,6 +134,9 @@ SYMBOLS = {
     "ehb_exchange_search_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, _VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_search_ex_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, _VP]),
     "ehb_exchange_search_by_label_ex_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP]),
+    "ehb_exchange_search_beam_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "ehb_exchange_search_by_label_beam_dev": (C.c_int, [_VP, _VP, _U64, _VP, _U32, _U32, C.c_int, _VP, _VP, _VP,
+                                                        _VP]),
     "ehb_exchange_timed_out": (C.c_int, [_VP, C.POINTER(_U32)]),
 }
 
@@ -480,6 +485,14 @@ class ShardedIndex:
                                                         _p(out_l), _p(out_d), _p(out_c)), labels)
         return out_l, out_d, out_c
 
+    def search_by_label_beam(self, labels, k, ef=0, precision=FP32):
+        """search_by_label() with max(ef, k + 1) up to 4096 (ehb_sharded_search_by_label_beam)."""
+        lab = np.ascontiguousarray(np.atleast_1d(labels), dtype=np.uint64)
+        out_l, out_d, out_c = _alloc(lab.shape[0], k)
+        _check_key(lib().ehb_sharded_search_by_label_beam(self._h, lab.shape[0], _p(lab), k, ef, int(precision),
+                                                          _p(out_l), _p(out_d), _p(out_c)), labels)
+        return out_l, out_d, out_c
+
     @property
     def size(self):
         n = C.c_uint64()
@@ -499,6 +512,15 @@ class ShardedIndex:
         labels, dists, counts = _alloc(q.shape[0], k)
         check(lib().ehb_sharded_search_ex(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
                                           _p(counts)))
+        return labels, dists, counts
+
+    def search_beam(self, q, k, ef=0, precision=FP32):
+        """search() with max(ef, k) up to 4096: the wide-beam walk on every shard above 512, then the same merge
+        (ehb_sharded_search_beam); up to 512 exactly search()."""
+        q = np.ascontiguousarray(q, dtype=np.float32).reshape(-1, self.dim)
+        labels, dists, counts = _alloc(q.shape[0], k)
+        check(lib().ehb_sharded_search_beam(self._h, q.shape[0], _p(q), k, ef, int(precision), _p(labels), _p(dists),
+                                            _p(counts)))
         return labels, dists, counts
 
     def search_bruteforce(self, q, k, precision=FP32):

@@ -828,6 +828,23 @@ int ehb::copy_results(uint64_t nq, uint32_t k, const uint64_t* dl, const float* 
   return EHB_OK;
 }
 
+int ehb_index::grow_beam(const ehb::WalkPlan& plan, uint64_t nq, uint32_t ef_eff, cudaStream_t s, uint32_t* warps) {
+  if (!beam_done) CU(cudaEventCreateWithFlags(&beam_done, cudaEventDisableTiming));
+  CU(cudaStreamWaitEvent(s, beam_done, 0));
+  CU(ehb::beam_warps(plan, view(), sms, nq, warps));
+  CU(beam_vtab.grow((size_t)*warps * plan.vtab, 0, -1, s));
+  if (plan.bf16) CU(beam_keys.grow(nq * ef_eff, 0, -1, s));
+  return EHB_OK;
+}
+
+int ehb_index::reserve_beam(uint64_t nq, uint32_t ef_eff, int precision, cudaStream_t s) {
+  const ehb::WalkPlan plan = walk_plan(nq, ef_eff, precision == EHB_BF16);
+  if (plan.form != ehb::WalkForm::beam) return EHB_OK;
+  std::lock_guard<std::mutex> bl(beam_mu);
+  uint32_t warps = 0;
+  return grow_beam(plan, nq, ef_eff, s, &warps);
+}
+
 int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uint32_t k, uint32_t ef_in, uint64_t* dl,
                           float* dd, uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink, bool* pushed,
                           int precision) {
@@ -842,14 +859,13 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
   uint32_t warps = 0;
   if (beam) {
     bl.lock();
-    if (!beam_done) CU(cudaEventCreateWithFlags(&beam_done, cudaEventDisableTiming));
-    CU(cudaStreamWaitEvent(s, beam_done, 0));
-    CU(ehb::beam_warps(plan, view(), sms, nq, &warps));
-    CU(beam_vtab.grow((size_t)warps * plan.vtab, 0, -1, s));
-    if (bf16) CU(beam_keys.grow(nq * ef_eff, 0, -1, s));
+    RET(grow_beam(plan, nq, ef_eff, s, &warps));
   }
-  // the team walk writes destination 0 only (a bf16 search never plans one: its re-rank stores to every destination)
-  if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team;
+  // the team walk writes destination 0 only (a bf16 search never plans one: its re-rank stores to every destination),
+  // and so does the re-rank of more than kMaxEf results (its sink form collects at most that many keys in shared
+  // memory): the exchange's merge kernel then pushes the block
+  const bool rerank_sink = sink && bf16 && k <= ehb::kMaxEf;
+  if (pushed) *pushed = sink && plan.form != ehb::WalkForm::team && (!bf16 || rerank_sink);
   const float* q = dq;
   if (metric == EHB_COSINE) {
     CU(sl->q_norm.grow(nq * dim, 0, -1, s));
@@ -878,7 +894,7 @@ int ehb_index::search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uin
                                  beam_vtab.p, warps, s));
     else
       CU(ehb::launch_search(plan, g, q, (uint32_t)nq, ef_eff, ef_eff, ks, sl->walk_counts.p, sl->stats.p, s));
-    if (sink)
+    if (rerank_sink)
       CU(ehb::launch_rerank_sink(ks.keys, ef_eff, sl->q_pad.p, vecs.p, dpad, dim, metric == EHB_L2 ? 0 : 1,
                                  labels.p, nq, k, *sink, dc, s));
     else
@@ -1478,9 +1494,10 @@ int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint3
 
 int ehb_index_search_dev_sink_held(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, uint64_t nq, const float* dq,
                                    uint32_t k, uint32_t ef, int precision, const ehb::ResultSink* sink, uint32_t* dc,
-                                   cudaStream_t stream, bool* pushed) {
+                                   cudaStream_t stream, bool* pushed, uint32_t max_beam) {
   bool none;
-  RET(ehb::check_request(ix, false, precision, !dq || !sink || !sink->n || !sink->labels[0], nq, k, k, &ef, &none));
+  RET(ehb::check_request(ix, false, precision, !dq || !sink || !sink->n || !sink->labels[0], nq, k, k, &ef, &none,
+                         max_beam));
   if (none) return EHB_OK;
   RET(ix->prepare(lk, false, precision, nq));
   ehb::SlotLease ls(ix);

@@ -70,6 +70,9 @@ __global__ void __launch_bounds__(32, 1)
         }
       }
     }
+    // the exchange's slice flags (walk.cuh): the persistent grid finishes queries [i W, (i + 1) W) in round i, so the
+    // contiguous slices still complete roughly in order
+    if constexpr (!kKeys) sink_query_done(sink, q, nq, c.lane);
     if (c.lane == 0) {
       if (out_counts) out_counts[q] = found;
       if (stats) {

@@ -507,32 +507,48 @@ int ehb_exchange_merge_dev(ehb_exchange* ex, float* out_dists_dev, uint64_t* out
 }
 
 // One sharded graph search step, fused: this rank's search stores every query's top-k straight into every peer's
-// receive buffer from its last kernel (the fp32 walk's epilogue, or the re-rank after a bf16 walk: coalesced stores
-// over NVLink while the other queries are still running) and raises per-slice flags; then one kernel waits for the
-// peers' flags and merges.  Falls back to push-after-walk when the batch is small enough for the team walk (fp32
-// only).  Call in lock step on every rank.  Everything that can be rejected is checked before the epoch advances:
-// a rank that failed after it would be one step out of phase with its peers, whose merges would then wait for it
-// until they time out.
-int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+// receive buffer from its last kernel (the fp32 walk's epilogue, the wide-beam walk's, or the re-rank after a bf16
+// walk: coalesced stores over NVLink while the other queries are still running) and raises per-slice flags; then one
+// kernel waits for the peers' flags and merges.  Falls back to push-after-walk when the batch is small enough for the
+// team walk (fp32 only).  Call in lock step on every rank.  Everything that can be rejected is checked before the
+// epoch advances, and the wide-beam scratch is grown before it too: a rank that failed after it would be one step out
+// of phase with its peers, whose merges would then wait for it until they time out.  Locks in the order of the
+// by-label step: ex->mu, then the reader side of ix->rw, held from the check through the search launch so that the
+// walk plan the scratch was reserved for is the one that runs.  max_beam: 512 (_ex) or kMaxBeam (_beam).
+static int exchange_fused_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
                                uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
-                               uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream) {
-  if (!ex || !ix || !queries_dev || !out_labels_dev) return fail(EHB_ERR_INVALID, "null argument");
+                               uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream, uint32_t max_beam) {
+  if (!ex || !ix) return fail(EHB_ERR_INVALID, "null argument");
+  std::lock_guard<std::mutex> g(ex->mu);
+  std::shared_lock<ehb::RwLock> lk(ix->rw);
   bool none;
-  {
-    std::shared_lock<ehb::RwLock> lk(ix->rw);  // ef == 0 reads the index default; the search below gets the checked ef
-    RET(ehb::check_request(ix, false, precision, false, nq, k, k, &ef, &none));
-  }
+  RET(ehb::check_request(ix, false, precision, !queries_dev || !out_labels_dev, nq, k, k, &ef, &none, max_beam));
   if (none || nq * k > ex->max_elems) return fail(EHB_ERR_INVALID, "nq * k exceeds the exchange capacity");
   if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
   CU(cudaSetDevice(ex->device));
-  std::lock_guard<std::mutex> g(ex->mu);
+  const cudaStream_t s = (cudaStream_t)stream;
+  RET(ix->prepare(lk, false, precision, nq));
+  RET(ix->reserve_beam(nq, std::max(ef, k), precision, s));
   ex->epoch++;
   const ehb::ResultSink sink = step_sink(ex, nq, k);
   bool pushed = false;
-  RET(ehb_index_search_dev_sink(ix, nq, queries_dev, k, ef, precision, &sink, shard_counts_dev, (cudaStream_t)stream,
-                                &pushed));
+  RET(ehb_index_search_dev_sink_held(ix, lk, nq, queries_dev, k, ef, precision, &sink, shard_counts_dev, s, &pushed,
+                                     max_beam));
   CU(cudaSetDevice(ex->device));
-  return launch_exchange_merge(ex, nq, k, out_dists_dev, out_labels_dev, out_counts_dev, (cudaStream_t)stream, pushed);
+  return launch_exchange_merge(ex, nq, k, out_dists_dev, out_labels_dev, out_counts_dev, s, pushed);
+}
+
+int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                               uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
+                               uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream) {
+  return exchange_fused_step(ex, ix, nq, queries_dev, k, ef, precision, out_dists_dev, out_labels_dev, out_counts_dev,
+                             shard_counts_dev, stream, ehb::kMaxEf);
+}
+int ehb_exchange_search_beam_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                                 uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
+                                 uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream) {
+  return exchange_fused_step(ex, ix, nq, queries_dev, k, ef, precision, out_dists_dev, out_labels_dev, out_counts_dev,
+                             shard_counts_dev, stream, ehb::kMaxBeam);
 }
 
 // Key mode over the exchange: a row step at epoch e (every holder pushes its stored rows to every rank, and every
@@ -540,16 +556,18 @@ int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, con
 // k + 1 step at e + 1 over the pushed rows, the merge, and the self-removal.  The reader side of ix->rw is held from
 // prepare through the search launch, so the resolved ids cannot move under a compaction.  Locks in the order of
 // ehb_exchange_search_ex_dev: ex->mu first, then ix->rw (a writer-preferring lock taken in the other order by a
-// second thread on the same exchange could deadlock).
-int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
-                                        uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
-                                        uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream) {
+// second thread on the same exchange could deadlock).  The wide-beam scratch of the k + 1 search is grown before the
+// first epoch, like every check.  max_beam: 512 (_ex) or kMaxBeam (_beam).
+static int exchange_by_label_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                  uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                  uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream,
+                                  uint32_t max_beam) {
   if (!ex || !ix) return fail(EHB_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> g(ex->mu);
   std::shared_lock<ehb::RwLock> lk(ix->rw);
   bool none;
   RET(ehb::check_request(ix, false, precision, !labels_host || !out_labels_dev || !out_dists_dev || !out_counts_dev,
-                         nq, k, k + 1ull, &ef, &none));
+                         nq, k, k + 1ull, &ef, &none, max_beam));
   if (none) return EHB_OK;
   const uint32_t k1 = k + 1;
   if (nq > ex->max_nq || nq * k1 > ex->max_elems)
@@ -559,6 +577,7 @@ int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_
   CU(cudaSetDevice(ex->device));
   const cudaStream_t s = (cudaStream_t)stream;
   RET(ix->prepare(lk, false, precision, nq));
+  RET(ix->reserve_beam(nq, std::max(ef, k1), precision, s));
   uint64_t* h_self = (uint64_t*)ex->bl_host;
   uint32_t* h_ids = (uint32_t*)(h_self + ex->max_nq);
   uint32_t* h_verdict = h_ids + ex->max_nq;
@@ -587,13 +606,26 @@ int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_
   const float* rows = (const float*)(ex->local + ex->rows_off) + parity * ex->row_stride;
   const ehb::ResultSink sink = step_sink(ex, nq, k1);
   bool pushed = false;
-  RET(ehb_index_search_dev_sink_held(ix, lk, nq, rows, k1, ef, precision, &sink, nullptr, s, &pushed));
+  RET(ehb_index_search_dev_sink_held(ix, lk, nq, rows, k1, ef, precision, &sink, nullptr, s, &pushed, max_beam));
   CU(cudaSetDevice(ex->device));
   RET(launch_exchange_merge(ex, nq, k1, ex->bl_dists, ex->bl_labels, ex->bl_counts, s, pushed));
   CU(ehb::launch_drop_self(ex->bl_self, ex->bl_labels, ex->bl_dists, ex->bl_counts, nq, k, out_labels_dev,
                            out_dists_dev, out_counts_dev, s));
   CU(cudaEventRecord(ex->bl_done, s));
   return EHB_OK;
+}
+
+int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                        uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                        uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream) {
+  return exchange_by_label_step(ex, ix, nq, labels_host, k, ef, precision, out_dists_dev, out_labels_dev,
+                                out_counts_dev, stream, ehb::kMaxEf);
+}
+int ehb_exchange_search_by_label_beam_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                          uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                          uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream) {
+  return exchange_by_label_step(ex, ix, nq, labels_host, k, ef, precision, out_dists_dev, out_labels_dev,
+                                out_counts_dev, stream, ehb::kMaxBeam);
 }
 
 int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
@@ -827,9 +859,9 @@ int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
 // Every shard searches, device 0 merges into m_labels / m_dists / m_counts (queued on st[0]).  Caller holds mu.
 // q: host queries, or nullptr when every q_dev already holds them (queued on the shards' streams).
 // brute: the exact / bf16 brute force instead of the graph walk (a bf16 walk re-ranks straight into device 0's gather
-// block, like the fp32 walk).
+// block, like the fp32 walk).  beam: ehb_index_search_beam_dev on every shard instead of ehb_index_search_ex_dev.
 static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
-                         int precision) {
+                         int precision, bool beam = false) {
   const uint32_t G = (uint32_t)sh->shard.size();
   const uint32_t dim = sh->prm.dim;
   const uint64_t blk = (nq * k * 12ull + 255) / 256 * 256;
@@ -859,7 +891,8 @@ static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* 
     if (brute)
       RET(ehb_index_search_bruteforce_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, precision, dl, dd, sh->cnt_dev[i]->p, s));
     else
-      RET(ehb_index_search_ex_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, ef, precision, dl, dd, sh->cnt_dev[i]->p, s));
+      RET((beam ? ehb_index_search_beam_dev : ehb_index_search_ex_dev)(sh->shard[i], nq, sh->q_dev[i]->p, k, ef,
+                                                                       precision, dl, dd, sh->cnt_dev[i]->p, s));
     CU(cudaSetDevice(sh->dev[i]));
     if (i && !sh->peer_direct && sh->dev[i] != sh->dev[0])
       CU(cudaMemcpyPeerAsync(sh->gather.p + blk * i, sh->dev[0], dst, sh->dev[i], nq * k * 12ull, s));
@@ -873,26 +906,27 @@ static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* 
 }
 
 // ehb::check_request on every shard, each under its reader lock (ef == 0 reads the shard's default; each shard's search
-// resolves and checks it again under its own lock).
+// resolves and checks it again under its own lock).  max_beam: the graph walk's width limit (512, or kMaxBeam).
 static int check_shards(ehb_sharded* sh, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
-                        uint64_t k_walk, uint32_t ef, bool* none) {
+                        uint64_t k_walk, uint32_t ef, bool* none, uint32_t max_beam = ehb::kMaxEf) {
   for (ehb_index* ix : sh->shard) {
     std::shared_lock<ehb::RwLock> lk(ix->rw);
     uint32_t ef_shard = ef;
-    RET(ehb::check_request(ix, brute, precision, null_buf, nq, k, k_walk, brute ? nullptr : &ef_shard, none));
+    RET(ehb::check_request(ix, brute, precision, null_buf, nq, k, k_walk, brute ? nullptr : &ef_shard, none,
+                           max_beam));
   }
   return EHB_OK;
 }
 
 // Host queries in, merged host results out.
 static int sharded_search(ehb_sharded* sh, bool brute, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
-                          int precision, uint64_t* ol, float* od, uint32_t* oc) {
+                          int precision, uint64_t* ol, float* od, uint32_t* oc, bool beam = false) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   bool none;
-  RET(check_shards(sh, brute, precision, nq && (!q || !ol), nq, k, k, ef, &none));
+  RET(check_shards(sh, brute, precision, nq && (!q || !ol), nq, k, k, ef, &none, beam ? ehb::kMaxBeam : ehb::kMaxEf));
   if (none) return EHB_OK;
   std::lock_guard<std::mutex> g(sh->mu);
-  RET(sharded_merge(sh, brute, nq, q, k, ef, precision));
+  RET(sharded_merge(sh, brute, nq, q, k, ef, precision, beam));
   RET(ehb::copy_results(nq, k, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, ol, od, oc, sh->st[0]));
   CU(cudaStreamSynchronize(sh->st[0]));
   return EHB_OK;
@@ -909,6 +943,10 @@ int ehb_sharded_search_ex(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t
 int ehb_sharded_search_bruteforce(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, int precision, uint64_t* ol,
                                   float* od, uint32_t* oc) {
   return sharded_search(sh, true, nq, q, k, 0, precision, ol, od, oc);
+}
+int ehb_sharded_search_beam(ehb_sharded* sh, uint64_t nq, const float* q, uint32_t k, uint32_t ef, int precision,
+                            uint64_t* ol, float* od, uint32_t* oc) {
+  return sharded_search(sh, false, nq, q, k, ef, precision, ol, od, oc, true);
 }
 
 int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, float* out) {
@@ -935,12 +973,14 @@ int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, f
 
 // The rows are laid out in owner order: shard o gathers its labels' rows into its own staging rows
 // [first[o], first[o] + m_o) and copies them into every other shard's staging buffer; each shard then scatters the
-// staging rows to their query positions in q_dev, and the k + 1 search + merge of ehb_sharded_search_ex runs on them.
-int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
-                                   int precision, uint64_t* ol, float* od, uint32_t* oc) {
+// staging rows to their query positions in q_dev, and the k + 1 search + merge of ehb_sharded_search_ex (beam:
+// ehb_sharded_search_beam) runs on them.
+static int sharded_by_label(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                            int precision, uint64_t* ol, float* od, uint32_t* oc, bool beam) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   bool none;
-  RET(check_shards(sh, false, precision, nq && (!labels || !ol), nq, k, k + 1ull, ef, &none));
+  RET(check_shards(sh, false, precision, nq && (!labels || !ol), nq, k, k + 1ull, ef, &none,
+                   beam ? ehb::kMaxBeam : ehb::kMaxEf));
   if (none) return EHB_OK;
   const uint32_t k1 = k + 1;
   std::lock_guard<std::mutex> g(sh->mu);
@@ -988,7 +1028,7 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
     CU(cudaMemcpyAsync(sh->q_pos[i]->p, order.data(), nq * 4, cudaMemcpyHostToDevice, s));
     CU(ehb::launch_gather_rows(sh->q_stage[i]->p, dim, nullptr, sh->q_dev[i]->p, dim, sh->q_pos[i]->p, nq, dim, s));
   }
-  RET(sharded_merge(sh, false, nq, nullptr, k1, ef, precision));
+  RET(sharded_merge(sh, false, nq, nullptr, k1, ef, precision, beam));
   CU(cudaSetDevice(sh->dev[0]));
   cudaStream_t s0 = sh->st[0];
   CU(sh->s_self.grow(nq, 0, -1, s0));
@@ -1001,6 +1041,15 @@ int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t*
   RET(ehb::copy_results(nq, k, sh->s_labels.p, sh->s_dists.p, sh->s_counts.p, ol, od, oc, s0));
   CU(cudaStreamSynchronize(s0));
   return EHB_OK;
+}
+
+int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                                   int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  return sharded_by_label(sh, nq, labels, k, ef, precision, ol, od, oc, false);
+}
+int ehb_sharded_search_by_label_beam(ehb_sharded* sh, uint64_t nq, const uint64_t* labels, uint32_t k, uint32_t ef,
+                                     int precision, uint64_t* ol, float* od, uint32_t* oc) {
+  return sharded_by_label(sh, nq, labels, k, ef, precision, ol, od, oc, true);
 }
 
 }  // extern "C"

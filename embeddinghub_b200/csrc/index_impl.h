@@ -221,10 +221,11 @@ int copy_results(uint64_t nq, uint32_t k, const uint64_t* dl, const float* dd, c
 int ehb_index_search_dev_sink(ehb_index* ix, uint64_t nq, const float* dq, uint32_t k, uint32_t ef, int precision,
                               const ehb::ResultSink* sink, uint32_t* dc, cudaStream_t stream, bool* pushed);
 // The same for a caller that already holds the reader side of ix->rw as `lk` (a second shared acquire would deadlock
-// behind a queued writer) and has made the device current
+// behind a queued writer) and has made the device current.  max_beam: the width limit of ehb::check_request (512, or
+// kMaxBeam for the wide-beam exchange steps)
 int ehb_index_search_dev_sink_held(ehb_index* ix, std::shared_lock<ehb::RwLock>& lk, uint64_t nq, const float* dq,
                                    uint32_t k, uint32_t ef, int precision, const ehb::ResultSink* sink, uint32_t* dc,
-                                   cudaStream_t stream, bool* pushed);
+                                   cudaStream_t stream, bool* pushed, uint32_t max_beam = ehb::kMaxEf);
 // The stored rows of n live labels into rows_dev ([n][dim] on the index's device), queued on `stream`; an unknown or
 // tombstoned label fails with EHB_ERR_NOT_FOUND before anything is queued (exchange.cu: by-label sharded searches)
 int ehb_index_gather_dev(ehb_index* ix, uint64_t n, const uint64_t* labels_host, float* rows_dev, cudaStream_t stream);
@@ -379,6 +380,14 @@ struct ehb_index {
   int search_dev(ehb::SearchSlot* sl, uint64_t nq, const float* dq, uint32_t k, uint32_t ef_in, uint64_t* dl, float* dd,
                  uint32_t* dc, cudaStream_t s, const ehb::ResultSink* sink = nullptr, bool* pushed = nullptr,
                  int precision = EHB_FP32);
+  // The wide-beam scratch a search_dev of nq queries at beam ef_eff (= max(ef, k)) needs, grown now on s, so that the
+  // search's own grow does nothing: the exchange steps call it before their epoch advances, so that an allocation
+  // failure (EHB_ERR_OOM) leaves the rank in phase.  Nothing happens when the plan is not the wide-beam walk.  A grow
+  // synchronises s and frees the old buffer (which waits for the device).  Caller holds the reader lock, so the plan
+  // cannot change before the search.
+  int reserve_beam(uint64_t nq, uint32_t ef_eff, int precision, cudaStream_t s);
+  // caller holds beam_mu: waits for the previous wide-beam search on s, then grows the scratch for `plan`
+  int grow_beam(const ehb::WalkPlan& plan, uint64_t nq, uint32_t ef_eff, cudaStream_t s, uint32_t* warps);
   int bruteforce_dev(uint64_t nq, const float* dq, uint32_t k, int precision, uint64_t* dl, float* dd, uint32_t* dc,
                      cudaStream_t s);
   void reset_content();

@@ -120,9 +120,11 @@ class ShardedSearcher:
                 md=t.empty((nq, k), dtype=t.float32, device=dev), mc=t.empty(nq, dtype=t.int32, device=dev))
         return self._buf[key]
 
-    def _local(self, q, nq, k, ef, stream_ptr, bruteforce, precision, lp, dp, cp):
+    def _local(self, q, nq, k, ef, stream_ptr, bruteforce, precision, lp, dp, cp, beam=False):
         if bruteforce:
             self.ix.search_bruteforce_dev(q.data_ptr(), nq, k, precision, lp, dp, cp, stream_ptr)
+        elif beam:
+            self.ix.search_beam_dev(q.data_ptr(), nq, k, ef, lp, dp, cp, stream_ptr, precision)
         else:
             self.ix.search_dev(q.data_ptr(), nq, k, ef, lp, dp, cp, stream_ptr, precision)
 
@@ -130,11 +132,20 @@ class ShardedSearcher:
         """q: CUDA float32 tensor [nq, dim].  Returns (labels int64-viewed-u64, dists, counts) CUDA tensors
         holding the global top-k on every rank.  precision (FP32 or BF16) applies to graph searches and brute force
         alike, on every exchange.  Nothing synchronises the host."""
+        return self._search_dev(q, k, ef, stream_ptr, bruteforce, precision, False)
+
+    def search_beam_dev(self, q, k, ef, stream_ptr, precision=0):
+        """search_dev() of the graph walk with max(ef, k) up to 4096: the wide-beam walk above 512.  World 1:
+        NativeIndex.search_beam_dev; the peer exchange: one ehb_exchange_search_beam_dev step; exchange="nccl": the
+        local beam search, then the same all-gather and merge."""
+        return self._search_dev(q, k, ef, stream_ptr, False, precision, True)
+
+    def _search_dev(self, q, k, ef, stream_ptr, bruteforce, precision, beam):
         nq = q.shape[0]
         b = self._bufs(nq, k)
         if self.world == 1:
             self._local(q, nq, k, ef, stream_ptr, bruteforce, precision, b["l"].data_ptr(), b["d"].data_ptr(),
-                        b["c"].data_ptr())
+                        b["c"].data_ptr(), beam)
             return b["l"], b["d"], b["c"]
         if self.exchange == "peer":
             self._ensure_exchange(nq, k)
@@ -142,10 +153,10 @@ class ShardedSearcher:
                 # fused: the search's last kernel (the fp32 walk's epilogue, or the re-rank after a bf16 walk)
                 # stores each query's top-k into every peer's receive buffer and raises the slice flags; one kernel
                 # waits for the peers' flags and merges
-                check(lib().ehb_exchange_search_ex_dev(self._ex, self.ix._h, nq, C.c_void_p(q.data_ptr()), k, ef,
-                                                       int(precision), C.c_void_p(b["md"].data_ptr()),
-                                                       C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
-                                                       C.c_void_p(b["c"].data_ptr()), C.c_void_p(stream_ptr)))
+                step = lib().ehb_exchange_search_beam_dev if beam else lib().ehb_exchange_search_ex_dev
+                check(step(self._ex, self.ix._h, nq, C.c_void_p(q.data_ptr()), k, ef, int(precision),
+                           C.c_void_p(b["md"].data_ptr()), C.c_void_p(b["ml"].data_ptr()),
+                           C.c_void_p(b["mc"].data_ptr()), C.c_void_p(b["c"].data_ptr()), C.c_void_p(stream_ptr)))
                 return b["ml"], b["md"], b["mc"]
             lp, dp = C.c_void_p(), C.c_void_p()
             check(lib().ehb_exchange_begin(self._ex, nq, k, C.byref(lp), C.byref(dp)))
@@ -158,7 +169,7 @@ class ShardedSearcher:
         import torch.distributed as dist
 
         self._local(q, nq, k, ef, stream_ptr, bruteforce, precision, b["l"].data_ptr(), b["d"].data_ptr(),
-                    b["c"].data_ptr())
+                    b["c"].data_ptr(), beam)
         dist.all_gather_into_tensor(b["recv"].view(-1), b["send"], group=self.group)
         check(lib().ehb_merge_topk_packed_dev(self.world, nq, k, C.c_void_p(b["recv"].data_ptr()),
                                               b["recv"].shape[1], C.c_void_p(b["md"].data_ptr()),
@@ -177,6 +188,14 @@ class ShardedSearcher:
         else 4 (a label on two ranks).  At world 1 it is NativeIndex.search_by_label (KeyError for an unknown label),
         which synchronises the host, with the results copied into CUDA tensors on stream_ptr.  exchange="nccl" raises
         ValueError: it has no row exchange."""
+        return self._by_label_dev(labels, k, ef, stream_ptr, precision, False)
+
+    def search_by_label_beam_dev(self, labels, k, ef, stream_ptr, precision=0):
+        """search_by_label_dev() with max(ef, k + 1) up to 4096: one ehb_exchange_search_by_label_beam_dev step on
+        the peer exchange, NativeIndex.search_by_label_beam at world 1; exchange="nccl" raises ValueError."""
+        return self._by_label_dev(labels, k, ef, stream_ptr, precision, True)
+
+    def _by_label_dev(self, labels, k, ef, stream_ptr, precision, beam):
         if self.exchange == "nccl":
             raise ValueError("search_by_label_dev needs the peer exchange (exchange='peer'); the NCCL path only "
                              "exchanges result lists")
@@ -185,7 +204,8 @@ class ShardedSearcher:
         if self.world == 1:
             # a host search (it synchronises); the results are allocated and copied on stream_ptr, so work queued
             # there afterwards reads them in order
-            ol, od, oc = self.ix.search_by_label(lab, k, ef=ef, precision=precision)
+            search = self.ix.search_by_label_beam if beam else self.ix.search_by_label
+            ol, od, oc = search(lab, k, ef=ef, precision=precision)
             t = self._torch
             dev = t.device("cuda", self.device)
             s = t.cuda.ExternalStream(stream_ptr, device=dev) if stream_ptr else t.cuda.current_stream(dev)
@@ -194,8 +214,8 @@ class ShardedSearcher:
                              for a in (ol.view(np.int64), od, oc.view(np.int32)))
         b = self._bufs(nq, k)
         self._ensure_exchange(nq, k + 1, self.ix.dim)
-        check(lib().ehb_exchange_search_by_label_ex_dev(self._ex, self.ix._h, nq, lab.ctypes.data_as(C.c_void_p), k,
-                                                        ef, int(precision), C.c_void_p(b["md"].data_ptr()),
-                                                        C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
-                                                        C.c_void_p(stream_ptr)))
+        step = lib().ehb_exchange_search_by_label_beam_dev if beam else lib().ehb_exchange_search_by_label_ex_dev
+        check(step(self._ex, self.ix._h, nq, lab.ctypes.data_as(C.c_void_p), k, ef, int(precision),
+                   C.c_void_p(b["md"].data_ptr()), C.c_void_p(b["ml"].data_ptr()), C.c_void_p(b["mc"].data_ptr()),
+                   C.c_void_p(stream_ptr)))
         return b["ml"], b["md"], b["mc"]

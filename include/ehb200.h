@@ -350,6 +350,19 @@ int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels_ho
 int ehb_sharded_search_by_label_ex(ehb_sharded* sh, uint64_t nq, const uint64_t* labels_host, uint32_t k, uint32_t ef,
                                    int precision, uint64_t* out_labels_host, float* out_dists_host,
                                    uint32_t* out_counts_host);
+/* The sharded searches with a beam above 512: ehb_index_search_beam_dev on every shard, storing into device_ids[0]'s
+ * gather buffer, then the same merge; by label, the same row staging, the k + 1 beam search on every shard, the merge
+ * and the self-removal rule.  Checks and their order as ehb_index_search_beam / ehb_index_search_by_label_beam
+ * (max(ef, k_walk) > EHB_MAX_BEAM fails with EHB_ERR_INVALID).  Up to max(ef, k_walk) == 512 each call is exactly
+ * ehb_sharded_search_ex / ehb_sharded_search_by_label_ex.  Above, the result equals ehb_merge_topk_dev over every
+ * shard's own ehb_index_search_beam_dev output (labels, distance bits, counts), followed by label by the rule.  The
+ * gather buffer on device_ids[0] is n_dev * nq * k_walk * 12 bytes (10k queries at k = 4096 over 8 shards: 3.9 GB),
+ * and each shard grows its own wide-beam scratch as ehb_index_search_beam does. */
+int ehb_sharded_search_beam(ehb_sharded* sh, uint64_t nq, const float* queries_host, uint32_t k, uint32_t ef,
+                            int precision, uint64_t* out_labels_host, float* out_dists_host, uint32_t* out_counts_host);
+int ehb_sharded_search_by_label_beam(ehb_sharded* sh, uint64_t nq, const uint64_t* labels_host, uint32_t k,
+                                     uint32_t ef, int precision, uint64_t* out_labels_host, float* out_dists_host,
+                                     uint32_t* out_counts_host);
 
 /* Shard exchange for one-process-per-GPU deployments (torchrun / MPI): replaces "one ncclAllGather of the
  * per-shard top-k + merge kernel" (SURVEY.md §8e) with ONE kernel per rank that pushes this rank's lists
@@ -421,6 +434,35 @@ int ehb_exchange_search_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, con
 int ehb_exchange_search_by_label_ex_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
                                         uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
                                         uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream);
+/* The exchange steps with a beam above 512 (same arguments as the _ex forms).
+ * - ehb_exchange_search_beam_dev is the fused step with each rank's search being ehb_index_search_beam_dev: the
+ *   wide-beam walk (or, at EHB_BF16, the re-rank after it) stores each query's top-k into every peer's receive buffer
+ *   and raises the slice flags, then the merge (at EHB_BF16 with k_walk > 512 the re-rank writes this rank's block
+ *   and the merge kernel pushes it).  ehb_exchange_search_by_label_beam_dev is the row step, then that
+ *   fused step at k + 1, the merge and the self-removal rule of ehb_exchange_search_by_label_ex_dev.
+ * - Up to max(ef, k_walk) == 512 (k_walk: k, or k + 1 by label) each call is exactly its _ex counterpart: the same
+ *   kernels, results and counters.  Above, on every rank the result equals ehb_merge_topk_dev over every rank's own
+ *   ehb_index_search_beam_dev output (labels, distance bits, counts), followed by label by the self-removal rule;
+ *   shard_counts_dev is this shard's own beam counts.
+ * - Checked in the order of every other search, each before the epoch advances and with the output buffers
+ *   untouched, so the next step still pairs with the peers': an unknown precision, a null pointer, nq == 0 or
+ *   k == 0 (as in the _ex form: the fused step fails with EHB_ERR_INVALID, by label writes nothing), max(ef, k_walk)
+ *   > EHB_MAX_BEAM, nq * k_walk above max_nq * max_k (and by label nq > max_nq), by label an index dim above max_dim,
+ *   then the peers not attached (EHB_ERR_STATE).
+ * - The index's wide-beam scratch (ehb_index_search_beam) is grown for this nq and beam before the epoch advances,
+ *   so an allocation failure returns EHB_ERR_OOM with this rank still in phase.  OOM is local to the rank: the
+ *   peers' merges of that step still wait for it and time out (ehb_exchange_timed_out).  A step that grows the
+ *   scratch synchronises `stream` and frees the old buffer, which waits for the whole device; on a device shared by
+ *   several ranks of one process, size the scratch (one ehb_index_search_beam_dev of the largest nq and beam) before
+ *   the first fused step, since that wait would include a peer's merge waiting for this rank.
+ * - Memory: the receive buffer is 2 * world * max_nq * max_k * 12 bytes per rank (7.9 GB at world 8, max_nq 10k,
+ *   max_k 4096). */
+int ehb_exchange_search_beam_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const float* queries_dev, uint32_t k,
+                                 uint32_t ef, int precision, float* out_dists_dev, uint64_t* out_labels_dev,
+                                 uint32_t* out_counts_dev, uint32_t* shard_counts_dev, void* stream);
+int ehb_exchange_search_by_label_beam_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const uint64_t* labels_host,
+                                          uint32_t k, uint32_t ef, int precision, float* out_dists_dev,
+                                          uint64_t* out_labels_dev, uint32_t* out_counts_dev, void* stream);
 int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out /* 1: a wait for a peer gave up (~20 s) */);
 
 /* Named integer options (A/B switches and construction knobs that are not part of
