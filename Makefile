@@ -9,6 +9,7 @@ OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(SRCS))
 LIB       := embeddinghub_b200/libehb200.so
 
 all: $(LIB) oracle tests/cpp/ann_index_cases tests/cpp/concurrent_search tests/cpp/sharded_two_dev tests/cpp/rwlock_stress \
+     tests/cpp/exchange_layout \
      tests/cpp/libbf16_probe.so tests/cpp/libi8_probe.so tests/cpp/ann_index_bf16 tests/cpp/ann_index_by_key
 
 # test-only extern "C" wrappers around the K3 launchers of the shipped library (run by tests/test_gpu_bf16_gemm.py)
@@ -40,6 +41,10 @@ tests/cpp/concurrent_search: tests/cpp/concurrent_search.c include/ehb200.h $(LI
 # host-only stress test of the reader/writer lock (run by tests/test_abi_cpu.py; no GPU needed)
 tests/cpp/rwlock_stress: tests/cpp/rwlock_stress.cu $(CSRC)/index_impl.h
 	$(NVCC) $(ARCH) -O2 -std=c++17 --expt-relaxed-constexpr $< -o $@ -lpthread
+
+# host-only check of the shard exchange's buffer layout (run by tests/test_exchange_layout_cpu.py; no GPU needed)
+tests/cpp/exchange_layout: tests/cpp/exchange_layout.cu $(CSRC)/exchange_layout.cuh
+	$(NVCC) $(ARCH) -O2 -std=c++17 --expt-relaxed-constexpr -Xcompiler -Wall $< -o $@
 
 # n_dev = 2 through the C ABI (run by tests/test_gpu_round2.py)
 tests/cpp/sharded_two_dev: tests/cpp/sharded_two_dev.c include/ehb200.h $(LIB)

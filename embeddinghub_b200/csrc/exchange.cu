@@ -18,6 +18,7 @@
 //    buffering so consecutive steps need no barrier.
 #include <thread>
 
+#include "exchange_layout.cuh"
 #include "index_impl.h"
 #include "merge.cuh"
 
@@ -25,29 +26,55 @@ using ehb::fail;
 
 namespace ehb {
 
-constexpr uint32_t kMaxWorld = 16;
-constexpr uint32_t kMaxSlices = 256;
-
-struct ExchangeView {
-  unsigned char* recv[kMaxWorld];  // recv buffer of every rank as mapped HERE ([2][world][stride])
-  uint32_t* flags[kMaxWorld];      // flag array of every rank ([2][world][kMaxSlices])
-  uint32_t world, rank;
-  uint64_t stride;                 // bytes per rank block
+// Every rank's exported allocation as mapped HERE, and its layout (exchange_layout.cuh).
+struct PeerView {
+  unsigned char* base[kMaxWorld];
+  uint32_t rank;
+  ExchangeLayout L;
 };
+
+// The end of slice s's push: every thread's stores are ordered before the slice's flag on every peer.
+__device__ __forceinline__ void publish_slice(const PeerView& v, uint32_t parity, uint32_t epoch, uint32_t s) {
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x < v.L.world && threadIdx.x != v.rank)
+    st_release_sys(v.L.flags(v.base[threadIdx.x], parity, v.rank) + s, epoch);
+  __syncthreads();
+}
+
+// Waits until every peer has raised slice s's flag.  Bounded (~20 s): a peer that never arrives must not wedge the
+// GPU, so the wait gives up, sets the timeout word the host reads, and returns true (in the threads that gave up).
+__device__ __forceinline__ bool await_slice(const PeerView& v, uint32_t parity, uint32_t epoch, uint32_t s,
+                                            uint32_t* timeout_word) {
+  bool gave_up = false;
+  if (threadIdx.x < v.L.world && threadIdx.x != v.rank) {
+    const uint32_t* f = v.L.flags(v.base[v.rank], parity, threadIdx.x) + s;
+    uint32_t spins = 0;
+    while (ld_acquire_sys(f) != epoch) {
+      __nanosleep(64);
+      if (++spins > (1u << 28)) {
+        atomicExch(timeout_word, 1u);
+        gave_up = true;
+        break;
+      }
+    }
+  }
+  __syncthreads();
+  return gave_up;
+}
 
 // One persistent launch per rank and step; grid <= resident capacity so no CTA waits on an unscheduled one.
 // 1024 threads per CTA: the push is a plain copy and the merge is one latency-bound warp per query, so both
 // want as many warps per SM as one resident CTA can hold.
 constexpr uint32_t kExchangeThreads = 1024;
-__global__ void __launch_bounds__(kExchangeThreads) exchange_merge_kernel(ExchangeView ev, uint32_t parity, uint32_t epoch,
+__global__ void __launch_bounds__(kExchangeThreads) exchange_merge_kernel(PeerView v, uint32_t parity, uint32_t epoch,
                                                              uint64_t nq, uint32_t k, uint32_t qs, uint32_t nslices,
                                                              float* __restrict__ out_dists,
                                                              uint64_t* __restrict__ out_labels,
                                                              uint32_t* __restrict__ out_counts,
                                                              uint32_t* __restrict__ timeout_flag, uint32_t skip_push) {
-  const uint32_t W = ev.world, me = ev.rank;
-  const uint64_t blk = ((uint64_t)parity * W + me) * ev.stride;  // my block inside ANY rank's buffer
-  const unsigned char* mine = ev.recv[me] + blk;                 // written by my search kernels
+  const uint32_t W = v.L.world, me = v.rank;
+  const unsigned char* mine = v.L.recv(v.base[me], parity, me);  // written by my search kernels
   const uint64_t lab_bytes = nq * k * 8ull;
   // ---- phase 1: push my slices to every peer, then raise their flags ------------------------------------
   // (skipped when the producer was the one-warp walk: its epilogue already stored every query's results into
@@ -59,52 +86,25 @@ __global__ void __launch_bounds__(kExchangeThreads) exchange_merge_kernel(Exchan
     const float* src_d = (const float*)(mine + lab_bytes);
     for (uint32_t g = 0; g < W; ++g) {
       if (g == me) continue;
-      uint64_t* dst_l = (uint64_t*)(ev.recv[g] + blk);
-      float* dst_d = (float*)(ev.recv[g] + blk + lab_bytes);
+      unsigned char* dst = v.L.recv(v.base[g], parity, me);
+      uint64_t* dst_l = (uint64_t*)dst;
+      float* dst_d = (float*)(dst + lab_bytes);
       for (uint64_t i = e0 + threadIdx.x; i < e1; i += blockDim.x) dst_l[i] = src_l[i];
       for (uint64_t i = e0 + threadIdx.x; i < e1; i += blockDim.x) dst_d[i] = src_d[i];
     }
-    __threadfence_system();  // every thread's stores are ordered before the flags below
-    __syncthreads();
-    if (threadIdx.x < W && threadIdx.x != me)
-      st_release_sys(ev.flags[threadIdx.x] + ((uint64_t)parity * W + me) * kMaxSlices + s, epoch);
-    __syncthreads();
+    publish_slice(v, parity, epoch, s);
   }
   // ---- phase 2: wait for each slice from every peer, merge its queries -------------------------------------
-  const unsigned char* base = ev.recv[me] + (uint64_t)parity * W * ev.stride;
+  const unsigned char* base = v.L.recv(v.base[me], parity, 0);
   const uint32_t warps = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (uint32_t s = blockIdx.x; s < nslices; s += gridDim.x) {
-    if (threadIdx.x < W && threadIdx.x != me) {
-      const uint32_t* f = ev.flags[me] + ((uint64_t)parity * W + threadIdx.x) * kMaxSlices + s;
-      // bounded (~20 s): a peer that never arrives must not wedge the GPU; the host reports the flag
-      uint32_t spins = 0;
-      while (ld_acquire_sys(f) != epoch) {
-        __nanosleep(64);
-        if (++spins > (1u << 28)) {
-          atomicExch(timeout_flag, 1u);
-          break;
-        }
-      }
-    }
-    __syncthreads();
+    await_slice(v, parity, epoch, s, timeout_flag);
     const uint64_t q0 = (uint64_t)s * qs, q1 = min(nq, q0 + qs);
     for (uint64_t q = q0 + w; q < q1; q += warps)
-      merge_one_query(W, q, lane, k, (const float*)(base + lab_bytes), (const uint64_t*)base, ev.stride, ev.stride,
+      merge_one_query(W, q, lane, k, (const float*)(base + lab_bytes), (const uint64_t*)base, v.L.stride, v.L.stride,
                       out_dists, out_labels, out_counts);
   }
 }
-
-// The query rows of a by-label step (ehb_exchange_search_by_label_ex_dev) in every rank's exported block, as mapped
-// HERE.  All parity-indexed like the receive buffer.
-struct RowView {
-  float* rows[kMaxWorld];           // [2][row_stride]: a step of dimension dim uses [nq][dim] of its parity
-  unsigned char* marks[kMaxWorld];  // [2][world][max_nq]: marks[p][g][q] = 1 when rank g holds query q's label
-  uint64_t* digests[kMaxWorld];     // [2][world]: each rank's digest of its label list
-  uint32_t* flags[kMaxWorld];       // the flag array of the receive buffer
-  uint32_t world, rank;
-  uint64_t row_stride;              // floats per parity (a multiple of 64)
-  uint64_t max_nq;
-};
 
 // Bits of the verdict word of a row step.  Every rank reads the same digests, so kRowsDigest is set on every rank or on
 // none; when it is clear every rank was given the same list and reads the same marks, so the whole word is equal.
@@ -113,25 +113,25 @@ constexpr uint32_t kRowsShared = 2;    // a query that more than one rank holds
 constexpr uint32_t kRowsDigest = 4;    // a peer's label list differs from this rank's
 constexpr uint32_t kRowsTimeout = 8;   // a peer never raised its flags (the timeout word is set too)
 
-// One persistent launch per rank (grid sized like exchange_merge_kernel).  Phase 1: every query this rank holds
-// (ids[q] != kInvalid) has its stored row copied from vecs (dpad stride) into row q of every rank's row region, this
-// rank's own included: one warp per row, each 16-byte chunk read once and stored to every destination.  The whole
-// mark vector and (with slice 0) the digest go to every rank too; then the slice flags, released at system scope.
-// Phase 2: wait for every peer's slice flags, count each query's holders over the ranks, compare the digests, and OR
-// the outcome into the local verdict word (zeroed before the launch).
-__global__ void __launch_bounds__(kExchangeThreads) exchange_rows_kernel(RowView v, uint32_t parity, uint32_t epoch,
+// The row step of a by-label search (ehb_exchange_search_by_label_ex_dev); one persistent launch per rank (grid sized
+// like exchange_merge_kernel).  Phase 1: every query this rank holds (ids[q] != kInvalid) has its stored row copied
+// from vecs (dpad stride) into row q of every rank's row region, this rank's own included: one warp per row, each
+// 16-byte chunk read once and stored to every destination.  The whole mark vector and (with slice 0) the digest go to
+// every rank too; then the slice flags, released at system scope.  Phase 2: wait for every peer's slice flags, count
+// each query's holders over the ranks, compare the digests, and OR the outcome into the local verdict word (zeroed
+// before the launch).
+__global__ void __launch_bounds__(kExchangeThreads) exchange_rows_kernel(PeerView v, uint32_t parity, uint32_t epoch,
                                                              uint64_t nq, uint32_t qs, uint32_t nslices,
                                                              const uint32_t* __restrict__ ids,
                                                              const float* __restrict__ vecs, uint32_t dpad,
                                                              uint32_t dim, uint64_t digest,
                                                              uint32_t* __restrict__ verdict,
                                                              uint32_t* __restrict__ timeout_flag) {
-  const uint32_t W = v.world, me = v.rank;
+  const uint32_t W = v.L.world, me = v.rank;
   const uint32_t warps = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // the row region is 256-byte aligned and each parity's part starts a whole number of 64 floats in
-  // (ehb_exchange::row_stride), so a row q * dim floats in is 16-byte aligned when dim is; dpad is a multiple of 4
+  // each parity's part of the row region is 256-byte aligned (exchange_layout.cuh), so a row q * dim floats in is
+  // 16-byte aligned when dim is; dpad is a multiple of 4
   const bool vec4 = (dim & 3) == 0;
-  const uint64_t row0 = (uint64_t)parity * v.row_stride;
   // ---- phase 1: rows, marks and digest to every rank, then the flags ------------------------------------------
   for (uint32_t s = blockIdx.x; s < nslices; s += gridDim.x) {
     const uint64_t q0 = min(nq, (uint64_t)s * qs), q1 = min(nq, q0 + qs);
@@ -139,55 +139,36 @@ __global__ void __launch_bounds__(kExchangeThreads) exchange_rows_kernel(RowView
       const uint32_t id = ids[q];
       if (id == kInvalid) continue;
       const float* src = vecs + (uint64_t)id * dpad;
-      const uint64_t at = row0 + q * dim;
+      const uint64_t at = q * dim;
       if (vec4) {
         for (uint32_t c = lane; c < dim / 4; c += 32) {
           const float4 x = reinterpret_cast<const float4*>(src)[c];
-          for (uint32_t g = 0; g < W; ++g) reinterpret_cast<float4*>(v.rows[g] + at)[c] = x;
+          for (uint32_t g = 0; g < W; ++g) *reinterpret_cast<float4*>(v.L.rows(v.base[g], parity, at + 4 * c)) = x;
         }
       } else {
         for (uint32_t c = lane; c < dim; c += 32) {
           const float x = src[c];
-          for (uint32_t g = 0; g < W; ++g) v.rows[g][at + c] = x;
+          for (uint32_t g = 0; g < W; ++g) *v.L.rows(v.base[g], parity, at + c) = x;
         }
       }
     }
-    const uint64_t mine = ((uint64_t)parity * W + me) * v.max_nq;
     for (uint64_t q = q0 + threadIdx.x; q < q1; q += blockDim.x) {
       const unsigned char held = ids[q] != kInvalid;
-      for (uint32_t g = 0; g < W; ++g) v.marks[g][mine + q] = held;
+      for (uint32_t g = 0; g < W; ++g) v.L.marks(v.base[g], parity, me)[q] = held;
     }
-    if (s == 0 && threadIdx.x < W) v.digests[threadIdx.x][(uint64_t)parity * W + me] = digest;
-    __threadfence_system();  // every thread's stores are ordered before the flags below
-    __syncthreads();
-    if (threadIdx.x < W && threadIdx.x != me)
-      st_release_sys(v.flags[threadIdx.x] + ((uint64_t)parity * W + me) * kMaxSlices + s, epoch);
-    __syncthreads();
+    if (s == 0 && threadIdx.x < W) *v.L.digest(v.base[threadIdx.x], parity, me) = digest;
+    publish_slice(v, parity, epoch, s);
   }
   // ---- phase 2: wait for each slice from every peer, count the holders ---------------------------------------
   for (uint32_t s = blockIdx.x; s < nslices; s += gridDim.x) {
-    if (threadIdx.x < W && threadIdx.x != me) {
-      const uint32_t* f = v.flags[me] + ((uint64_t)parity * W + threadIdx.x) * kMaxSlices + s;
-      uint32_t spins = 0;  // bounded (~20 s), as in exchange_merge_kernel
-      while (ld_acquire_sys(f) != epoch) {
-        __nanosleep(64);
-        if (++spins > (1u << 28)) {
-          atomicExch(timeout_flag, 1u);
-          atomicOr(verdict, kRowsTimeout);
-          break;
-        }
-      }
-    }
-    __syncthreads();
-    uint32_t bits = 0;
+    uint32_t bits = await_slice(v, parity, epoch, s, timeout_flag) ? kRowsTimeout : 0u;
     const uint64_t q0 = min(nq, (uint64_t)s * qs), q1 = min(nq, q0 + qs);
-    const unsigned char* marks = v.marks[me] + (uint64_t)parity * W * v.max_nq;
     for (uint64_t q = q0 + threadIdx.x; q < q1; q += blockDim.x) {
       uint32_t holders = 0;
-      for (uint32_t g = 0; g < W; ++g) holders += marks[(uint64_t)g * v.max_nq + q];
+      for (uint32_t g = 0; g < W; ++g) holders += v.L.marks(v.base[me], parity, g)[q];
       bits |= holders == 0 ? kRowsMissing : holders > 1 ? kRowsShared : 0u;
     }
-    if (s == 0 && threadIdx.x < W && v.digests[me][(uint64_t)parity * W + threadIdx.x] != digest) bits |= kRowsDigest;
+    if (s == 0 && threadIdx.x < W && *v.L.digest(v.base[me], parity, threadIdx.x) != digest) bits |= kRowsDigest;
     if (bits) atomicOr(verdict, bits);
   }
 }
@@ -200,43 +181,42 @@ __global__ void __launch_bounds__(kExchangeThreads) exchange_rows_kernel(RowView
 struct ehb_exchange {
   int device = 0;
   uint32_t world = 1, rank = 0;
-  uint64_t stride = 0, max_elems = 0;
-  unsigned char* local = nullptr;   // [flags (+ timeout word at the end of the flag page) | recv]
-  size_t flag_bytes = 0, total_bytes = 0;
+  ehb::ExchangeLayout L{};  // of the exported allocation, the same on every rank
+  uint64_t max_elems = 0;
+  uint32_t max_dim = 0;
+  ehb::DevBuf<unsigned char> local;  // the exported allocation: ONE, because an IPC handle covers one allocation
   unsigned char* mapped[ehb::kMaxWorld] = {nullptr};  // base of every rank's allocation as mapped here
   bool opened[ehb::kMaxWorld] = {false};
   bool attached = false;
-  uint32_t* slice_count = nullptr;  // [kMaxSlices], zero between steps (raised by the walk's epilogue)
+  ehb::DevBuf<uint32_t> slice_count;  // [kMaxSlices], zero between steps (raised by the walk's epilogue)
   uint32_t same_device_ranks = 1;  // ranks (this one included) whose exchange kernels share this GPU (tests)
   uint32_t epoch = 0;
   uint64_t slot_nq = 0;
   uint32_t slot_k = 0;
   int sms = 132;
   std::mutex mu;
-  // by-label steps (max_dim > 0).  In the exported block, after the receive buffer: the row region, the marks and the
-  // digests (ehb::RowView).  Local scratch: the resolved ids, the query labels, the merged k + 1 lists, the verdict word;
-  // pinned staging of the ids, labels and verdict; `bl_done` ends the last by-label step's use of the scratch.
-  uint64_t max_nq = 0;
-  uint32_t max_dim = 0;
-  size_t rows_off = 0, marks_off = 0, digests_off = 0;
-  uint64_t row_stride = 0;  // floats per parity of the row region: max_nq * max_dim rounded up to a multiple of 64
-  unsigned char* bl = nullptr;
-  uint32_t* bl_ids = nullptr;
-  uint64_t* bl_self = nullptr;
-  uint64_t* bl_labels = nullptr;
-  float* bl_dists = nullptr;
-  uint32_t* bl_counts = nullptr;
-  uint32_t* bl_verdict = nullptr;
-  unsigned char* bl_host = nullptr;  // [max_nq] u64 labels | [max_nq] u32 ids | u32 verdict
+  // by-label steps (max_dim > 0).  Local scratch: the resolved ids, the query labels, the merged k + 1 lists, the
+  // verdict word; pinned staging of the labels, ids and verdict; `bl_done` ends the last by-label step's use of them.
+  ehb::DevBuf<uint32_t> bl_ids, bl_counts, bl_verdict;
+  ehb::DevBuf<uint64_t> bl_self, bl_labels;
+  ehb::DevBuf<float> bl_dists;
+  ehb::PinBuf h_self, h_ids, h_verdict;
   cudaEvent_t bl_done = nullptr;
-};
 
-namespace {
-size_t round256(size_t b) { return (b + 255) / 256 * 256; }
-}  // namespace
+  // Waits for this rank's work and closes the peers' mappings before the buffers free themselves.
+  ~ehb_exchange() {
+    cudaSetDevice(device);
+    cudaDeviceSynchronize();
+    for (uint32_t g = 0; g < world; ++g)
+      if (opened[g]) cudaIpcCloseMemHandle(mapped[g]);
+    if (bl_done) cudaEventDestroy(bl_done);
+  }
+};
 
 extern "C" {
 
+// Everything a step uses is allocated here: a cudaFree inside a step waits for the whole device, which with two ranks
+// on one GPU means a peer's spinning kernel.
 int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64_t max_nq, uint32_t max_k,
                            uint32_t max_dim, ehb_exchange** out) {
   if (!out) return fail(EHB_ERR_INVALID, "null argument");
@@ -249,38 +229,30 @@ int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64
   ex->device = device;
   ex->world = world;
   ex->rank = rank;
+  ex->L = ehb::ExchangeLayout::make(world, max_nq, max_k, max_dim);
   ex->max_elems = max_nq * max_k;
-  ex->stride = (ex->max_elems * 12ull + 255) / 256 * 256;
-  ex->flag_bytes = (2ull * world * ehb::kMaxSlices * 4 + 4 + 4095) / 4096 * 4096;
-  ex->total_bytes = ex->flag_bytes + 2ull * world * ex->stride;
-  ex->max_nq = max_nq;
   ex->max_dim = max_dim;
-  if (max_dim) {
-    ex->row_stride = (max_nq * max_dim + 63) / 64 * 64;
-    ex->rows_off = ex->total_bytes;
-    ex->marks_off = ex->rows_off + round256(2ull * ex->row_stride * 4);
-    ex->digests_off = ex->marks_off + round256(2ull * world * max_nq);
-    ex->total_bytes = ex->digests_off + round256(2ull * world * 8);
-  }
   cudaDeviceGetAttribute(&ex->sms, cudaDevAttrMultiProcessorCount, device);
-  cudaError_t e = cudaMalloc((void**)&ex->local, ex->total_bytes);
-  if (e == cudaSuccess) e = cudaMemset(ex->local, 0, ex->flag_bytes);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&ex->slice_count, ehb::kMaxSlices * 4);
-  if (e == cudaSuccess) e = cudaMemset(ex->slice_count, 0, ehb::kMaxSlices * 4);
-  if (e == cudaSuccess && max_dim) {
-    const size_t ids = round256(max_nq * 4), self = round256(max_nq * 8), labs = round256(ex->max_elems * 8),
-                 dists = round256(ex->max_elems * 4), counts = round256(max_nq * 4);
-    e = cudaMalloc((void**)&ex->bl, ids + self + labs + dists + counts + 256);
-    if (e == cudaSuccess) {
-      unsigned char* p = ex->bl;
-      ex->bl_ids = (uint32_t*)p;
-      ex->bl_self = (uint64_t*)(p += ids);
-      ex->bl_labels = (uint64_t*)(p += self);
-      ex->bl_dists = (float*)(p += labs);
-      ex->bl_counts = (uint32_t*)(p += dists);
-      ex->bl_verdict = (uint32_t*)(p += counts);
-      e = cudaMallocHost((void**)&ex->bl_host, max_nq * 12 + 4);
-    }
+  cudaError_t e = cudaSuccess;
+  auto dev = [&](auto& buf, size_t n, int fill) {
+    if (e == cudaSuccess) e = buf.grow(n, 0, fill, nullptr);
+  };
+  auto pin = [&](ehb::PinBuf& buf, size_t bytes) {
+    if (e == cudaSuccess) e = buf.reserve(bytes);
+  };
+  dev(ex->local, ex->L.total_bytes, -1);
+  if (e == cudaSuccess) e = cudaMemset(ex->local.p, 0, ex->L.flag_bytes);
+  dev(ex->slice_count, ehb::kMaxSlices, 0);
+  if (max_dim) {
+    dev(ex->bl_ids, max_nq, -1);
+    dev(ex->bl_self, max_nq, -1);
+    dev(ex->bl_labels, ex->max_elems, -1);
+    dev(ex->bl_dists, ex->max_elems, -1);
+    dev(ex->bl_counts, max_nq, -1);
+    dev(ex->bl_verdict, 1, -1);
+    pin(ex->h_self, max_nq * 8);
+    pin(ex->h_ids, max_nq * 4);
+    pin(ex->h_verdict, 4);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ex->bl_done, cudaEventDisableTiming);
     // load the step's own kernels now: under lazy module loading a first launch may wait for every kernel running in
     // the context, and with two ranks in one process one of those is a peer's exchange kernel waiting for this rank
@@ -290,15 +262,10 @@ int ehb_exchange_create_ex(int32_t device, uint32_t world, uint32_t rank, uint64
     if (e == cudaSuccess) e = ehb::load_drop_self();
   }
   if (e != cudaSuccess) {
-    if (ex->bl_done) cudaEventDestroy(ex->bl_done);
-    if (ex->bl_host) cudaFreeHost(ex->bl_host);
-    if (ex->bl) cudaFree(ex->bl);
-    if (ex->slice_count) cudaFree(ex->slice_count);
-    if (ex->local) cudaFree(ex->local);
     delete ex;
     return fail(e == cudaErrorMemoryAllocation ? EHB_ERR_OOM : EHB_ERR_CUDA, cudaGetErrorString(e));
   }
-  ex->mapped[rank] = ex->local;
+  ex->mapped[rank] = ex->local.p;
   ex->attached = world == 1;
   *out = ex;
   return EHB_OK;
@@ -310,16 +277,6 @@ int ehb_exchange_create(int32_t device, uint32_t world, uint32_t rank, uint64_t 
 }
 
 int ehb_exchange_destroy(ehb_exchange* ex) {
-  if (!ex) return EHB_OK;
-  cudaSetDevice(ex->device);
-  cudaDeviceSynchronize();
-  for (uint32_t g = 0; g < ex->world; ++g)
-    if (ex->opened[g]) cudaIpcCloseMemHandle(ex->mapped[g]);
-  if (ex->bl_done) cudaEventDestroy(ex->bl_done);
-  if (ex->bl_host) cudaFreeHost(ex->bl_host);
-  if (ex->bl) cudaFree(ex->bl);
-  if (ex->slice_count) cudaFree(ex->slice_count);
-  if (ex->local) cudaFree(ex->local);
   delete ex;
   return EHB_OK;
 }
@@ -329,7 +286,7 @@ int ehb_exchange_ipc_handle(ehb_exchange* ex, void* out_handle) {
   if (!ex || !out_handle) return fail(EHB_ERR_INVALID, "null argument");
   CU(cudaSetDevice(ex->device));
   cudaIpcMemHandle_t h;
-  CU(cudaIpcGetMemHandle(&h, ex->local));
+  CU(cudaIpcGetMemHandle(&h, ex->local.p));
   static_assert(sizeof(cudaIpcMemHandle_t) == EHB_IPC_HANDLE_BYTES, "handle size");
   std::memcpy(out_handle, &h, sizeof(h));
   return EHB_OK;
@@ -366,7 +323,7 @@ int ehb_exchange_attach_local(ehb_exchange* ex, uint32_t peer_rank, ehb_exchange
     cudaGetLastError();
   }
   if (!ex->mapped[peer_rank] && peer->device == ex->device) ex->same_device_ranks++;
-  ex->mapped[peer_rank] = peer->local;
+  ex->mapped[peer_rank] = peer->local.p;
   bool all = true;
   for (uint32_t g = 0; g < ex->world; ++g) all = all && ex->mapped[g] != nullptr;
   ex->attached = all;
@@ -383,7 +340,7 @@ int ehb_exchange_begin(ehb_exchange* ex, uint64_t nq, uint32_t k, uint64_t** lab
   ex->slot_nq = nq;
   ex->slot_k = k;
   const uint32_t parity = ex->epoch & 1u;
-  unsigned char* blk = ex->local + ex->flag_bytes + ((uint64_t)parity * ex->world + ex->rank) * ex->stride;
+  unsigned char* blk = ex->L.recv(ex->local.p, parity, ex->rank);
   *labels_dev = (uint64_t*)blk;
   *dists_dev = (float*)(blk + nq * k * 8ull);
   return EHB_OK;
@@ -402,77 +359,69 @@ void slice_plan(const ehb_exchange* ex, uint64_t nq, uint32_t* qs, uint32_t* nsl
   *nslices = (uint32_t)((nq + per - 1) / per);
 }
 
+// Every rank's mapping of the exported allocation, as the exchange kernels and step_sink read it.
+ehb::PeerView peer_view(const ehb_exchange* ex) {
+  ehb::PeerView v{};
+  std::copy(ex->mapped, ex->mapped + ex->world, v.base);
+  v.rank = ex->rank;
+  v.L = ex->L;
+  return v;
+}
+
+// Every CTA of an exchange kernel must be resident (a waiting CTA may depend on a peer's CTA): one CTA per SM, and
+// when several ranks share this GPU (single-GPU tests) they split the SMs.
+uint32_t resident_grid(const ehb_exchange* ex, uint32_t nslices) {
+  return std::min<uint32_t>(nslices, std::max<uint32_t>(1, (uint32_t)ex->sms / ex->same_device_ranks));
+}
+
 int launch_exchange_merge(ehb_exchange* ex, uint64_t nq, uint32_t k, float* out_dists_dev, uint64_t* out_labels_dev,
                           uint32_t* out_counts_dev, cudaStream_t stream, bool skip_push) {
-  ehb::ExchangeView ev;
-  std::memset(&ev, 0, sizeof(ev));
-  for (uint32_t r = 0; r < ex->world; ++r) {
-    ev.flags[r] = (uint32_t*)ex->mapped[r];
-    ev.recv[r] = ex->mapped[r] + ex->flag_bytes;
-  }
-  ev.world = ex->world;
-  ev.rank = ex->rank;
-  ev.stride = ex->stride;
   uint32_t qs, nslices;
   slice_plan(ex, nq, &qs, &nslices);
-  // every CTA must be resident (a waiting CTA may depend on a peer's CTA): one CTA per SM, and when several ranks
-  // share this GPU (single-GPU tests) they split the SMs
-  uint32_t grid = std::min<uint32_t>(nslices, std::max<uint32_t>(1, (uint32_t)ex->sms / ex->same_device_ranks));
-  ehb::exchange_merge_kernel<<<grid, ehb::kExchangeThreads, 0, stream>>>(
-      ev, ex->epoch & 1u, ex->epoch, nq, k, qs, nslices, out_dists_dev, out_labels_dev, out_counts_dev,
-      (uint32_t*)(ex->local + ex->flag_bytes - 4), skip_push ? 1u : 0u);
+  ehb::exchange_merge_kernel<<<resident_grid(ex, nslices), ehb::kExchangeThreads, 0, stream>>>(
+      peer_view(ex), ex->epoch & 1u, ex->epoch, nq, k, qs, nslices, out_dists_dev, out_labels_dev, out_counts_dev,
+      ex->L.timeout(ex->local.p), skip_push ? 1u : 0u);
   CU(cudaGetLastError());
   return EHB_OK;
 }
 
+static_assert(ehb::kMaxSinks >= ehb::kMaxWorld, "step_sink gives every rank a destination");
+
 // The destinations of this rank's [nq][k] results at the current epoch: its own block of its own buffer first, then
 // its block of every peer's buffer, with the slice flags the search's last kernel raises.
 ehb::ResultSink step_sink(ehb_exchange* ex, uint64_t nq, uint32_t k) {
-  const uint32_t parity = ex->epoch & 1u, W = ex->world, me = ex->rank;
-  const uint64_t blk = ((uint64_t)parity * W + me) * ex->stride;
+  const ehb::PeerView v = peer_view(ex);
+  const uint32_t parity = ex->epoch & 1u, me = ex->rank;
   uint32_t qs, nslices;
   slice_plan(ex, nq, &qs, &nslices);
   ehb::ResultSink sink;
   std::memset(&sink, 0, sizeof(sink));
   uint32_t t = 0;
   auto add = [&](uint32_t r) {
-    unsigned char* base = ex->mapped[r] + ex->flag_bytes + blk;
-    sink.labels[t] = (uint64_t*)base;
-    sink.dists[t] = (float*)(base + nq * k * 8ull);
-    sink.flags[t] = (uint32_t*)ex->mapped[r] + ((uint64_t)parity * W + me) * ehb::kMaxSlices;
+    unsigned char* blk = v.L.recv(v.base[r], parity, me);
+    sink.labels[t] = (uint64_t*)blk;
+    sink.dists[t] = (float*)(blk + nq * k * 8ull);
+    sink.flags[t] = v.L.flags(v.base[r], parity, me);
     ++t;
   };
   add(me);  // destination 0 = my own block of my own buffer
-  for (uint32_t r = 0; r < W; ++r)
+  for (uint32_t r = 0; r < ex->world; ++r)
     if (r != me) add(r);
   sink.n = t;
   sink.qs = qs;
   sink.epoch = ex->epoch;
-  sink.slice_count = ex->slice_count;
+  sink.slice_count = ex->slice_count.p;
   return sink;
 }
 
 // The row step of a by-label search at the current epoch.  Its slice count does not depend on nq (every rank raises
 // the same flags whatever list it was given); the verdict word must be zero on `stream`.
 int launch_exchange_rows(ehb_exchange* ex, const ehb_index* ix, uint64_t nq, uint64_t digest, cudaStream_t stream) {
-  ehb::RowView v;
-  std::memset(&v, 0, sizeof(v));
-  for (uint32_t r = 0; r < ex->world; ++r) {
-    v.rows[r] = (float*)(ex->mapped[r] + ex->rows_off);
-    v.marks[r] = ex->mapped[r] + ex->marks_off;
-    v.digests[r] = (uint64_t*)(ex->mapped[r] + ex->digests_off);
-    v.flags[r] = (uint32_t*)ex->mapped[r];
-  }
-  v.world = ex->world;
-  v.rank = ex->rank;
-  v.row_stride = ex->row_stride;
-  v.max_nq = ex->max_nq;
   const uint32_t nslices = std::min<uint32_t>(ehb::kMaxSlices, (uint32_t)ex->sms);
   const uint32_t qs = (uint32_t)((nq + nslices - 1) / nslices);
-  const uint32_t grid = std::min<uint32_t>(nslices, std::max<uint32_t>(1, (uint32_t)ex->sms / ex->same_device_ranks));
-  ehb::exchange_rows_kernel<<<grid, ehb::kExchangeThreads, 0, stream>>>(
-      v, ex->epoch & 1u, ex->epoch, nq, qs, nslices, ex->bl_ids, ix->vecs.p, ix->dpad, ix->dim, digest, ex->bl_verdict,
-      (uint32_t*)(ex->local + ex->flag_bytes - 4));
+  ehb::exchange_rows_kernel<<<resident_grid(ex, nslices), ehb::kExchangeThreads, 0, stream>>>(
+      peer_view(ex), ex->epoch & 1u, ex->epoch, nq, qs, nslices, ex->bl_ids.p, ix->vecs.p, ix->dpad, ix->dim, digest,
+      ex->bl_verdict.p, ex->L.timeout(ex->local.p));
   CU(cudaGetLastError());
   return EHB_OK;
 }
@@ -570,7 +519,7 @@ static int exchange_by_label_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, 
                          nq, k, k + 1ull, &ef, &none, max_beam));
   if (none) return EHB_OK;
   const uint32_t k1 = k + 1;
-  if (nq > ex->max_nq || nq * k1 > ex->max_elems)
+  if (nq > ex->L.max_nq || nq * k1 > ex->max_elems)
     return fail(EHB_ERR_INVALID, "nq or nq * (k + 1) exceeds the exchange capacity");
   if (ix->dim > ex->max_dim) return fail(EHB_ERR_INVALID, "the exchange has no room for rows of this dim (max_dim)");
   if (!ex->attached) return fail(EHB_ERR_STATE, "peers are not attached yet");
@@ -578,9 +527,9 @@ static int exchange_by_label_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, 
   const cudaStream_t s = (cudaStream_t)stream;
   RET(ix->prepare(lk, false, precision, nq));
   RET(ix->reserve_beam(nq, std::max(ef, k1), precision, s));
-  uint64_t* h_self = (uint64_t*)ex->bl_host;
-  uint32_t* h_ids = (uint32_t*)(h_self + ex->max_nq);
-  uint32_t* h_verdict = h_ids + ex->max_nq;
+  uint64_t* h_self = (uint64_t*)ex->h_self.p;
+  uint32_t* h_ids = (uint32_t*)ex->h_ids.p;
+  uint32_t* h_verdict = (uint32_t*)ex->h_verdict.p;
   // hnswlib getDataByLabel, as ehb_index_get_batch: a tombstoned label is not held
   for (uint64_t q = 0; q < nq; ++q)
     if (!ix->find_id(labels_host[q], &h_ids[q]) || ix->h_deleted[h_ids[q]]) h_ids[q] = ehb::kInvalid;
@@ -588,11 +537,11 @@ static int exchange_by_label_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, 
   CU(cudaStreamWaitEvent(s, ex->bl_done, 0));  // the previous by-label step is done with the scratch
   ex->epoch++;
   const uint32_t parity = ex->epoch & 1u;
-  CU(cudaMemsetAsync(ex->bl_verdict, 0, 4, s));
-  CU(cudaMemcpyAsync(ex->bl_ids, h_ids, nq * 4, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(ex->bl_self, h_self, nq * 8, cudaMemcpyHostToDevice, s));
+  CU(cudaMemsetAsync(ex->bl_verdict.p, 0, 4, s));
+  CU(cudaMemcpyAsync(ex->bl_ids.p, h_ids, nq * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(ex->bl_self.p, h_self, nq * 8, cudaMemcpyHostToDevice, s));
   RET(launch_exchange_rows(ex, ix, nq, label_digest(nq, labels_host), s));
-  CU(cudaMemcpyAsync(h_verdict, ex->bl_verdict, 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h_verdict, ex->bl_verdict.p, 4, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));  // the step's only host synchronisation
   // every rank reads the same verdict and returns the same status; each has consumed epoch e, so they stay in phase.
   // The digests decide first: they are fresh whatever lists the ranks were given, and a digest mismatch is seen by
@@ -603,13 +552,13 @@ static int exchange_by_label_step(ehb_exchange* ex, ehb_index* ix, uint64_t nq, 
   if (v & ehb::kRowsMissing) return fail(EHB_ERR_NOT_FOUND, "label not found on any rank");
   if (v & ehb::kRowsShared) return fail(EHB_ERR_STATE, "a label is stored on more than one rank");
   ex->epoch++;
-  const float* rows = (const float*)(ex->local + ex->rows_off) + parity * ex->row_stride;
+  const float* rows = ex->L.rows(ex->local.p, parity);
   const ehb::ResultSink sink = step_sink(ex, nq, k1);
   bool pushed = false;
   RET(ehb_index_search_dev_sink_held(ix, lk, nq, rows, k1, ef, precision, &sink, nullptr, s, &pushed, max_beam));
   CU(cudaSetDevice(ex->device));
-  RET(launch_exchange_merge(ex, nq, k1, ex->bl_dists, ex->bl_labels, ex->bl_counts, s, pushed));
-  CU(ehb::launch_drop_self(ex->bl_self, ex->bl_labels, ex->bl_dists, ex->bl_counts, nq, k, out_labels_dev,
+  RET(launch_exchange_merge(ex, nq, k1, ex->bl_dists.p, ex->bl_labels.p, ex->bl_counts.p, s, pushed));
+  CU(ehb::launch_drop_self(ex->bl_self.p, ex->bl_labels.p, ex->bl_dists.p, ex->bl_counts.p, nq, k, out_labels_dev,
                            out_dists_dev, out_counts_dev, s));
   CU(cudaEventRecord(ex->bl_done, s));
   return EHB_OK;
@@ -639,7 +588,7 @@ int ehb_exchange_search_dev(ehb_exchange* ex, ehb_index* ix, uint64_t nq, const 
 int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out) {
   if (!ex || !out) return fail(EHB_ERR_INVALID, "null argument");
   CU(cudaSetDevice(ex->device));
-  CU(cudaMemcpy(out, ex->local + ex->flag_bytes - 4, 4, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(out, ex->L.timeout(ex->local.p), 4, cudaMemcpyDeviceToHost));
   return EHB_OK;
 }
 
@@ -648,35 +597,61 @@ int ehb_exchange_timed_out(ehb_exchange* ex, uint32_t* out) {
 // =====================================================================================================
 // ehb_sharded: one process, n_dev GPUs
 // =====================================================================================================
+namespace ehb {
+// One shard of an ehb_sharded: its index, its device, and the stream, event and buffers it searches with.
+struct Shard {
+  ehb_index* ix;
+  int dev;
+  cudaStream_t st = nullptr;
+  cudaEvent_t done = nullptr;
+  DevBuf<float> q_dev;              // the queries
+  DevBuf<unsigned char> local_out;  // [labels | dists] when this device cannot store into device 0
+  DevBuf<uint32_t> cnt_dev;
+  // by-label searches: the gathered rows in owner order and each row's query position
+  DevBuf<float> q_stage;
+  DevBuf<uint32_t> q_pos;
+
+  Shard(ehb_index* ix, int dev) : ix(ix), dev(dev) {}
+  // Waits for the device before anything is freed; the buffers free themselves after, still on this device.
+  ~Shard() {
+    cudaSetDevice(dev);
+    cudaDeviceSynchronize();
+    if (st) cudaStreamDestroy(st);
+    if (done) cudaEventDestroy(done);
+    ehb_index_destroy(ix);
+  }
+};
+}  // namespace ehb
+
 struct ehb_sharded {
-  std::vector<ehb_index*> shard;
-  std::vector<int> dev;
+  std::vector<std::unique_ptr<ehb::Shard>> shards;
   uint64_t span = 0;  // labels per shard range (0: label % n_dev)
   ehb_params prm;
   bool peer_direct = true;  // every device can store into device 0
-  // device-0 gather + result buffers, per-device query staging
+  // device-0 gather + result buffers
   ehb::DevBuf<unsigned char> gather;       // [n_dev][labels | dists]
   ehb::DevBuf<float> m_dists;
   ehb::DevBuf<uint64_t> m_labels;
   ehb::DevBuf<uint32_t> m_counts;
-  std::vector<ehb::DevBuf<float>*> q_dev;   // per device
-  std::vector<ehb::DevBuf<unsigned char>*> local_out;  // per device (no peer access): [labels | dists]
-  std::vector<ehb::DevBuf<uint32_t>*> cnt_dev;
-  // by-label searches: per device, the gathered rows in owner order and each row's query position; on device 0 the
-  // query labels and the results after self-removal
-  std::vector<ehb::DevBuf<float>*> q_stage;
-  std::vector<ehb::DevBuf<uint32_t>*> q_pos;
+  // by-label searches, on device 0: the query labels and the results after self-removal
   ehb::DevBuf<uint64_t> s_self, s_labels;
   ehb::DevBuf<float> s_dists;
   ehb::DevBuf<uint32_t> s_counts;
-  std::vector<cudaStream_t> st;
-  std::vector<cudaEvent_t> done;
   cudaEvent_t q_ready = nullptr;
   std::mutex mu;
   uint64_t next_label = 0;
 
+  // The shards go first; the device-0 buffers free themselves after, on device 0.
+  ~ehb_sharded() {
+    if (shards.empty()) return;
+    const int dev0 = shards[0]->dev;
+    shards.clear();
+    cudaSetDevice(dev0);
+    if (q_ready) cudaEventDestroy(q_ready);
+  }
+
   uint32_t owner(uint64_t label) const {
-    const uint64_t G = shard.size();
+    const uint64_t G = shards.size();
     return (uint32_t)(span ? (label / span) % G : label % G);
   }
 };
@@ -684,31 +659,6 @@ struct ehb_sharded {
 extern "C" {
 
 int ehb_sharded_destroy(ehb_sharded* sh) {
-  if (!sh) return EHB_OK;
-  for (size_t g = 0; g < sh->shard.size(); ++g) {
-    cudaSetDevice(sh->dev[g]);
-    cudaDeviceSynchronize();
-    if (g < sh->st.size() && sh->st[g]) cudaStreamDestroy(sh->st[g]);
-    if (g < sh->done.size() && sh->done[g]) cudaEventDestroy(sh->done[g]);
-    if (g < sh->q_dev.size()) delete sh->q_dev[g];
-    if (g < sh->local_out.size()) delete sh->local_out[g];
-    if (g < sh->cnt_dev.size()) delete sh->cnt_dev[g];
-    if (g < sh->q_stage.size()) delete sh->q_stage[g];
-    if (g < sh->q_pos.size()) delete sh->q_pos[g];
-    ehb_index_destroy(sh->shard[g]);
-  }
-  if (!sh->dev.empty()) {
-    cudaSetDevice(sh->dev[0]);
-    if (sh->q_ready) cudaEventDestroy(sh->q_ready);
-    sh->gather.release();
-    sh->m_dists.release();
-    sh->m_labels.release();
-    sh->m_counts.release();
-    sh->s_self.release();
-    sh->s_labels.release();
-    sh->s_dists.release();
-    sh->s_counts.release();
-  }
   delete sh;
   return EHB_OK;
 }
@@ -730,19 +680,10 @@ int ehb_sharded_create(const ehb_params* p, const int32_t* device_ids, uint32_t 
       pg.device = device_ids[g];
       ehb_index* ix = nullptr;
       RET(ehb_index_create(&pg, &ix));
-      sh->shard.push_back(ix);
-      sh->dev.push_back(device_ids[g]);
-      cudaStream_t s = nullptr;
-      cudaEvent_t e = nullptr;
-      CU(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-      sh->st.push_back(s);
-      CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      sh->done.push_back(e);
-      sh->q_dev.push_back(new ehb::DevBuf<float>());
-      sh->local_out.push_back(new ehb::DevBuf<unsigned char>());
-      sh->cnt_dev.push_back(new ehb::DevBuf<uint32_t>());
-      sh->q_stage.push_back(new ehb::DevBuf<float>());
-      sh->q_pos.push_back(new ehb::DevBuf<uint32_t>());
+      sh->shards.push_back(std::make_unique<ehb::Shard>(ix, device_ids[g]));
+      ehb::Shard& s = *sh->shards.back();
+      CU(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
+      CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
       if (g > 0 && device_ids[g] != device_ids[0]) {  // device g must be able to store into device 0
         int can = 0;
         CU(cudaDeviceCanAccessPeer(&can, device_ids[g], device_ids[0]));
@@ -762,7 +703,7 @@ int ehb_sharded_create(const ehb_params* p, const int32_t* device_ids, uint32_t 
   int rc = body();
   if (rc != EHB_OK) {
     const std::string msg = ehb::last_error_text();
-    ehb_sharded_destroy(sh);
+    delete sh;
     return fail(rc, msg);
   }
   *out = sh;
@@ -771,14 +712,14 @@ int ehb_sharded_create(const ehb_params* p, const int32_t* device_ids, uint32_t 
 
 int ehb_sharded_n_shards(ehb_sharded* sh, uint32_t* out) {
   if (!sh || !out) return fail(EHB_ERR_INVALID, "null argument");
-  *out = (uint32_t)sh->shard.size();
+  *out = (uint32_t)sh->shards.size();
   return EHB_OK;
 }
 
 // Borrow shard i (stats, tuning); owned by the sharded index.
 int ehb_sharded_shard(ehb_sharded* sh, uint32_t i, ehb_index** out) {
-  if (!sh || !out || i >= sh->shard.size()) return fail(EHB_ERR_INVALID, "bad argument");
-  *out = sh->shard[i];
+  if (!sh || !out || i >= sh->shards.size()) return fail(EHB_ERR_INVALID, "bad argument");
+  *out = sh->shards[i]->ix;
   return EHB_OK;
 }
 
@@ -787,7 +728,7 @@ int ehb_sharded_add(ehb_sharded* sh, uint64_t n, const float* vecs, const uint64
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   if (n && !vecs) return fail(EHB_ERR_INVALID, "null vectors");
   std::lock_guard<std::mutex> g(sh->mu);
-  const size_t G = sh->shard.size(), dim = sh->prm.dim;
+  const size_t G = sh->shards.size(), dim = sh->prm.dim;
   std::vector<std::vector<float>> rows(G);
   std::vector<std::vector<uint64_t>> labs(G);
   for (uint64_t i = 0; i < n; ++i) {
@@ -797,7 +738,7 @@ int ehb_sharded_add(ehb_sharded* sh, uint64_t n, const float* vecs, const uint64
     labs[o].push_back(l);
   }
   for (size_t o = 0; o < G; ++o)
-    if (!labs[o].empty()) RET(ehb_index_add(sh->shard[o], labs[o].size(), rows[o].data(), labs[o].data()));
+    if (!labs[o].empty()) RET(ehb_index_add(sh->shards[o]->ix, labs[o].size(), rows[o].data(), labs[o].data()));
   if (!labels) sh->next_label += n;
   return EHB_OK;
 }
@@ -805,20 +746,20 @@ int ehb_sharded_add(ehb_sharded* sh, uint64_t n, const float* vecs, const uint64
 int ehb_sharded_remove(ehb_sharded* sh, uint64_t n, const uint64_t* labels) {
   if (!sh || (n && !labels)) return fail(EHB_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> g(sh->mu);
-  for (uint64_t i = 0; i < n; ++i) RET(ehb_index_remove(sh->shard[sh->owner(labels[i])], 1, labels + i));
+  for (uint64_t i = 0; i < n; ++i) RET(ehb_index_remove(sh->shards[sh->owner(labels[i])]->ix, 1, labels + i));
   return EHB_OK;
 }
 
 int ehb_sharded_get(ehb_sharded* sh, uint64_t label, float* out) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  return ehb_index_get(sh->shard[sh->owner(label)], label, out);
+  return ehb_index_get(sh->shards[sh->owner(label)]->ix, label, out);
 }
 
 int ehb_sharded_size(ehb_sharded* sh, uint64_t* out) {
   if (!sh || !out) return fail(EHB_ERR_INVALID, "null argument");
   uint64_t tot = 0, v = 0;
-  for (ehb_index* ix : sh->shard) {
-    RET(ehb_index_size(ix, &v));
+  for (const auto& s : sh->shards) {
+    RET(ehb_index_size(s->ix, &v));
     tot += v;
   }
   *out = tot;
@@ -829,13 +770,13 @@ int ehb_sharded_size(ehb_sharded* sh, uint64_t* out) {
 static int on_every_shard(ehb_sharded* sh, int (*fn)(ehb_index*)) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   std::lock_guard<std::mutex> g(sh->mu);
-  const size_t G = sh->shard.size();
+  const size_t G = sh->shards.size();
   std::vector<int> rc(G, EHB_OK);
   std::vector<std::string> msg(G);
   std::vector<std::thread> th;
   for (size_t i = 0; i < G; ++i)
     th.emplace_back([&, i]() {
-      rc[i] = fn(sh->shard[i]);
+      rc[i] = fn(sh->shards[i]->ix);
       if (rc[i] != EHB_OK) msg[i] = ehb::last_error_text();
     });
   for (auto& t : th) t.join();
@@ -852,7 +793,7 @@ int ehb_sharded_compact(ehb_sharded* sh) { return on_every_shard(sh, ehb_index_c
 
 int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
-  for (ehb_index* ix : sh->shard) RET(ehb_index_set_ef(ix, ef));
+  for (const auto& s : sh->shards) RET(ehb_index_set_ef(s->ix, ef));
   return EHB_OK;
 }
 
@@ -862,44 +803,46 @@ int ehb_sharded_set_ef(ehb_sharded* sh, uint32_t ef) {
 // block, like the fp32 walk).  beam: ehb_index_search_beam_dev on every shard instead of ehb_index_search_ex_dev.
 static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* q, uint32_t k, uint32_t ef,
                          int precision, bool beam = false) {
-  const uint32_t G = (uint32_t)sh->shard.size();
+  const uint32_t G = (uint32_t)sh->shards.size();
   const uint32_t dim = sh->prm.dim;
   const uint64_t blk = (nq * k * 12ull + 255) / 256 * 256;
-  CU(cudaSetDevice(sh->dev[0]));
-  cudaStream_t s0 = sh->st[0];
+  const int dev0 = sh->shards[0]->dev;
+  CU(cudaSetDevice(dev0));
+  cudaStream_t s0 = sh->shards[0]->st;
   CU(sh->gather.grow(blk * G, 0, -1, s0));
   CU(sh->m_labels.grow(nq * k, 0, -1, s0));
   CU(sh->m_dists.grow(nq * k, 0, -1, s0));
   CU(sh->m_counts.grow(nq, 0, -1, s0));
   CU(cudaEventRecord(sh->q_ready, s0));  // orders the peers' stores after earlier merges on device 0
   for (uint32_t i = 0; i < G; ++i) {
-    CU(cudaSetDevice(sh->dev[i]));
-    cudaStream_t s = sh->st[i];
-    CU(sh->q_dev[i]->grow(nq * dim, 0, -1, s));
-    CU(sh->cnt_dev[i]->grow(nq, 0, -1, s));
-    if (q) CU(cudaMemcpyAsync(sh->q_dev[i]->p, q, nq * dim * 4, cudaMemcpyHostToDevice, s));
+    ehb::Shard& sd = *sh->shards[i];
+    CU(cudaSetDevice(sd.dev));
+    cudaStream_t s = sd.st;
+    CU(sd.q_dev.grow(nq * dim, 0, -1, s));
+    CU(sd.cnt_dev.grow(nq, 0, -1, s));
+    if (q) CU(cudaMemcpyAsync(sd.q_dev.p, q, nq * dim * 4, cudaMemcpyHostToDevice, s));
     unsigned char* dst;
-    if (i == 0 || sh->peer_direct || sh->dev[i] == sh->dev[0]) {
+    if (i == 0 || sh->peer_direct || sd.dev == dev0) {
       dst = sh->gather.p + blk * i;  // device i's kernels store straight into device 0's gather block
       if (i) CU(cudaStreamWaitEvent(s, sh->q_ready, 0));
     } else {
-      CU(sh->local_out[i]->grow(blk, 0, -1, s));
-      dst = sh->local_out[i]->p;
+      CU(sd.local_out.grow(blk, 0, -1, s));
+      dst = sd.local_out.p;
     }
     uint64_t* dl = (uint64_t*)dst;
     float* dd = (float*)(dst + nq * k * 8ull);
     if (brute)
-      RET(ehb_index_search_bruteforce_dev(sh->shard[i], nq, sh->q_dev[i]->p, k, precision, dl, dd, sh->cnt_dev[i]->p, s));
+      RET(ehb_index_search_bruteforce_dev(sd.ix, nq, sd.q_dev.p, k, precision, dl, dd, sd.cnt_dev.p, s));
     else
-      RET((beam ? ehb_index_search_beam_dev : ehb_index_search_ex_dev)(sh->shard[i], nq, sh->q_dev[i]->p, k, ef,
-                                                                       precision, dl, dd, sh->cnt_dev[i]->p, s));
-    CU(cudaSetDevice(sh->dev[i]));
-    if (i && !sh->peer_direct && sh->dev[i] != sh->dev[0])
-      CU(cudaMemcpyPeerAsync(sh->gather.p + blk * i, sh->dev[0], dst, sh->dev[i], nq * k * 12ull, s));
-    CU(cudaEventRecord(sh->done[i], s));
+      RET((beam ? ehb_index_search_beam_dev : ehb_index_search_ex_dev)(sd.ix, nq, sd.q_dev.p, k, ef, precision, dl, dd,
+                                                                       sd.cnt_dev.p, s));
+    CU(cudaSetDevice(sd.dev));
+    if (i && !sh->peer_direct && sd.dev != dev0)
+      CU(cudaMemcpyPeerAsync(sh->gather.p + blk * i, dev0, dst, sd.dev, nq * k * 12ull, s));
+    CU(cudaEventRecord(sd.done, s));
   }
-  CU(cudaSetDevice(sh->dev[0]));
-  for (uint32_t i = 1; i < G; ++i) CU(cudaStreamWaitEvent(s0, sh->done[i], 0));
+  CU(cudaSetDevice(dev0));
+  for (uint32_t i = 1; i < G; ++i) CU(cudaStreamWaitEvent(s0, sh->shards[i]->done, 0));
   CU(ehb::launch_merge_topk(G, nq, k, (const float*)(sh->gather.p + nq * k * 8ull), (const uint64_t*)sh->gather.p, blk,
                             blk, sh->m_dists.p, sh->m_labels.p, sh->m_counts.p, s0));
   return EHB_OK;
@@ -909,7 +852,8 @@ static int sharded_merge(ehb_sharded* sh, bool brute, uint64_t nq, const float* 
 // resolves and checks it again under its own lock).  max_beam: the graph walk's width limit (512, or kMaxBeam).
 static int check_shards(ehb_sharded* sh, bool brute, int precision, bool null_buf, uint64_t nq, uint32_t k,
                         uint64_t k_walk, uint32_t ef, bool* none, uint32_t max_beam = ehb::kMaxEf) {
-  for (ehb_index* ix : sh->shard) {
+  for (const auto& s : sh->shards) {
+    ehb_index* ix = s->ix;
     std::shared_lock<ehb::RwLock> lk(ix->rw);
     uint32_t ef_shard = ef;
     RET(ehb::check_request(ix, brute, precision, null_buf, nq, k, k_walk, brute ? nullptr : &ef_shard, none,
@@ -927,8 +871,8 @@ static int sharded_search(ehb_sharded* sh, bool brute, uint64_t nq, const float*
   if (none) return EHB_OK;
   std::lock_guard<std::mutex> g(sh->mu);
   RET(sharded_merge(sh, brute, nq, q, k, ef, precision, beam));
-  RET(ehb::copy_results(nq, k, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, ol, od, oc, sh->st[0]));
-  CU(cudaStreamSynchronize(sh->st[0]));
+  RET(ehb::copy_results(nq, k, sh->m_labels.p, sh->m_dists.p, sh->m_counts.p, ol, od, oc, sh->shards[0]->st));
+  CU(cudaStreamSynchronize(sh->shards[0]->st));
   return EHB_OK;
 }
 
@@ -952,7 +896,7 @@ int ehb_sharded_search_beam(ehb_sharded* sh, uint64_t nq, const float* q, uint32
 int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, float* out) {
   if (!sh) return fail(EHB_ERR_INVALID, "null handle");
   if (n && (!labels || !out)) return fail(EHB_ERR_INVALID, "null buffer");
-  const size_t G = sh->shard.size(), dim = sh->prm.dim;
+  const size_t G = sh->shards.size(), dim = sh->prm.dim;
   std::vector<std::vector<uint64_t>> labs(G), pos(G);
   for (uint64_t i = 0; i < n; ++i) {
     const uint32_t o = sh->owner(labels[i]);
@@ -963,7 +907,7 @@ int ehb_sharded_get_batch(ehb_sharded* sh, uint64_t n, const uint64_t* labels, f
   for (size_t o = 0; o < G; ++o) {
     if (labs[o].empty()) continue;
     rows[o].resize(labs[o].size() * dim);
-    RET(ehb_index_get_batch(sh->shard[o], labs[o].size(), labs[o].data(), rows[o].data()));
+    RET(ehb_index_get_batch(sh->shards[o]->ix, labs[o].size(), labs[o].data(), rows[o].data()));
   }
   for (size_t o = 0; o < G; ++o)
     for (size_t j = 0; j < pos[o].size(); ++j)
@@ -984,7 +928,7 @@ static int sharded_by_label(ehb_sharded* sh, uint64_t nq, const uint64_t* labels
   if (none) return EHB_OK;
   const uint32_t k1 = k + 1;
   std::lock_guard<std::mutex> g(sh->mu);
-  const uint32_t G = (uint32_t)sh->shard.size();
+  const uint32_t G = (uint32_t)sh->shards.size();
   const uint32_t dim = sh->prm.dim;
   std::vector<std::vector<uint64_t>> labs(G);
   std::vector<uint32_t> order;  // query position of each staging row
@@ -1002,35 +946,36 @@ static int sharded_by_label(ehb_sharded* sh, uint64_t nq, const uint64_t* labels
       order.insert(order.end(), pos[o].begin(), pos[o].end());
     }
   }
-  for (uint32_t i = 0; i < G; ++i) {
-    CU(cudaSetDevice(sh->dev[i]));
-    CU(sh->q_stage[i]->grow(nq * dim, 0, -1, sh->st[i]));
-    CU(sh->q_pos[i]->grow(nq, 0, -1, sh->st[i]));
-    CU(sh->q_dev[i]->grow(nq * dim, 0, -1, sh->st[i]));
+  for (const auto& sd : sh->shards) {
+    CU(cudaSetDevice(sd->dev));
+    CU(sd->q_stage.grow(nq * dim, 0, -1, sd->st));
+    CU(sd->q_pos.grow(nq, 0, -1, sd->st));
+    CU(sd->q_dev.grow(nq * dim, 0, -1, sd->st));
   }
   for (uint32_t o = 0; o < G; ++o) {
     if (labs[o].empty()) continue;
+    const ehb::Shard& so = *sh->shards[o];
     const uint64_t m = labs[o].size();
-    float* rows = sh->q_stage[o]->p + first[o] * dim;
-    RET(ehb_index_gather_dev(sh->shard[o], m, labs[o].data(), rows, sh->st[o]));
-    CU(cudaSetDevice(sh->dev[o]));
+    float* rows = so.q_stage.p + first[o] * dim;
+    RET(ehb_index_gather_dev(so.ix, m, labs[o].data(), rows, so.st));
+    CU(cudaSetDevice(so.dev));
     for (uint32_t i = 0; i < G; ++i)
       if (i != o)
-        CU(cudaMemcpyPeerAsync(sh->q_stage[i]->p + first[o] * dim, sh->dev[i], rows, sh->dev[o], m * dim * 4ull,
-                               sh->st[o]));
-    CU(cudaEventRecord(sh->done[o], sh->st[o]));
+        CU(cudaMemcpyPeerAsync(sh->shards[i]->q_stage.p + first[o] * dim, sh->shards[i]->dev, rows, so.dev,
+                               m * dim * 4ull, so.st));
+    CU(cudaEventRecord(so.done, so.st));
   }
   for (uint32_t i = 0; i < G; ++i) {
-    CU(cudaSetDevice(sh->dev[i]));
-    cudaStream_t s = sh->st[i];
+    const ehb::Shard& sd = *sh->shards[i];
+    CU(cudaSetDevice(sd.dev));
     for (uint32_t o = 0; o < G; ++o)
-      if (o != i && !labs[o].empty()) CU(cudaStreamWaitEvent(s, sh->done[o], 0));
-    CU(cudaMemcpyAsync(sh->q_pos[i]->p, order.data(), nq * 4, cudaMemcpyHostToDevice, s));
-    CU(ehb::launch_gather_rows(sh->q_stage[i]->p, dim, nullptr, sh->q_dev[i]->p, dim, sh->q_pos[i]->p, nq, dim, s));
+      if (o != i && !labs[o].empty()) CU(cudaStreamWaitEvent(sd.st, sh->shards[o]->done, 0));
+    CU(cudaMemcpyAsync(sd.q_pos.p, order.data(), nq * 4, cudaMemcpyHostToDevice, sd.st));
+    CU(ehb::launch_gather_rows(sd.q_stage.p, dim, nullptr, sd.q_dev.p, dim, sd.q_pos.p, nq, dim, sd.st));
   }
   RET(sharded_merge(sh, false, nq, nullptr, k1, ef, precision, beam));
-  CU(cudaSetDevice(sh->dev[0]));
-  cudaStream_t s0 = sh->st[0];
+  CU(cudaSetDevice(sh->shards[0]->dev));
+  cudaStream_t s0 = sh->shards[0]->st;
   CU(sh->s_self.grow(nq, 0, -1, s0));
   CU(sh->s_labels.grow(nq * k, 0, -1, s0));
   CU(sh->s_dists.grow(nq * k, 0, -1, s0));
