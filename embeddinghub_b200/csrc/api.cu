@@ -498,6 +498,37 @@ ehb::BuildGraph ehb_index::build_graph() const {
   return bg;
 }
 
+ehb::WalkCfg ehb_index::build_cfg(uint64_t jobs) const {
+  const uint32_t efc = std::max(prm.ef_construction, M);
+  if (efc <= ehb::kMaxRegEfc) return walk_cfg(efc, 256, jobs, 1);
+  // the set and the ordered list the heuristic walks, both in shared memory; the visited table is in HBM; a wider beam
+  // keeps proportionally more tombstoned candidates pending (as the wide-beam walk's plan)
+  ehb::WalkCfg c = walk_cfg(efc, 2u * ehb::align_up(efc, 32), jobs, 1);
+  c.hash_size = 0;
+  if (n_deleted) c.dcap = std::max(ehb::kDeletedQueue, ehb::align_up(efc / 4, 32));
+  return c;
+}
+
+int ehb_index::reserve_build_beam(ehb::BuildBeam* bm) {
+  *bm = ehb::BuildBeam{nullptr, 0, 0};
+  const uint32_t efc = std::max(prm.ef_construction, M);
+  if (efc <= ehb::kMaxRegEfc) return EHB_OK;
+  bm->vsize = ehb::align_up(2u * M0 * efc + 64u, 32);  // walk_cfg's "roomy" table, as the wide-beam walk's
+  // Sized for the form without tombstones, whose footprint is the smaller one, so that the size does not depend on the
+  // tombstones of the moment (a compaction's re-links run after it has dropped them); a launch never uses more warps
+  // than the tables here hold.
+  ehb::BuildGraph bg = build_graph();
+  bg.g.deleted = nullptr;
+  ehb::WalkCfg cfg = build_cfg(1);
+  cfg.dcap = 0;
+  uint32_t warps = 0;
+  CU(ehb::build_beam_warps(bg, cfg, sms, &warps));
+  CU(b_vtab.grow((size_t)warps * bm->vsize, 0, -1, stream));
+  bm->vtab = b_vtab.p;
+  bm->warps = (uint32_t)(b_vtab.n / bm->vsize);
+  return EHB_OK;
+}
+
 int ehb_index::build() {
   if (!needs_build()) return EHB_OK;
   const uint32_t maxb = prm.build_batch ? prm.build_batch : 16384;
@@ -508,8 +539,10 @@ int ehb_index::build() {
     return e;
   };
   RET(ensure_build_scratch((uint64_t)std::min<uint64_t>(maxb, std::max<uint64_t>(n, 1)) * M * 2, 1, false));
+  ehb::BuildBeam bm;
+  RET(reserve_build_beam(&bm));
   CU(cudaMemsetAsync(b_counters.p + 3, 0, 4, stream));  // error flag of earlier builds
-  ehb::WalkCfg cfg = walk_cfg(std::max(prm.ef_construction, M), 256, std::min<uint64_t>(maxb, n), 1);
+  ehb::WalkCfg cfg = build_cfg(std::min<uint64_t>(maxb, n));
   uint32_t wpb = wpb_for(cfg, 256);
   while (n_linked < n) {
     if (n_linked == 0) {
@@ -527,7 +560,7 @@ int ehb_index::build() {
     RET(ensure_build_scratch(edges, 1, false));
     ehb::BuildGraph bg = build_graph();
     ehb::BuildBuffers bb = build_buffers(edges);
-    CU(ehb::launch_build_batch(bg, cfg, nullptr, (uint32_t)n_linked, (uint32_t)b, ehb::kBuildInsert, bb, wpb,
+    CU(ehb::launch_build_batch(bg, cfg, nullptr, (uint32_t)n_linked, (uint32_t)b, ehb::kBuildInsert, bb, wpb, bm,
                                stream));
     for (uint64_t i = n_linked; i < n_linked + b; ++i)
       if ((int)h_levels[i] > max_level) max_level = h_levels[i], entry = (uint32_t)i;
@@ -568,7 +601,7 @@ int ehb_index::build() {
         CU(cudaMemcpyAsync(b_ids.p, ups.data() + off, (size_t)b * 4, cudaMemcpyHostToDevice, stream));
         ehb::BuildGraph bg = build_graph();
         ehb::BuildBuffers bb = build_buffers(edges);
-        CU(ehb::launch_build_batch(bg, cfg, b_ids.p, 0, b, ehb::kBuildUpdate, bb, wpb, stream));
+        CU(ehb::launch_build_batch(bg, cfg, b_ids.p, 0, b, ehb::kBuildUpdate, bb, wpb, bm, stream));
       }
       CU(cudaStreamSynchronize(stream));
     }
@@ -658,6 +691,8 @@ int ehb_index::compact() {
   const uint64_t stage_rows = std::max<uint64_t>(1, std::min<uint64_t>(nn, (256ull << 20) / (dpad * 4ull)));
   const uint32_t warps = std::min<uint32_t>(std::max<uint32_t>(nrows, 1), ehb::kRepairWarps);
   RET(ensure_build_scratch(0, warps, true));
+  ehb::BuildBeam bm;  // (the re-links of step 5)
+  RET(reserve_build_beam(&bm));
   CU(repaired.grow(std::max<uint64_t>(nrows, 1) * M0, 0, -1, s));
   CU(d_remap.grow(n_old, 0, -1, s));
   CU(d_inv.grow(nn, 0, -1, s));
@@ -672,8 +707,8 @@ int ehb_index::compact() {
     ehb::BuildGraph bg = build_graph();
     ehb::BuildBuffers bb = build_buffers(0);
     bb.repair_out = repaired.p;
-    const ehb::WalkCfg cfg = walk_cfg(bg.efc, 256, warps, 1);
-    CU(ehb::launch_build_batch(bg, cfg, rows.p, 0, nrows, ehb::kBuildRepair, bb, wpb_for(cfg, 256), s));
+    const ehb::WalkCfg cfg = build_cfg(warps);
+    CU(ehb::launch_build_batch(bg, cfg, rows.p, 0, nrows, ehb::kBuildRepair, bb, wpb_for(cfg, 256), bm, s));
     CU(ehb::launch_compact_apply(rows.p, nrows, repaired.p, links0.p, links_up.p, M0, M, (uint32_t)cap, s));
   }
   // 4. renumber the adjacency into the new arrays, find the orphans, move the vectors
@@ -1216,7 +1251,7 @@ int ehb_index_create(const ehb_params* p, ehb_index** out) {
   if (!p || !out) return fail(EHB_ERR_INVALID, "null argument");
   if (p->dim == 0 || p->dim > ehb::kMaxDim) return fail(EHB_ERR_INVALID, "dim must be in 1..4096");
   if (p->M < 2 || p->M > 16) return fail(EHB_ERR_INVALID, "M must be in 2..16");
-  if (p->ef_construction > 256) return fail(EHB_ERR_INVALID, "ef_construction must be <= 256");
+  if (p->ef_construction > ehb::kMaxBeam) return fail(EHB_ERR_INVALID, "ef_construction must be <= 4096");
   if (p->metric < 0 || p->metric > 2) return fail(EHB_ERR_INVALID, "unknown metric");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);

@@ -18,16 +18,23 @@
 //     does one edge at a time.
 // Results are deterministic: candidates are ordered by (distance, id) before
 // any selection, so atomic arrival order never matters.
-// The kernels are in build_impl.cuh, instantiated per row shape in build_inst_*.cu.
+// The kernels are in build_impl.cuh, instantiated per row shape in build_inst_*.cu (ef_construction <= 256) and
+// build_inst_beam_*.cu (the wide form, up to 4096).
 #include "kernels.h"
 
 namespace ehb {
 
 cudaError_t launch_build_batch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
-                               uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
+                               uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, const BuildBeam& bm,
+                               cudaStream_t s) {
   if (b == 0) return cudaSuccess;
-  return with_dpad(bg.g.dpad,
-                   [&](auto d) { return BuildShape<decltype(d)::value>::launch(bg, cfg, ids, first, b, mode, bb, wpb, s); });
+  return with_dpad(bg.g.dpad, [&](auto d) {
+    return BuildShape<decltype(d)::value>::launch(bg, cfg, ids, first, b, mode, bb, wpb, bm, s);
+  });
+}
+
+cudaError_t build_beam_warps(const BuildGraph& bg, const WalkCfg& cfg, int sms, uint32_t* warps) {
+  return with_dpad(bg.g.dpad, [&](auto d) { return BuildBeamShape<decltype(d)::value>::warps(bg, cfg, sms, warps); });
 }
 
 }  // namespace ehb

@@ -203,6 +203,108 @@ __global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCf
   }
 }
 
+// The wide form's result sets are the shared-memory SList of the wide-beam walk (walk.cuh).  Its key list holds
+// 2 L keys (cfg.lcap = 2 L, L = align_up(set capacity, 32)): the ordered list that heuristic_select and
+// list_remove_id read in keys[0, L), the set in keys[L, 2 L).
+__device__ __forceinline__ void set_init(SList& u, const WarpCtx& c) {
+  const uint32_t L = c.lcap / 2u;
+  u.hi = (uint32_t*)(c.keys + L);
+  u.id = u.hi + L;
+  u.C = L / 32u;
+}
+// Empties the set (UList: the register form; SList: the wide form, set_init) into c.keys[0..c.cnt) in ascending
+// (distance, id) order: the list the selection heuristic walks.
+template <int KPL>
+__device__ __forceinline__ void set_to_list(WarpCtx& c, UList<KPL>& u) {
+  ul_extract_all<KPL>(c, u);
+}
+__device__ __forceinline__ void set_to_list(WarpCtx& c, SList& u) {
+  sl_begin_extract(u, c.lane);
+  c.cnt = 0;
+  for (;;) {
+    const uint64_t key = sl_take_min(u, true, c.lane);
+    if (key == kMaxKey) break;
+    if (c.lane == 0) c.keys[c.cnt] = key;
+    c.cnt++;
+  }
+  __syncwarp();
+}
+
+// Phase A for one point p in the wide form: build_search_kernel's body over the SList (the register kernel keeps its
+// own copy, so that its code stays as it was).
+template <int LPV, int NQ, bool HASDEL>
+__device__ __forceinline__ void link_point(WarpCtx& c, const Aux& a, const BuildGraph& bg, uint32_t p, int is_update,
+                                           const BuildBuffers& bb) {
+  const GraphView& g = bg.g;
+  float4 qr[NQ];
+  load_row_query<LPV, NQ>(c, qr, g, p);
+  SList ul;
+  set_init(ul, c);
+  WalkCounters wc = {0, 0, 0, 0};
+  const int level_p = bg.levels[p];
+  const int top = g.max_level;
+  uint32_t cur = g.entry;
+  if (c.lane == 0) c.cand_id[0] = cur;
+  __syncwarp();
+  eval_candidates<LPV, NQ>(c, g.vecs, qr, 1, g.metric);
+  float curdist = c.cand_dist[0];
+  __syncwarp();
+  if (level_p < top) greedy_descent<LPV, NQ>(c, g, qr, cur, curdist, top, level_p, wc);
+  uint32_t* links0 = const_cast<uint32_t*>(g.links0);
+  uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
+  for (int level = min(level_p, top); level >= 0; --level) {
+    beam_search<LPV, NQ, 0, false, HASDEL, 1, float, false, SList>(c, g, qr, ul, cur, curdist, level, bg.efc, kInvalid,
+                                                                   wc);
+    set_to_list(c, ul);
+    if (is_update) list_remove_id(c, p);
+    if (c.cnt == 0) continue;
+    uint32_t nsel = heuristic_select<LPV, NQ>(c, g, g.M, a);
+    if constexpr (wide_shape(LPV, NQ))
+      if (level > 0) load_row_query<LPV, NQ>(c, qr, g, p);  // the selection replaced the shared-memory query
+    uint32_t width = level == 0 ? g.M0 : g.M;
+    uint32_t* row = level == 0 ? links0 + (size_t)p * g.M0 : links_up + (size_t)(g.up_off[p] + level - 1) * g.M;
+    if (is_update) {
+      // other warps of the wave may still walk this row: stage it, it lands before phase C
+      const uint32_t rid = level == 0 ? p : bg.cap + g.up_off[p] + (uint32_t)(level - 1);
+      row = stage_row(bb, rid, g.M0, c.lane);
+    }
+    if (c.lane < width) row[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
+    uint32_t base = 0;
+    if (c.lane == 0) base = atomicAdd(bb.edge_count, nsel);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (base + nsel > bb.edge_cap) {
+      if (c.lane == 0) atomicExch(bb.error_flag, 1u);
+    } else if (c.lane < nsel) {
+      uint32_t t = a.sel_id[c.lane];
+      bb.edge_row[base + c.lane] = level == 0 ? t : bg.cap + g.up_off[t] + (uint32_t)(level - 1);
+      bb.edge_src[base + c.lane] = p;
+      bb.edge_dist[base + c.lane] = a.sel_dist[c.lane];
+    }
+    cur = key_id(c.keys[0]);
+    curdist = key_dist(c.keys[0]);
+    __syncwarp();
+  }
+}
+
+// The wide form of phase A (efc > kMaxRegEfc): a persistent grid of one-warp blocks; warp w links points w, w + W, ...
+// of the wave, so the scratch depends on the resident warps, not on the wave (up to 16384 points).  The result set is
+// the shared-memory SList of the wide-beam walk (L = align_up(efc, 32) keys, the ordered list beside it: set_init), the
+// visited table warp w's slice of vsize entries of vtab in HBM.  Every point reads the pre-wave graph and its edge
+// records go through phases B and C as in the register form, so the schedule cannot change the result.
+template <int LPV, int NQ, bool HASDEL>
+__global__ void __launch_bounds__(32, 1)
+    build_search_beam_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ ids, uint32_t first, uint32_t b,
+                             int is_update, BuildBuffers bb, uint32_t vsize, uint32_t* __restrict__ vtab) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  WarpCtx c;
+  ctx_init(c, smem + 256, cfg, bg.g.dpad);
+  c.hash = vtab + (size_t)blockIdx.x * vsize;
+  c.hsize = vsize;
+  Aux a = aux_of(c);
+  for (uint32_t pi = blockIdx.x; pi < b; pi += gridDim.x)
+    link_point<LPV, NQ, HASDEL>(c, a, bg, ids ? ids[pi] : first + pi, is_update, bb);
+}
+
 // Adds one id per lane (kInvalid = none; the ids of one call are distinct) to the candidate set cand[0..ncand),
 // deduplicated through the visited table.  A probe-budget overflow falls back to a linear scan of what is
 // stored, so the set is exact.
@@ -223,14 +325,15 @@ __device__ __forceinline__ void cand_add(WarpCtx& c, uint32_t* cand, uint32_t& n
 
 // The keep-then-select step of hnswlib updatePoint for one row: the `keep` members of cand[0..ncand) closest
 // to `owner` (owner itself skipped), ordered by (distance, id), then the heuristic with Mmax.  The selected
-// ids are left in a.sel_id; returns their number.
-template <int LPV, int NQ, int KPL>
-__device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g, const Aux& a, const uint32_t* cand,
-                                                 uint32_t ncand, uint32_t owner, uint32_t keep, uint32_t Mmax) {
+// ids are left in a.sel_id; returns their number.  u holds the `keep`: UList<8> in the register form, the
+// shared-memory SList (up to kUpdCandCap - 1) in the wide form.
+template <int LPV, int NQ, class Set>
+__device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g, const Aux& a, Set& u,
+                                                 const uint32_t* cand, uint32_t ncand, uint32_t owner, uint32_t keep,
+                                                 uint32_t Mmax) {
   float4 qr[NQ];
   load_row_query<LPV, NQ>(c, qr, g, owner);
-  UList<KPL> u;
-  ul_clear<KPL>(u, keep, c.lane);
+  ul_clear(u, keep, c.lane);
   uint32_t cnt = 0, worst_hi = 0xFFFFFFFFu;
   for (uint32_t b0 = 0; b0 < ncand; b0 += 32) {
     uint32_t id = b0 + c.lane < ncand ? cand[b0 + c.lane] : kInvalid;
@@ -251,10 +354,10 @@ __device__ __forceinline__ uint32_t reselect_row(WarpCtx& c, const GraphView& g,
       uint32_t hj = __shfl_sync(0xffffffffu, myhi, l);
       uint32_t ij = __shfl_sync(0xffffffffu, myid, l);
       if (cnt >= keep && hj >= worst_hi) continue;
-      ul_insert<KPL>(u, hj, ij, keep, cnt, worst_hi, c.lane);
+      ul_insert(u, hj, ij, keep, cnt, worst_hi, c.lane);
     }
   }
-  ul_extract_all<KPL>(c, u);
+  set_to_list(c, u);
   return heuristic_select<LPV, NQ>(c, g, Mmax, a);
 }
 
@@ -280,19 +383,11 @@ static __global__ void update_tag_kernel(GraphView g, const uint8_t* __restrict_
   }
 }
 
-template <int LPV, int NQ, int KPL>
-__global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, WalkCfg cfg,
-                                                               const uint32_t* __restrict__ ids, uint32_t b,
-                                                               BuildBuffers bb, uint32_t warp_smem) {
-  extern __shared__ __align__(128) unsigned char smem[];
+// One moved point pi (= ids[pi] in the wave) with the warp's context; u holds the keep list (set_init done).
+template <int LPV, int NQ, class Set>
+__device__ __forceinline__ void update_point(WarpCtx& c, const Aux& a, Set& u, const BuildGraph& bg, uint32_t pi,
+                                             uint32_t p, const BuildBuffers& bb) {
   const GraphView& g = bg.g;
-  const uint32_t w = threadIdx.x >> 5;
-  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
-  if (pi >= b) return;
-  const uint32_t p = ids[pi];
-  WarpCtx c;
-  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
-  Aux a = aux_of(c);
   uint32_t* cand = bb.upd_cand + (size_t)pi * kUpdCandCap;
   const int level_p = min((int)bg.levels[p], g.max_level);
   for (int layer = 0; layer <= level_p; ++layer) {
@@ -315,12 +410,46 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
       const uint32_t rid = layer == 0 ? nbid : bg.cap + g.up_off[nbid] + (uint32_t)(layer - 1);
       if (bb.row_fill[rid] != pi + 1u) continue;  // a later moved point of this wave re-selects this row
       // nb is always a member of sCand
-      const uint32_t nsel = reselect_row<LPV, NQ, KPL>(c, g, a, cand, ncand, nbid, min(bg.efc, ncand - 1u), Mmax);
+      const uint32_t nsel = reselect_row<LPV, NQ>(c, g, a, u, cand, ncand, nbid, min(bg.efc, ncand - 1u), Mmax);
       uint32_t* row = stage_row(bb, rid, g.M0, c.lane);
       if (c.lane < Mmax) row[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
       __syncwarp();
     }
   }
+}
+
+template <int LPV, int NQ, int KPL>
+__global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, WalkCfg cfg,
+                                                               const uint32_t* __restrict__ ids, uint32_t b,
+                                                               BuildBuffers bb, uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t w = threadIdx.x >> 5;
+  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
+  if (pi >= b) return;
+  const uint32_t p = ids[pi];
+  WarpCtx c;
+  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, bg.g.dpad);
+  Aux a = aux_of(c);
+  UList<KPL> u;
+  update_point<LPV, NQ>(c, a, u, bg, pi, p, bb);
+}
+
+// The wide form's update re-selection (efc > kMaxRegEfc): the keep list (up to kUpdCandCap - 1) in an SList of
+// cfg.lcap / 2 keys beside its ordered list (set_init).  One warp per block and per moved point.
+template <int LPV, int NQ>
+__global__ void __launch_bounds__(32, 1) update_neighbors_wide_kernel(BuildGraph bg, WalkCfg cfg,
+                                                                      const uint32_t* __restrict__ ids, uint32_t b,
+                                                                      BuildBuffers bb, uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  (void)warp_smem;
+  const uint32_t pi = blockIdx.x;
+  if (pi >= b) return;
+  WarpCtx c;
+  ctx_init(c, smem + 256, cfg, bg.g.dpad);
+  Aux a = aux_of(c);
+  SList u;
+  set_init(u, c);
+  update_point<LPV, NQ>(c, a, u, bg, pi, ids[pi], bb);
 }
 
 // Compaction repair (ehb_index_compact): the row of a live node p at layer l that names deleted points is
@@ -330,19 +459,11 @@ __global__ void __launch_bounds__(128) update_neighbors_kernel(BuildGraph bg, Wa
 // neighbour's row.  Every warp reads the pre-compaction graph and writes its result to bb.repair_out
 // ([b][M0], kInvalid padded), so the outcome does not depend on scheduling.  rows[] holds row ids in the
 // edge_row convention (< cap: level-0 row of that node; >= cap: upper row - cap).  One warp per row.
-template <int LPV, int NQ, int KPL>
-__global__ void __launch_bounds__(128) repair_rows_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ rows,
-                                                          uint32_t b, BuildBuffers bb, uint32_t warp_smem) {
-  extern __shared__ __align__(128) unsigned char smem[];
+template <int LPV, int NQ, class Set>
+__device__ __forceinline__ void repair_row(WarpCtx& c, const Aux& a, Set& u, const BuildGraph& bg, uint32_t pi,
+                                           uint32_t r, const BuildBuffers& bb) {
   const GraphView& g = bg.g;
-  const uint32_t w = threadIdx.x >> 5;
-  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
-  if (pi >= b) return;
-  WarpCtx c;
-  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
-  Aux a = aux_of(c);
   uint32_t* cand = bb.upd_cand + (size_t)pi * kUpdCandCap;
-  const uint32_t r = rows[pi];
   uint32_t p = r, layer = 0;
   if (r >= bg.cap) {
     p = bg.up_owner[r - bg.cap];
@@ -359,9 +480,40 @@ __global__ void __launch_bounds__(128) repair_rows_kernel(BuildGraph bg, WalkCfg
     cand_add(c, cand, ncand, two == kInvalid || two == p || g.deleted[two] ? kInvalid : two);
   }
   const uint32_t nsel =
-      ncand ? reselect_row<LPV, NQ, KPL>(c, g, a, cand, ncand, p, min(bg.efc, ncand), layer ? g.M : g.M0) : 0u;
+      ncand ? reselect_row<LPV, NQ>(c, g, a, u, cand, ncand, p, min(bg.efc, ncand), layer ? g.M : g.M0) : 0u;
   uint32_t* out = bb.repair_out + (size_t)pi * g.M0;
   if (c.lane < g.M0) out[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
+}
+
+template <int LPV, int NQ, int KPL>
+__global__ void __launch_bounds__(128) repair_rows_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ rows,
+                                                          uint32_t b, BuildBuffers bb, uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t w = threadIdx.x >> 5;
+  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
+  if (pi >= b) return;
+  WarpCtx c;
+  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, bg.g.dpad);
+  Aux a = aux_of(c);
+  UList<KPL> u;
+  repair_row<LPV, NQ>(c, a, u, bg, pi, rows[pi], bb);
+}
+
+// The wide form's compaction repair: keep min(efc, |C|) in an SList, as update_neighbors_wide_kernel.
+template <int LPV, int NQ>
+__global__ void __launch_bounds__(32, 1) repair_rows_wide_kernel(BuildGraph bg, WalkCfg cfg,
+                                                                 const uint32_t* __restrict__ rows, uint32_t b,
+                                                                 BuildBuffers bb, uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  (void)warp_smem;
+  const uint32_t pi = blockIdx.x;
+  if (pi >= b) return;
+  WarpCtx c;
+  ctx_init(c, smem + 256, cfg, bg.g.dpad);
+  Aux a = aux_of(c);
+  SList u;
+  set_init(u, c);
+  repair_row<LPV, NQ>(c, a, u, bg, pi, rows[pi], bb);
 }
 
 static __global__ void edge_count_kernel(BuildBuffers bb) {
@@ -506,9 +658,13 @@ static cudaError_t apply_staged(const BuildGraph& bg, const BuildBuffers& bb, cu
 
 template <uint32_t DPAD>
 cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
-                                     uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s) {
+                                     uint32_t b, int mode, BuildBuffers& bb, uint32_t wpb, const BuildBeam& bm,
+                                     cudaStream_t s) {
   constexpr int LPV = row_lpv(DPAD * 4u), NQ = row_nq(DPAD, DPAD * 4u);
-  constexpr int KPL = 8;  // ef_construction <= 256
+  constexpr int KPL = 8;  // the register form: ef_construction <= kMaxRegEfc
+  // the wide form (efc > kMaxRegEfc): shared-memory sets, the search's visited tables in bm.vtab
+  const bool beam = bg.efc > kMaxRegEfc;
+  if (beam && (!bm.vtab || bm.warps == 0 || bm.vsize == 0)) return cudaErrorInvalidValue;
   cudaError_t e;
   const bool is_update = mode == kBuildUpdate;
   if (mode == kBuildUpdate || mode == kBuildRepair) {
@@ -516,9 +672,12 @@ cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, c
     // the two-hop candidate sets are deduplicated through a visited table of >= 4096 entries
     WalkCfg ucfg = cfg;
     if (ucfg.hash_size < 4096) ucfg.hash_size = 4096;
-    uint32_t uwsm = build_warp_smem(ucfg, bg.g.dpad), uwpb = wpb;
+    // the wide form keeps up to min(efc, kUpdCandCap - 1) candidates in an SList beside their ordered list
+    if (beam) ucfg.lcap = 2u * align_up(min(bg.efc, kUpdCandCap), 32);
+    uint32_t uwsm = build_warp_smem(ucfg, bg.g.dpad), uwpb = beam ? 1u : wpb;  // the wide kernels: one warp per block
     while (uwpb > 1 && (size_t)uwsm * uwpb > 200 * 1024) uwpb >>= 1;
-    auto ku = mode == kBuildUpdate ? update_neighbors_kernel<LPV, NQ, KPL> : repair_rows_kernel<LPV, NQ, KPL>;
+    auto ku = beam ? BuildBeamShape<DPAD>::rows(mode)
+                   : (mode == kBuildUpdate ? update_neighbors_kernel<LPV, NQ, KPL> : repair_rows_kernel<LPV, NQ, KPL>);
     if ((e = cudaFuncSetAttribute(ku, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)uwsm * uwpb))) !=
         cudaSuccess)
       return e;
@@ -555,11 +714,18 @@ cudaError_t BuildShape<DPAD>::launch(const BuildGraph& bg, const WalkCfg& cfg, c
   while (msmem > 200 * 1024 && mwpb > 1) mwpb >>= 1, msmem = (size_t)mwsm * mwpb;
   dim3 grid((b + wpb - 1) / wpb), block(32 * wpb);
   uint32_t ethreads = bb.edge_cap;
-  auto ks = bg.g.deleted ? build_search_kernel<LPV, NQ, KPL, true> : build_search_kernel<LPV, NQ, KPL, false>;
   auto km = merge_rows_kernel<LPV, NQ>;
-  if ((e = cudaFuncSetAttribute(ks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(km, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem)) != cudaSuccess) return e;
-  ks<<<grid, block, smem, s>>>(bg, cfg, ids, first, b, is_update ? 1 : 0, bb, wsm);
+  if (beam) {
+    // one warp per block, at most one per visited-table slice
+    const BuildSearchBeamKernel kb = BuildBeamShape<DPAD>::search(bg.g.deleted != nullptr);
+    if ((e = cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm)) != cudaSuccess) return e;
+    kb<<<min(b, bm.warps), 32, wsm, s>>>(bg, cfg, ids, first, b, is_update ? 1 : 0, bb, bm.vsize, bm.vtab);
+  } else {
+    auto ks = bg.g.deleted ? build_search_kernel<LPV, NQ, KPL, true> : build_search_kernel<LPV, NQ, KPL, false>;
+    if ((e = cudaFuncSetAttribute(ks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+    ks<<<grid, block, smem, s>>>(bg, cfg, ids, first, b, is_update ? 1 : 0, bb, wsm);
+  }
   edge_count_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);
   edge_alloc_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);
   edge_scatter_kernel<<<(ethreads + 255) / 256, 256, 0, s>>>(bb);

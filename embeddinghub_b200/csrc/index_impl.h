@@ -318,6 +318,9 @@ struct ehb_index {
   ehb::DevBuf<uint32_t> b_edge_row, b_edge_src, b_row_cnt, b_row_fill, b_row_start, b_touched, b_seg_src, b_counters,
       b_ids, b_upd_cand, b_side_row, b_side_out;
   ehb::DevBuf<float> b_edge_dist, b_seg_dist, b_stage_in;
+  // the wide construction form's visited tables (ef_construction > 256): one HBM slice per resident warp of its
+  // persistent grid (reserve_build_beam)
+  ehb::DevBuf<uint32_t> b_vtab;
 
   // tuning (0 = auto)
   uint32_t t_slots = 0, t_groups = 0, t_hash_bits = 0, t_wpb = 0, t_team = 0;
@@ -356,6 +359,12 @@ struct ehb_index {
   int ensure_build_scratch(uint64_t edges, uint32_t batch, bool updates);
   ehb::BuildBuffers build_buffers(uint64_t edges);
   ehb::BuildGraph build_graph() const;
+  // the search configuration of a build launch of `jobs` warps: walk_cfg's register form for efc <= kMaxRegEfc, else
+  // the wide form's (launch_build_batch)
+  ehb::WalkCfg build_cfg(uint64_t jobs) const;
+  // Grows b_vtab for the wide form's persistent grid and describes it in *bm (all zero for efc <= kMaxRegEfc).  Called
+  // before the graph is touched, so that running out of memory (EHB_ERR_OOM) leaves the index as it was.
+  int reserve_build_beam(ehb::BuildBeam* bm);
   int build();
   int compact();
   bool needs_build() const { return n_linked != n || !pending_updates.empty(); }

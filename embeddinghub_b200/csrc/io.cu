@@ -298,7 +298,7 @@ int ehb_index_load(const char* path, int32_t device, ehb_index** out) {
     if (std::fread(&p, sizeof(p), 1, f) != 1 || std::fread(hdr, 8, 6, f) != 6) return fail(EHB_ERR_IO, "bad header");
     const uint64_t n = hdr[0], rows = hdr[1];
     if (p.dim == 0 || p.dim > ehb::kMaxDim || p.M < 2 || p.M > 16 || p.metric < 0 || p.metric > 2 ||
-        p.ef_construction > 256 || n >= 0x7FFFFFFFull || rows > n * 31ull || hdr[5] >= (1ull << 40))
+        p.ef_construction > ehb::kMaxBeam || n >= 0x7FFFFFFFull || rows > n * 31ull || hdr[5] >= (1ull << 40))
       return fail(EHB_ERR_IO, "corrupt header");
     struct stat st;
     if (fstat(fileno(f), &st) != 0 || (uint64_t)st.st_size != file_bytes(p, n, rows))

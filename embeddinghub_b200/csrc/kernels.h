@@ -10,6 +10,7 @@ namespace ehb {
 constexpr uint32_t kMaxDim = 4096;  // pad_dim() supports rows up to 4096 floats
 constexpr uint32_t kMaxEf = 512;    // register-resident list: 16 keys per lane
 constexpr uint32_t kMaxBeam = 4096; // wide-beam walk (WalkForm::beam): shared-memory list, visited table in HBM
+constexpr uint32_t kMaxRegEfc = 256;    // construction beam in the register set (UList<8>); wider: K5's wide form
 constexpr uint32_t kUpdCandCap = 1088;  // update path: sCand capacity per moved point, >= 1 + 32 + 32*32
 constexpr uint32_t kRepairWarps = 8192; // compaction repair: warps of the persistent grid (upd_cand slots)
 
@@ -183,13 +184,39 @@ enum BuildMode : int {
   kBuildUpdate = 1,  // hnswlib updatePoint of the already linked points ids[0..b)
   kBuildRepair = 2,  // compaction: re-select the rows ids[0..b) (row ids as edge_row) into bb.repair_out
 };
+// The wide form of K5 (bg.efc > kMaxRegEfc): its construction search runs as a persistent grid of one-warp blocks,
+// each with a visited table of vsize = align_up(2 M0 efc + 64, 32) entries in vtab, which holds `warps` of them.  The
+// launch uses min(b, warps) warps.  Unused (all zero) in the register form.
+struct BuildBeam {
+  uint32_t* vtab;
+  uint32_t vsize;
+  uint32_t warps;
+};
+// cfg: walk_cfg's for the search; in the wide form lcap = 2 align_up(efc, 32) (the set and its ordered list),
+// hash_size = 0 and, with tombstones, dcap = max(kDeletedQueue, align_up(efc / 4, 32)).
 cudaError_t launch_build_batch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first,
-                               uint32_t b, int mode, BuildBuffers& bb, uint32_t warps_per_block, cudaStream_t s);
+                               uint32_t b, int mode, BuildBuffers& bb, uint32_t warps_per_block, const BuildBeam& bm,
+                               cudaStream_t s);
+// The resident warps of the wide form's construction search for cfg and the tombstone state of bg.g, on sms SMs
+// (cudaErrorInvalidConfiguration when not even one fits an SM).
+cudaError_t build_beam_warps(const BuildGraph& bg, const WalkCfg& cfg, int sms, uint32_t* warps);
 // K5 for rows of DPAD floats (build_impl.cuh; instantiated per shape in build_inst_*.cu)
 template <uint32_t DPAD>
 struct BuildShape {
   static cudaError_t launch(const BuildGraph& bg, const WalkCfg& cfg, const uint32_t* ids, uint32_t first, uint32_t b,
-                            int mode, BuildBuffers& bb, uint32_t wpb, cudaStream_t s);
+                            int mode, BuildBuffers& bb, uint32_t wpb, const BuildBeam& bm, cudaStream_t s);
+};
+// The wide form's kernels for rows of DPAD floats (build_impl.cuh; instantiated per shape in build_inst_beam_*.cu):
+// the construction search (with or without tombstones) and the update / repair re-selection (rows(kBuildUpdate) or
+// rows(kBuildRepair)) with its keep list in shared memory.
+using BuildSearchBeamKernel = void (*)(BuildGraph, WalkCfg, const uint32_t*, uint32_t, uint32_t, int, BuildBuffers,
+                                       uint32_t, uint32_t*);
+using BuildRowsKernel = void (*)(BuildGraph, WalkCfg, const uint32_t*, uint32_t, BuildBuffers, uint32_t);
+template <uint32_t DPAD>
+struct BuildBeamShape {
+  static BuildSearchBeamKernel search(bool hasdel);
+  static BuildRowsKernel rows(int mode);
+  static cudaError_t warps(const BuildGraph& bg, const WalkCfg& cfg, int sms, uint32_t* out);
 };
 
 // K6 — compaction (ehb_index_compact).  Row ids follow the edge_row convention: < cap a level-0 row, >= cap an

@@ -66,7 +66,8 @@ typedef struct ehb_params {
   int32_t metric;           /* ehb_metric                                      */
   uint64_t capacity;        /* initial capacity in vectors; grows by doubling  */
   uint32_t M;               /* 2..16 (level-0 rows hold 2*M ids)               */
-  uint32_t ef_construction;
+  uint32_t ef_construction; /* 0 (= 200) .. 4096, EHB_ERR_INVALID above; the
+                               build searches at max(ef_construction, M)      */
   uint32_t ef_search;       /* default ef of searches (hnswlib ef_)            */
   uint64_t seed;            /* level generator seed                            */
   int32_t device;           /* CUDA device ordinal                             */
