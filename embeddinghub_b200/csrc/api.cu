@@ -138,6 +138,14 @@ ehb::WalkCfg ehb_index::walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t j
   return c;
 }
 
+ehb::WalkCfg ehb_index::beam_cfg(uint32_t ef, uint32_t smem_list, uint64_t jobs, bool bf16) const {
+  ehb::WalkCfg c = walk_cfg(ef, smem_list, jobs, 1, bf16);
+  c.hash_size = 0;
+  // tombstoned candidates wait in the side queue; a wider beam keeps proportionally more of them pending
+  if (n_deleted) c.dcap = std::max(ehb::kDeletedQueue, ehb::align_up(ef / 4, 32));
+  return c;
+}
+
 uint32_t ehb_index::wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16) const {
   uint32_t w = t_wpb ? t_wpb : 1;
   while (w > 1 && (size_t)(ehb::warp_smem_bytes(c, dpad, bf16 ? 2u : 4u) + extra) * w > 220 * 1024) w >>= 1;
@@ -162,16 +170,12 @@ ehb::WalkPlan ehb_index::walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) cons
   // speculative expansions only add work (C5 shape, Q=10k).
   if (ef_eff > ehb::kMaxEf) {  // the wide-beam walk: result set in shared memory, visited table in HBM
     p.kpl = 0;
-    p.hasdel = n_deleted != 0;
     p.T = 1;
     p.U = 0;
     p.form = ehb::WalkForm::beam;
     p.screen = false;
-    p.cfg = walk_cfg(ef_eff, ehb::align_up(ef_eff, 32), nq, 1, bf16);
-    p.cfg.hash_size = 0;
-    // tombstoned candidates wait in the side queue; a wider beam keeps proportionally more of them pending
-    if (n_deleted) p.cfg.dcap = std::max(ehb::kDeletedQueue, ehb::align_up(ef_eff / 4, 32));
-    p.vtab = ehb::align_up(2u * M0 * ef_eff + 64u, 32);  // walk_cfg's "roomy" table
+    p.cfg = beam_cfg(ef_eff, ehb::align_up(ef_eff, 32), nq, bf16);
+    p.vtab = beam_vtab_size(ef_eff);
     p.wpb = 1;
     return p;
   }
@@ -501,19 +505,14 @@ ehb::BuildGraph ehb_index::build_graph() const {
 ehb::WalkCfg ehb_index::build_cfg(uint64_t jobs) const {
   const uint32_t efc = std::max(prm.ef_construction, M);
   if (efc <= ehb::kMaxRegEfc) return walk_cfg(efc, 256, jobs, 1);
-  // the set and the ordered list the heuristic walks, both in shared memory; the visited table is in HBM; a wider beam
-  // keeps proportionally more tombstoned candidates pending (as the wide-beam walk's plan)
-  ehb::WalkCfg c = walk_cfg(efc, 2u * ehb::align_up(efc, 32), jobs, 1);
-  c.hash_size = 0;
-  if (n_deleted) c.dcap = std::max(ehb::kDeletedQueue, ehb::align_up(efc / 4, 32));
-  return c;
+  return beam_cfg(efc, 2u * ehb::align_up(efc, 32), jobs);  // the set and the ordered list the heuristic walks
 }
 
 int ehb_index::reserve_build_beam(ehb::BuildBeam* bm) {
   *bm = ehb::BuildBeam{nullptr, 0, 0};
   const uint32_t efc = std::max(prm.ef_construction, M);
   if (efc <= ehb::kMaxRegEfc) return EHB_OK;
-  bm->vsize = ehb::align_up(2u * M0 * efc + 64u, 32);  // walk_cfg's "roomy" table, as the wide-beam walk's
+  bm->vsize = beam_vtab_size(efc);
   // Sized for the form without tombstones, whose footprint is the smaller one, so that the size does not depend on the
   // tombstones of the moment (a compaction's re-links run after it has dropped them); a launch never uses more warps
   // than the tables here hold.

@@ -99,13 +99,10 @@ cudaError_t BeamShape<DPAD, RowT>::warps(const WalkPlan& p, int sms, uint64_t nq
   uint32_t smem = 0;
   const BeamKernel kern = beam_kernel<DPAD, RowT>(p, &smem);
   if (!kern) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  int per_sm = 0;
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32, smem);
-  if (e != cudaSuccess) return e;
-  if (per_sm < 1) return cudaErrorInvalidConfiguration;
-  *out = (uint32_t)std::min<uint64_t>(nq, (uint64_t)per_sm * (uint64_t)sms);
-  return cudaSuccess;
+  uint32_t resident = 0;
+  const cudaError_t e = resident_warps((const void*)kern, smem, sms, &resident);
+  if (e == cudaSuccess) *out = (uint32_t)std::min<uint64_t>(nq, resident);
+  return e;
 }
 
 template <uint32_t DPAD, class RowT>

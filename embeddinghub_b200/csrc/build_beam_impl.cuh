@@ -18,15 +18,7 @@ BuildRowsKernel BuildBeamShape<DPAD>::rows(int mode) {
 }
 template <uint32_t DPAD>
 cudaError_t BuildBeamShape<DPAD>::warps(const BuildGraph& bg, const WalkCfg& cfg, int sms, uint32_t* out) {
-  const BuildSearchBeamKernel kern = search(bg.g.deleted != nullptr);
-  const uint32_t smem = build_warp_smem(cfg, DPAD);
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  int per_sm = 0;
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32, smem);
-  if (e != cudaSuccess) return e;
-  if (per_sm < 1) return cudaErrorInvalidConfiguration;
-  *out = (uint32_t)per_sm * (uint32_t)sms;
-  return cudaSuccess;
+  return resident_warps((const void*)search(bg.g.deleted != nullptr), build_warp_smem(cfg, DPAD), sms, out);
 }
 
 }  // namespace ehb

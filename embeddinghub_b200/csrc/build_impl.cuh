@@ -142,67 +142,6 @@ static __global__ void apply_staged_kernel(BuildBuffers bb, uint32_t* links0, ui
   if (j == 0) bb.row_fill[rid] = 0u;
 }
 
-template <int LPV, int NQ, int KPL, bool HASDEL>
-__global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ ids,
-                                                           uint32_t first, uint32_t b, int is_update, BuildBuffers bb,
-                                                           uint32_t warp_smem) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  const GraphView& g = bg.g;
-  const uint32_t w = threadIdx.x >> 5;
-  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
-  if (pi >= b) return;
-  const uint32_t p = ids ? ids[pi] : first + pi;
-  WarpCtx c;
-  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
-  Aux a = aux_of(c);
-  float4 qr[NQ];
-  load_row_query<LPV, NQ>(c, qr, g, p);
-  UList<KPL> ul;
-  WalkCounters wc = {0, 0, 0, 0};
-  const int level_p = bg.levels[p];
-  const int top = g.max_level;
-  uint32_t cur = g.entry;
-  if (c.lane == 0) c.cand_id[0] = cur;
-  __syncwarp();
-  eval_candidates<LPV, NQ>(c, g.vecs, qr, 1, g.metric);
-  float curdist = c.cand_dist[0];
-  __syncwarp();
-  if (level_p < top) greedy_descent<LPV, NQ>(c, g, qr, cur, curdist, top, level_p, wc);
-  uint32_t* links0 = const_cast<uint32_t*>(g.links0);
-  uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
-  for (int level = min(level_p, top); level >= 0; --level) {
-    beam_search<LPV, NQ, KPL, false, HASDEL>(c, g, qr, ul, cur, curdist, level, bg.efc, kInvalid, wc);
-    ul_extract_all<KPL>(c, ul);  // the list the selection heuristic walks
-    if (is_update) list_remove_id(c, p);
-    if (c.cnt == 0) continue;
-    uint32_t nsel = heuristic_select<LPV, NQ>(c, g, g.M, a);
-    if constexpr (wide_shape(LPV, NQ))
-      if (level > 0) load_row_query<LPV, NQ>(c, qr, g, p);  // the selection replaced the shared-memory query
-    uint32_t width = level == 0 ? g.M0 : g.M;
-    uint32_t* row = level == 0 ? links0 + (size_t)p * g.M0 : links_up + (size_t)(g.up_off[p] + level - 1) * g.M;
-    if (is_update) {
-      // other warps of the wave may still walk this row: stage it, it lands before phase C
-      const uint32_t rid = level == 0 ? p : bg.cap + g.up_off[p] + (uint32_t)(level - 1);
-      row = stage_row(bb, rid, g.M0, c.lane);
-    }
-    if (c.lane < width) row[c.lane] = c.lane < nsel ? a.sel_id[c.lane] : kInvalid;
-    uint32_t base = 0;
-    if (c.lane == 0) base = atomicAdd(bb.edge_count, nsel);
-    base = __shfl_sync(0xffffffffu, base, 0);
-    if (base + nsel > bb.edge_cap) {
-      if (c.lane == 0) atomicExch(bb.error_flag, 1u);
-    } else if (c.lane < nsel) {
-      uint32_t t = a.sel_id[c.lane];
-      bb.edge_row[base + c.lane] = level == 0 ? t : bg.cap + g.up_off[t] + (uint32_t)(level - 1);
-      bb.edge_src[base + c.lane] = p;
-      bb.edge_dist[base + c.lane] = a.sel_dist[c.lane];
-    }
-    cur = key_id(c.keys[0]);
-    curdist = key_dist(c.keys[0]);
-    __syncwarp();
-  }
-}
-
 // The wide form's result sets are the shared-memory SList of the wide-beam walk (walk.cuh).  Its key list holds
 // 2 L keys (cfg.lcap = 2 L, L = align_up(set capacity, 32)): the ordered list that heuristic_select and
 // list_remove_id read in keys[0, L), the set in keys[L, 2 L).
@@ -212,6 +151,10 @@ __device__ __forceinline__ void set_init(SList& u, const WarpCtx& c) {
   u.id = u.hi + L;
   u.C = L / 32u;
 }
+// Readies a freshly declared set: the register form's needs nothing, the wide form's points into the key list.
+template <int KPL>
+__device__ __forceinline__ void set_begin(UList<KPL>&, const WarpCtx&) {}
+__device__ __forceinline__ void set_begin(SList& u, const WarpCtx& c) { set_init(u, c); }
 // Empties the set (UList: the register form; SList: the wide form, set_init) into c.keys[0..c.cnt) in ascending
 // (distance, id) order: the list the selection heuristic walks.
 template <int KPL>
@@ -230,16 +173,16 @@ __device__ __forceinline__ void set_to_list(WarpCtx& c, SList& u) {
   __syncwarp();
 }
 
-// Phase A for one point p in the wide form: build_search_kernel's body over the SList (the register kernel keeps its
-// own copy, so that its code stays as it was).
-template <int LPV, int NQ, bool HASDEL>
+// Phase A for one point p: search, select, write p's own rows, emit the reverse-edge records.  Set is the result set:
+// UList<KPL> in the register form, the shared-memory SList (KPL = 0) in the wide form.
+template <int LPV, int NQ, int KPL, bool HASDEL, class Set>
 __device__ __forceinline__ void link_point(WarpCtx& c, const Aux& a, const BuildGraph& bg, uint32_t p, int is_update,
                                            const BuildBuffers& bb) {
   const GraphView& g = bg.g;
   float4 qr[NQ];
   load_row_query<LPV, NQ>(c, qr, g, p);
-  SList ul;
-  set_init(ul, c);
+  Set ul;
+  set_begin(ul, c);
   WalkCounters wc = {0, 0, 0, 0};
   const int level_p = bg.levels[p];
   const int top = g.max_level;
@@ -253,7 +196,7 @@ __device__ __forceinline__ void link_point(WarpCtx& c, const Aux& a, const Build
   uint32_t* links0 = const_cast<uint32_t*>(g.links0);
   uint32_t* links_up = const_cast<uint32_t*>(g.links_up);
   for (int level = min(level_p, top); level >= 0; --level) {
-    beam_search<LPV, NQ, 0, false, HASDEL, 1, float, false, SList>(c, g, qr, ul, cur, curdist, level, bg.efc, kInvalid,
+    beam_search<LPV, NQ, KPL, false, HASDEL, 1, float, false, Set>(c, g, qr, ul, cur, curdist, level, bg.efc, kInvalid,
                                                                    wc);
     set_to_list(c, ul);
     if (is_update) list_remove_id(c, p);
@@ -286,6 +229,23 @@ __device__ __forceinline__ void link_point(WarpCtx& c, const Aux& a, const Build
   }
 }
 
+// The register form of phase A (efc <= kMaxRegEfc): one warp per point of the wave.
+template <int LPV, int NQ, int KPL, bool HASDEL>
+__global__ void __launch_bounds__(128) build_search_kernel(BuildGraph bg, WalkCfg cfg, const uint32_t* __restrict__ ids,
+                                                           uint32_t first, uint32_t b, int is_update, BuildBuffers bb,
+                                                           uint32_t warp_smem) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const GraphView& g = bg.g;
+  const uint32_t w = threadIdx.x >> 5;
+  const uint32_t pi = blockIdx.x * (blockDim.x >> 5) + w;
+  if (pi >= b) return;
+  const uint32_t p = ids ? ids[pi] : first + pi;
+  WarpCtx c;
+  ctx_init(c, smem + (size_t)w * warp_smem + 256, cfg, g.dpad);
+  Aux a = aux_of(c);
+  link_point<LPV, NQ, KPL, HASDEL, UList<KPL>>(c, a, bg, p, is_update, bb);
+}
+
 // The wide form of phase A (efc > kMaxRegEfc): a persistent grid of one-warp blocks; warp w links points w, w + W, ...
 // of the wave, so the scratch depends on the resident warps, not on the wave (up to 16384 points).  The result set is
 // the shared-memory SList of the wide-beam walk (L = align_up(efc, 32) keys, the ordered list beside it: set_init), the
@@ -302,7 +262,7 @@ __global__ void __launch_bounds__(32, 1)
   c.hsize = vsize;
   Aux a = aux_of(c);
   for (uint32_t pi = blockIdx.x; pi < b; pi += gridDim.x)
-    link_point<LPV, NQ, HASDEL>(c, a, bg, ids ? ids[pi] : first + pi, is_update, bb);
+    link_point<LPV, NQ, 0, HASDEL, SList>(c, a, bg, ids ? ids[pi] : first + pi, is_update, bb);
 }
 
 // Adds one id per lane (kInvalid = none; the ids of one call are distinct) to the candidate set cand[0..ncand),
@@ -383,7 +343,7 @@ static __global__ void update_tag_kernel(GraphView g, const uint8_t* __restrict_
   }
 }
 
-// One moved point pi (= ids[pi] in the wave) with the warp's context; u holds the keep list (set_init done).
+// One moved point pi (= ids[pi] in the wave) with the warp's context; u holds the keep list (set_begin done).
 template <int LPV, int NQ, class Set>
 __device__ __forceinline__ void update_point(WarpCtx& c, const Aux& a, Set& u, const BuildGraph& bg, uint32_t pi,
                                              uint32_t p, const BuildBuffers& bb) {
@@ -448,7 +408,7 @@ __global__ void __launch_bounds__(32, 1) update_neighbors_wide_kernel(BuildGraph
   ctx_init(c, smem + 256, cfg, bg.g.dpad);
   Aux a = aux_of(c);
   SList u;
-  set_init(u, c);
+  set_begin(u, c);
   update_point<LPV, NQ>(c, a, u, bg, pi, ids[pi], bb);
 }
 
@@ -512,7 +472,7 @@ __global__ void __launch_bounds__(32, 1) repair_rows_wide_kernel(BuildGraph bg, 
   ctx_init(c, smem + 256, cfg, bg.g.dpad);
   Aux a = aux_of(c);
   SList u;
-  set_init(u, c);
+  set_begin(u, c);
   repair_row<LPV, NQ>(c, a, u, bg, pi, rows[pi], bb);
 }
 

@@ -347,6 +347,11 @@ struct ehb_index {
   // bf16: the walk reads the bf16 shadow (rows of dpad * 2 bytes); screen: a screened fp32 walk (no TMA ring)
   ehb::WalkCfg walk_cfg(uint32_t ef_eff, uint32_t smem_list, uint64_t jobs, uint32_t team, bool bf16 = false,
                         bool dense = false, bool screen = false) const;
+  // The wide-beam geometry, shared by the wide-beam walk (walk_plan) and the wide construction form (build_cfg): a
+  // beam of ef over a shared-memory key list of smem_list keys, no visited table in shared memory (each warp has
+  // beam_vtab_size(ef) entries in HBM) and, with tombstones, a side queue that grows with the beam.
+  ehb::WalkCfg beam_cfg(uint32_t ef, uint32_t smem_list, uint64_t jobs, bool bf16 = false) const;
+  uint32_t beam_vtab_size(uint32_t ef) const { return ehb::align_up(2u * M0 * ef + 64u, 32); }  // walk_cfg's "roomy"
   uint32_t wpb_for(const ehb::WalkCfg& c, uint32_t extra, bool bf16 = false) const;
   // every choice of the graph-walk kernel for a search of nq queries with beam ef_eff (the shadow exists if bf16)
   ehb::WalkPlan walk_plan(uint64_t nq, uint32_t ef_eff, bool bf16) const;

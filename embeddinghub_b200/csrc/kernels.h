@@ -64,6 +64,10 @@ cudaError_t beam_warps(const WalkPlan& p, const GraphView& g, int sms, uint64_t 
 cudaError_t launch_search_beam(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
                                uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                                uint32_t* vtab, uint32_t warps, cudaStream_t s);
+// The resident warps of a persistent grid of one-warp blocks of `kern` with smem bytes of dynamic shared memory each,
+// on sms SMs (sets the kernel's dynamic shared-memory limit to smem; cudaErrorInvalidConfiguration when not even one
+// block fits an SM).
+cudaError_t resident_warps(const void* kern, uint32_t smem, int sms, uint32_t* out);
 template <uint32_t DPAD, class RowT>
 struct BeamShape {
   static cudaError_t warps(const WalkPlan& p, int sms, uint64_t nq, uint32_t* out);

@@ -27,6 +27,16 @@ cudaError_t beam_warps(const WalkPlan& p, const GraphView& g, int sms, uint64_t 
   });
 }
 
+cudaError_t resident_warps(const void* kern, uint32_t smem, int sms, uint32_t* out) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  int per_sm = 0;
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32, smem);
+  if (e != cudaSuccess) return e;
+  if (per_sm < 1) return cudaErrorInvalidConfiguration;
+  *out = (uint32_t)per_sm * (uint32_t)sms;
+  return cudaSuccess;
+}
+
 cudaError_t launch_search_beam(const WalkPlan& p, const GraphView& g, const float* queries, uint32_t nq, uint32_t k,
                                uint32_t ef, const ResultSink& sink, uint32_t* out_counts, uint32_t* stats,
                                uint32_t* vtab, uint32_t warps, cudaStream_t s) {
