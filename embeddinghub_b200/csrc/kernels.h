@@ -41,8 +41,9 @@ struct WalkPlan {
 void walk_kernel_name(const WalkPlan& p, char* out, size_t out_bytes);
 
 // K2 — batched k-NN graph walk (hnswlib searchKnn), one warp per query, plain, dense or wide form.  ef >= k.
-// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, 0, 0.  With g.codes8
-// set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the int8 screen copy (walk.cuh beam_search).
+// stats: [nq][kStatWords] u32 = hops_upper, hops_base, evals, overflow, screened, survivors, screened_upper (those
+// of the upper-layer descent), 0.  With g.codes8 set (metric 1, rows > 1 KB) the fp32 walk screens candidates on the
+// int8 screen copy (walk.cuh greedy_descent, beam_search).
 // With p.bf16 the walk reads the bf16 shadow g.vecs16 (fp32 queries, fp32 accumulation) and writes the retained
 // set, not results: sink.keys[nq][k] gets the (ordered distance, internal id) keys nearest-first (call with k = ef
 // to keep all of them) and out_counts the retained count; launch_rerank then produces the fp32 results.

@@ -161,15 +161,16 @@ cudaError_t launch_to_i8(const float* in, uint32_t dpad, int8_t* codes, float4* 
   return cudaGetLastError();
 }
 
-// per query: hops_upper, hops_base, evals, overflow flag, screened, survivors, 0, 0 -> sums (overflow: queries)
+// per query: hops_upper, hops_base, evals, overflow flag, screened, survivors, screened_upper, 0 -> sums (overflow:
+// queries)
 __global__ void sum_stats_kernel(const uint32_t* __restrict__ stats, uint32_t nq, unsigned long long* out) {
   unsigned long long a[kStatWords] = {};
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += gridDim.x * blockDim.x) {
     const uint4 s = ((const uint4*)stats)[2 * i], t = ((const uint4*)stats)[2 * i + 1];
-    a[0] += s.x, a[1] += s.y, a[2] += s.z, a[3] += s.w ? 1 : 0, a[4] += t.x, a[5] += t.y;
+    a[0] += s.x, a[1] += s.y, a[2] += s.z, a[3] += s.w ? 1 : 0, a[4] += t.x, a[5] += t.y, a[6] += t.z;
   }
 #pragma unroll
-  for (int j = 0; j < 6; ++j) {
+  for (int j = 0; j < 7; ++j) {
     for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(0xffffffffu, a[j], o);
     if ((threadIdx.x & 31) == 0) atomicAdd(&out[j], a[j]);
   }

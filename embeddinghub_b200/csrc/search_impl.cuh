@@ -28,6 +28,9 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
   UList<KPL> ul;
   ul_clear<KPL>(ul, ef, c.lane);
   if (g.n != 0) {
+    QueryPlanes<NQ> qp;  // a screened walk's integer query, for the descent and the base layer
+    if constexpr (kScreen)
+      if (walk_screens(g)) screen_setup<NQ>(c, g, qr, qp);
     uint32_t cur = g.entry;
     if (c.lane == 0) c.cand_id[0] = cur;
     __syncwarp();
@@ -35,8 +38,8 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
     float curdist = c.cand_dist[0];
     __syncwarp();
     wc.evals = 1;
-    greedy_descent<LPV, NQ, UDIV, RowT, kScreen>(c, g, qr, cur, curdist, g.max_level, 0, wc);
-    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV, RowT, kScreen>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc);
+    greedy_descent<LPV, NQ, UDIV, RowT, kScreen>(c, g, qr, cur, curdist, g.max_level, 0, wc, &qp);
+    beam_search<LPV, NQ, KPL, true, HASDEL, UDIV, RowT, kScreen>(c, g, qr, ul, cur, curdist, 0, ef, kInvalid, wc, &qp);
   }
   // nearest-first output: extract the k closest in ascending order into registers (element i -> lane i & 31,
   // slot i >> 5), then store them to every destination of the sink with coalesced stores
@@ -75,7 +78,7 @@ __device__ __forceinline__ void search_body(const GraphView& g, const WalkCfg& c
     if (out_counts) out_counts[q] = found;
     if (stats) {
       ((uint4*)stats)[2 * q] = make_uint4(wc.hops_upper, wc.hops_base, wc.evals, wc.overflow);
-      ((uint4*)stats)[2 * q + 1] = make_uint4(wc.screened, wc.survivors, 0u, 0u);
+      ((uint4*)stats)[2 * q + 1] = make_uint4(wc.screened, wc.survivors, wc.screened_upper, 0u);
     }
   }
 }

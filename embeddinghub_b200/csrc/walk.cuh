@@ -612,13 +612,72 @@ __device__ __forceinline__ void eval_candidates(WarpCtx& c, const RowT* __restri
 // (h in [-64, 64], l in [-64, 63]) in the codes' lane layout.  kQMax keeps every partial sum of K = sum k_i c_i inside
 // int32 at dpad 1536: kQMax * 127 * 1536 < 2^31.
 constexpr int kQMax = 8191;
-// Per-query terms of the screen's bound (beam_search): l1 >= |q|_1, l2 >= |q|_2, a: the walk chain's subnormal term,
+// Per-query terms of the screen's bound (screen_setup): l1 >= |q|_1, l2 >= |q|_2, a: the walk chain's subnormal term,
 // en >= |e|_2 for e = q - sq k, and sq.  They live in shared memory behind the mbarriers: held in registers through
 // the walk, they cost spills.
 struct ScreenQuery {
   float l1, l2, a, en, sq;
 };
 __device__ __forceinline__ ScreenQuery* screen_query(const WarpCtx& c) { return (ScreenQuery*)(c.mbar + 8); }
+// The integer query planes k = 128 h + l, in the codes' lane layout (a u32 of four signed bytes per chunk).
+template <int NQ>
+struct QueryPlanes {
+  uint32_t h[NQ], l[NQ];
+};
+// the walk screens its fp32 candidates (the plan set the int8 copy, which it does only for metric 1 and no ring)
+__device__ __forceinline__ bool walk_screens(const GraphView& g) { return g.codes8 && g.metric == 1; }
+// Once per query, before the upper-layer descent: the integer planes of the query (registers, kept through the whole
+// walk) and its ScreenQuery terms (shared memory).
+template <int NQ>
+__device__ __forceinline__ void screen_setup(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ],
+                                             QueryPlanes<NQ>& qp) {
+  float mx = 0.f, l1 = 0.f, l2 = 0.f;
+#pragma unroll
+  for (int t = 0; t < NQ; ++t) {
+    const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      mx = fmaxf(mx, fabsf(v[j]));
+      l1 = __fadd_ru(l1, fabsf(v[j]));
+      l2 = __fmaf_ru(v[j], v[j], l2);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {  // sums of non-negative terms rounded up: upper bounds
+    l1 = __fadd_ru(l1, __shfl_xor_sync(0xffffffffu, l1, o));
+    l2 = __fadd_ru(l2, __shfl_xor_sync(0xffffffffu, l2, o));
+  }
+  mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
+  // k = RN(q / sq) clamped to +-kQMax, and e = q - sq k, exact in double (sq k has at most 38 significant bits and
+  // lies within 14 binades of q when k != 0).  A zero, tiny or non-finite max |q| gets sq = 0: k = 0 and e = q (a
+  // NaN or infinite element then makes en non-finite, and every candidate is kept).
+  float sq = mx / (float)kQMax;
+  if (!(sq >= 0x1p-126f && sq <= 0x1.fffffep127f)) sq = 0.f;
+  double e2 = 0.0;
+#pragma unroll
+  for (int t = 0; t < NQ; ++t) {
+    const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
+    uint32_t h = 0, l = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = sq != 0.f ? max(-kQMax, min(kQMax, __float2int_rn(v[j] / sq))) : 0;
+      const double e = (double)v[j] - (double)sq * (double)k;
+      e2 = __fma_ru(e, e, e2);
+      const int kh = (k + 64) >> 7;  // floor: k - 128 kh in [-64, 63]
+      h |= (uint32_t)(kh & 0xFF) << (8 * j);
+      l |= (uint32_t)((k - 128 * kh) & 0xFF) << (8 * j);
+    }
+    qp.h[t] = h;
+    qp.l[t] = l;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) e2 = __dadd_ru(e2, __shfl_xor_sync(0xffffffffu, e2, o));
+  // the walk chain's subnormal inputs and products, flushed or not: d (2^-125 max|q| + 2^-124)
+  if (c.lane == 0)
+    *screen_query(c) = {l1, __fsqrt_ru(l2), __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f)),
+                        __double2float_ru(__dsqrt_ru(e2)), sq};
+  __syncwarp();
+}
 // Per candidate of cand_id[0..m) the warp loads the codes straight into registers (RB rows per batch: 96 registers
 // of codes per lane, 32 rows at dpad 384 down to 8 at 1536; loading the next batch during this one's math would
 // double them, and the kernel would spill at its 200-register budget)
@@ -626,13 +685,13 @@ __device__ __forceinline__ ScreenQuery* screen_query(const WarpCtx& c) { return 
 // terms (s, rinf, r2, nx) it forms L = RD(RD(1 - RU(s sq K)) - M'),
 //   M' = RU(gam l2 nx + min(l1 rinf, l2 r2) + en (nx + r2) + a),  gam = dpad 2^-24 / (1 - dpad 2^-24):
 // a lower bound on the distance RN(1 - P^) of the fp32 pass (DESIGN.md §9).  A candidate with f2ord(L) >= worst_hi
-// (the hop-start worst of a full result set, which only shrinks within the hop) cannot be admitted and is dropped;
-// a non-finite L keeps it.  The survivors move to the front of cand_id in their order, and their count is returned.
-// `unsure` (a bit per cand_id position) moves with them.
+// cannot be chosen and is dropped (beam_search: the hop-start worst of a full result set, which only shrinks within
+// the hop; greedy_descent: the current node's distance, which a move must beat); a non-finite L keeps it.  The
+// survivors move to the front of cand_id in their order, and their count is returned.  `unsure` (a bit per cand_id
+// position) moves with them.
 template <int NQ>
-__device__ __forceinline__ uint32_t screen_regs(WarpCtx& c, const GraphView& g, const uint32_t (&qh)[NQ],
-                                                const uint32_t (&ql)[NQ], uint32_t m, uint32_t worst_hi,
-                                                uint32_t& unsure) {
+__device__ __forceinline__ uint32_t screen_regs(WarpCtx& c, const GraphView& g, const QueryPlanes<NQ>& qp, uint32_t m,
+                                                uint32_t worst_hi, uint32_t& unsure) {
   constexpr int RB = 96 / NQ;
   const bool in = c.lane < m;
   const uint32_t id = in ? c.cand_id[c.lane] : kInvalid;
@@ -655,8 +714,8 @@ __device__ __forceinline__ uint32_t screen_regs(WarpCtx& c, const GraphView& g, 
       int h = 0, l = 0;
 #pragma unroll
       for (int t = 0; t < NQ; ++t) {
-        h = __dp4a((int)x[i][t], (int)qh[t], h);
-        l = __dp4a((int)x[i][t], (int)ql[t], l);
+        h = __dp4a((int)x[i][t], (int)qp.h[t], h);
+        l = __dp4a((int)x[i][t], (int)qp.l[t], l);
       }
       const int kv = __reduce_add_sync(0xffffffffu, 128 * h + l);
       if (c.lane == v0 + (uint32_t)i) K = kv;
@@ -970,9 +1029,10 @@ __device__ __forceinline__ uint32_t list_insert(WarpCtx& c, uint64_t key, uint32
 }
 
 // screened: evaluations made on the int8 screen copy first (fp32 screen); survivors: those of them whose fp32 row
-// was then read.  An fp32 walk reads evals - screened + survivors fp32 rows.
+// was then read.  An fp32 walk reads evals - screened + survivors fp32 rows.  screened_upper: the screened evaluations
+// of the upper-layer descent (part of screened).
 struct WalkCounters {
-  uint32_t hops_upper, hops_base, evals, overflow, screened, survivors;
+  uint32_t hops_upper, hops_base, evals, overflow, screened, survivors, screened_upper;
 };
 
 // Adjacency row of `node` at `level` -> one id per lane (kInvalid beyond the row).
@@ -993,10 +1053,15 @@ __device__ __forceinline__ uint32_t load_row(const GraphView& g, uint32_t node, 
 
 // hnswlib searchKnn's upper-layer descent: at each level move to the closest
 // neighbour until no neighbour improves.
+// A screened walk (SCREEN, walk_screens(g); *qp from screen_setup) screens each hop's neighbours on the int8 copy
+// against the current distance first and evaluates only the survivors in fp32.  The descent moves only to a
+// neighbour with d < curdist, and L <= d, so a neighbour with L >= curdist is never chosen; the survivors keep their
+// order, so a tie among them still goes to the earliest position, and the descent takes the same path.
 template <int LPV, int NQ, int UDIV = 1, class RowT = float, bool SCREEN = false>
 __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], uint32_t& cur,
                                                float& curdist, int from_level, int to_level_excl,
-                                               WalkCounters& wc) {
+                                               WalkCounters& wc, const QueryPlanes<NQ>* qp = nullptr) {
+  const bool screen = SCREEN && walk_screens(g);  // warp-uniform
   for (int level = from_level; level > to_level_excl; --level) {
     bool changed = true;
     while (changed) {
@@ -1010,7 +1075,16 @@ __device__ __forceinline__ void greedy_descent(WarpCtx& c, const GraphView& g, c
       if (nb != kInvalid) c.cand_id[__popc(mask & lanemask_lt())] = nb;
       __syncwarp();
       wc.evals += m;
-      eval_candidates<LPV, NQ, UDIV, RowT, SCREEN>(c, walk_rows<RowT>(g), qr, m, g.metric);
+      if (SCREEN && screen) {
+        uint32_t unsure = 0;
+        wc.screened += m;
+        wc.screened_upper += m;
+        m = screen_regs<NQ>(c, g, *qp, m, f2ord(curdist), unsure);
+        wc.survivors += m;
+        eval_regs<NQ>(c, g.vecs, qr, m, 1);
+      } else {
+        eval_candidates<LPV, NQ, UDIV, RowT, SCREEN>(c, walk_rows<RowT>(g), qr, m, g.metric);
+      }
       float bd = c.lane < m ? c.cand_dist[c.lane] : INFINITY;
       uint32_t bl = c.lane;
 #pragma unroll
@@ -1092,58 +1166,9 @@ template <int LPV, int NQ, int KPL, bool PREFETCH, bool HASDEL, int UDIV = 1, cl
           class Set = UList<KPL>>
 __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, const float4 (&qr)[NQ], Set& u,
                                             uint32_t ep, float epdist, int level, uint32_t ef, uint32_t exclude,
-                                            WalkCounters& wc) {
+                                            WalkCounters& wc, const QueryPlanes<NQ>* qp = nullptr) {
   static_assert(!SCREEN || (screen_shape(LPV, NQ) && std::is_same<RowT, float>::value), "no screen for this shape");
-  const bool screen = SCREEN && g.codes8 && g.metric == 1;  // warp-uniform
-  uint32_t qh[NQ], ql[NQ];  // the screen's integer query planes (kQMax)
-  if (screen) {
-    float mx = 0.f, l1 = 0.f, l2 = 0.f;
-#pragma unroll
-    for (int t = 0; t < NQ; ++t) {
-      const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        mx = fmaxf(mx, fabsf(v[j]));
-        l1 = __fadd_ru(l1, fabsf(v[j]));
-        l2 = __fmaf_ru(v[j], v[j], l2);
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {  // sums of non-negative terms rounded up: upper bounds
-      l1 = __fadd_ru(l1, __shfl_xor_sync(0xffffffffu, l1, o));
-      l2 = __fadd_ru(l2, __shfl_xor_sync(0xffffffffu, l2, o));
-    }
-    mx = __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(mx)));  // >= 0: ordered as its bits
-    // k = RN(q / sq) clamped to +-kQMax, and e = q - sq k, exact in double (sq k has at most 38 significant bits and
-    // lies within 14 binades of q when k != 0).  A zero, tiny or non-finite max |q| gets sq = 0: k = 0 and e = q (a
-    // NaN or infinite element then makes en non-finite, and every candidate is kept).
-    float sq = mx / (float)kQMax;
-    if (!(sq >= 0x1p-126f && sq <= 0x1.fffffep127f)) sq = 0.f;
-    double e2 = 0.0;
-#pragma unroll
-    for (int t = 0; t < NQ; ++t) {
-      const float v[4] = {qr[t].x, qr[t].y, qr[t].z, qr[t].w};
-      uint32_t h = 0, l = 0;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int k = sq != 0.f ? max(-kQMax, min(kQMax, __float2int_rn(v[j] / sq))) : 0;
-        const double e = (double)v[j] - (double)sq * (double)k;
-        e2 = __fma_ru(e, e, e2);
-        const int kh = (k + 64) >> 7;  // floor: k - 128 kh in [-64, 63]
-        h |= (uint32_t)(kh & 0xFF) << (8 * j);
-        l |= (uint32_t)((k - 128 * kh) & 0xFF) << (8 * j);
-      }
-      qh[t] = h;
-      ql[t] = l;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) e2 = __dadd_ru(e2, __shfl_xor_sync(0xffffffffu, e2, o));
-    // the walk chain's subnormal inputs and products, flushed or not: d (2^-125 max|q| + 2^-124)
-    if (c.lane == 0)
-      *screen_query(c) = {l1, __fsqrt_ru(l2), __fmul_ru((float)g.dpad, __fmaf_ru(mx, 0x1p-125f, 0x1p-124f)),
-                          __double2float_ru(__dsqrt_ru(e2)), sq};
-    __syncwarp();
-  }
+  const bool screen = SCREEN && walk_screens(g);  // warp-uniform; *qp from screen_setup
   hash_clear(c);
   ul_clear(u, ef, c.lane);
   const uint8_t* __restrict__ del = (HASDEL && c.dcap) ? g.deleted : nullptr;  // warp-uniform
@@ -1188,7 +1213,7 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       wc.evals += m;
       if (SCREEN && screen && cnt >= ef) {
         wc.screened += m;
-        m = screen_regs<NQ>(c, g, qh, ql, m, worst_hi, unsure);
+        m = screen_regs<NQ>(c, g, *qp, m, worst_hi, unsure);
         wc.survivors += m;
         eval_regs<NQ>(c, g.vecs, qr, m, 1);
       } else {
@@ -1208,6 +1233,10 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
       ovf_any = ovf_any || __any_sync(0xffffffffu, ovf);
       uint32_t qual = __ballot_sync(0xffffffffu, c.lane < m && (cnt < ef || myhi < worst_hi));
       const uint32_t delmask = (HASDEL && del) ? __ballot_sync(0xffffffffu, mydel) : 0u;
+      // A screened walk is bound by DRAM bandwidth, and most admitted candidates are evicted before they are
+      // expanded: it pulls a candidate's adjacency row towards L2 only when the candidate is closer than every
+      // unexpanded entry so far this hop, i.e. when it would be the next node expanded (hint only).
+      uint32_t next_hi = (SCREEN && screen) ? ul_min_unexpanded_hi(u) : 0xFFFFFFFFu;
       while (qual) {
         int j = __ffs(qual) - 1;
         qual &= qual - 1;
@@ -1222,7 +1251,10 @@ __device__ __forceinline__ void beam_search(WarpCtx& c, const GraphView& g, cons
         }
         if (ovf_any && ul_contains(u, ij)) continue;
         ul_insert(u, hj, ij, ef, cnt, worst_hi, c.lane);
-        if (PREFETCH && c.lane == 0) prefetch_l2(g.links0 + (size_t)ij * g.M0);
+        if (PREFETCH && (!(SCREEN && screen) || hj < next_hi)) {
+          next_hi = hj;
+          if (c.lane == 0) prefetch_l2(g.links0 + (size_t)ij * g.M0);
+        }
       }
     }
     if (HASDEL && dn) {

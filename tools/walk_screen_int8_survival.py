@@ -12,7 +12,10 @@ the bounds).  Prints one JSON line: evaluations per query, the screened share, e
 the projected algorithmic bytes per query of the row reads (dim bytes + 16 bytes of per-row terms per int8-screened
 evaluation, 2 dim per bf16-screened one, 4 dim per fp32 row read).  It also reports the share of screened hops whose
 next node the int8 bounds prove: spec, the closest unexpanded result before the hop's candidates, is expanded next
-when every int8 survivor has L > dist(spec) (no survivor can then come before it or evict it).
+when every int8 survivor has L > dist(spec) (no survivor can then come before it or evict it).  For the upper-layer
+greedy descent, which the walk screens against the current node's distance, it reports the evaluations per query,
+the share of them that survive the int8 bound (L < current distance) and the hops that move the descent, and the
+projected row bytes per query with the descent read in fp32 and with it screened.
 
   python tools/walk_screen_int8_survival.py [--n 200000] [--dim 768] [--queries 300] [--ef 128] [--threads 8]
 """
@@ -55,10 +58,11 @@ def int8_copy(x):
     return s, c.astype(np.float32), np.abs(r).max(1), np.linalg.norm(r, axis=1), np.linalg.norm(xd, axis=1)
 
 
-def walk(g, x, q, ef, visit):
+def walk(g, x, q, ef, visit, visit_up):
     """hnswlib searchKnn (no deletions) under 1 - dot; visit(worst or None, spec, ids, dists) sees each base-layer
     hop's new candidates with the hop-start worst distance when the result set was full, and the distance of the
-    closest unexpanded result at the hop's start (None when there is none)"""
+    closest unexpanded result at the hop's start (None when there is none); visit_up(cur_dist, ids, dists) sees each
+    upper-layer descent hop's neighbours with the current node's distance"""
     links0, up_off, links_up = g["links0"], g["up_off"], g["links_up"]
     dist = lambda ids: 1.0 - x[ids] @ q
     cur = int(g["entry"])
@@ -71,6 +75,7 @@ def walk(g, x, q, ef, visit):
             ids = row[row != 0xFFFFFFFF]
             if len(ids):
                 ds = dist(ids)
+                visit_up(cd, ids, ds)
                 j = int(np.argmin(ds))
                 if ds[j] < cd:
                     cd, cur, changed = float(ds[j]), int(ids[j]), True
@@ -123,12 +128,22 @@ def main():
     gam = dpad * 2.0 ** -24 / (1 - dpad * 2.0 ** -24)
     cb = bf16_constant(dpad)
     qs = np.random.default_rng(4321).standard_normal((a.queries, d), dtype=np.float32)
-    tot = {"evals": 0, "screened": 0, "bf16_kept": 0, "int8_kept": 0, "admissible": 0, "hops": 0, "proven": 0}
+    tot = {"evals": 0, "screened": 0, "bf16_kept": 0, "int8_kept": 0, "admissible": 0, "hops": 0, "proven": 0,
+           "up_evals": 0, "up_kept": 0, "up_moves": 0}
     margins = {"bf16": [], "int8": []}
     for q in qs:
         qd = q.astype(np.float64)
         q1, q2 = np.abs(qd).sum(), np.linalg.norm(qd)
         A = dpad * (2.0 ** -125 * np.abs(qd).max() + 2.0 ** -124)
+
+        def int8_lower(ids):
+            mi = gam * q2 * (2 * nx[ids] + r2[ids]) + np.minimum(q1 * rinf[ids], q2 * r2[ids]) + A
+            return 1.0 - s[ids] * (c[ids].astype(np.float64) @ qd) - mi, mi
+
+        def visit_up(cd, ids, ds):
+            tot["up_evals"] += len(ids)
+            tot["up_kept"] += int((int8_lower(ids)[0] < cd).sum())
+            tot["up_moves"] += int(ds.min() < cd)
 
         def visit(worst, spec, ids, ds):
             tot["evals"] += len(ids)
@@ -137,8 +152,7 @@ def main():
             tot["screened"] += len(ids)
             mb = cb * (np.abs(b[ids]).astype(np.float64) @ np.abs(qd)) + A
             lb = 1.0 - b[ids].astype(np.float64) @ qd - mb
-            mi = gam * q2 * (2 * nx[ids] + r2[ids]) + np.minimum(q1 * rinf[ids], q2 * r2[ids]) + A
-            li = 1.0 - s[ids] * (c[ids].astype(np.float64) @ qd) - mi
+            li, mi = int8_lower(ids)
             tot["bf16_kept"] += int((lb < worst).sum())
             tot["int8_kept"] += int((li < worst).sum())
             tot["admissible"] += int((ds < worst).sum())
@@ -147,13 +161,17 @@ def main():
             margins["bf16"].append(mb)
             margins["int8"].append(mi)
 
-        walk(g, x, q, a.ef, visit)
+        walk(g, x, q, a.ef, visit, visit_up)
     nq = a.queries
+    ue, uk = tot["up_evals"] / nq, tot["up_kept"] / max(tot["up_evals"], 1)
     ev, sc = tot["evals"] / nq, tot["screened"] / nq
     kb, ki = tot["bf16_kept"] / max(tot["screened"], 1), tot["int8_kept"] / max(tot["screened"], 1)
     unscreened = ev - sc
     bytes_bf16 = unscreened * 4 * d + sc * 2 * d + sc * kb * 4 * d
     bytes_int8 = unscreened * 4 * d + sc * (d + 16) + sc * ki * 4 * d
+    # with the descent's rows: read in fp32, or screened (int8 rows and terms, fp32 rows of the survivors)
+    bytes_descent_fp32 = bytes_int8 + ue * 4 * d
+    bytes_descent_int8 = bytes_int8 + ue * (d + 16) + ue * uk * 4 * d
     print(json.dumps({
         "n": a.n, "dim": d, "dpad": dpad, "queries": nq, "ef": a.ef, "graph_build_s": round(build_s, 1),
         "evals_per_query": round(ev, 1), "screened_share": round(sc / ev, 4),
@@ -165,7 +183,12 @@ def main():
         "fp32_rows_per_eval_int8": round((unscreened + sc * ki) / ev, 4),
         "row_bytes_per_query_bf16": round(bytes_bf16), "row_bytes_per_query_int8": round(bytes_int8),
         "row_bytes_ratio": round(bytes_int8 / bytes_bf16, 4),
-        "int8_proven_next_share": round(tot["proven"] / max(tot["hops"], 1), 4)}))
+        "int8_proven_next_share": round(tot["proven"] / max(tot["hops"], 1), 4),
+        "descent_evals_per_query": round(ue, 1), "descent_int8_survivor_share": round(uk, 4),
+        "descent_moves_per_query": round(tot["up_moves"] / nq, 2),
+        "row_bytes_per_query_with_descent_fp32": round(bytes_descent_fp32),
+        "row_bytes_per_query_with_descent_int8": round(bytes_descent_int8),
+        "descent_screen_bytes_ratio": round(bytes_descent_int8 / bytes_descent_fp32, 4)}))
 
 
 if __name__ == "__main__":
